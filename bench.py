@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""bench.py — PLIP dual-tower inference throughput on B200 (BASELINE.json metric: image-text pairs/s).
+"""bench.py — PLIP dual-tower inference throughput on H100 (BASELINE.json metric: image-text pairs/s).
 
     python bench.py --gpus N --steps K --warmup W                      # this repo's CUDA engine
     python bench.py --impl reference --gpus N --steps K --warmup W     # the reference's own CPU path
     python bench.py --config cfg3|cfg4|cfg5 ...                        # BASELINE.json configs[2..4] as their own lines
+    python bench.py ... --dump-outputs DIR                             # + the last timed step's outputs as DIR/<name>.npy
 
 Default workload ("pairs"): one step per GPU = one pass of the hot path over 1024 synthetic image-text pairs:
 vision tower (224x224, bf16 pixels resident in HBM) + text tower (77-token ids) + L2-normalise + logits_per_image
@@ -31,6 +32,7 @@ import torch
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
+CFG5_GALLERY = 400000             # 400k x 10k fp32 similarity block = 16 GB: fits one 80 GB GPU beside the towers' buffers
 PAIRS = 1024                      # images / captions per step per GPU (BASELINE cfg2/cfg3 micro-batch)
 FLOP_IMG = 8.81762e9              # SURVEY.md §8: dense FLOPs per image (vision tower + projection)
 FLOP_TXT = 5.95954e9              # per 77-token caption
@@ -42,7 +44,7 @@ WORKLOADS = {
     "cfg3": "BASELINE configs[2]: dual tower + logits_per_image, 4096 images x 1024 captions (77 tokens) per step, 1 GPU",
     "cfg4": "BASELINE configs[3]: zero-shot classification, 100000 synthetic uint8 tiles x 64 class prompts, images "
             "batch-sharded over the GPUs, all-gather of the image embeddings",
-    "cfg5": "BASELINE configs[4]: image->text retrieval, 1000000-tile gallery + 10000 text queries, gallery and queries "
+    "cfg5": "BASELINE configs[4]: image->text retrieval, 400000-tile gallery + 10000 text queries, gallery and queries "
             "sharded over the GPUs, all-gather of the query embeddings, full similarity matrix row-sharded",
 }
 
@@ -53,7 +55,8 @@ def _peaks():
         p = json.load(open(path))
         return {"bf16_tflops": p["bf16_tflops"], "bf16_tflops_sustained": p.get("bf16_tflops_sustained", p["bf16_tflops"]),
                 "hbm_gbs": p["hbm_gbs"], "source": "measured (MEASURED_PEAKS.json)"}
-    return {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "hbm_gbs": 3350.0,
+            "source": "NVIDIA H100 SXM data sheet (dense bf16, HBM3; a card allowed 700 W), not measured"}
 
 
 class ClockSampler:
@@ -124,18 +127,18 @@ def config_dict(name: str, ws: int):
     cfg = {"workload": WORKLOADS[name], "name": name, "seq_len": 77, "parallelism": f"dp{ws}"}
     if name == "pairs":
         cfg.update({"pairs_per_step_per_gpu": PAIRS,
-                    "l2_policy": "inputs alternate between 2 resident sets; pixels 308 MB/step > 126 MB L2",
+                    "l2_policy": "inputs alternate between 2 resident sets; pixels 308 MB/step > 50 MB L2",
                     "collective": "all_gather of text embeddings [1024,512] f32 per rank (NCCL)" if ws > 1 else "none"})
     elif name == "cfg3":
         cfg.update({"images_per_step": 4096, "captions_per_step": 1024,
-                    "l2_policy": "4 distinct micro-batches of 1024 images (1.2 GB of pixels) per step > 126 MB L2"})
+                    "l2_policy": "4 distinct micro-batches of 1024 images (1.2 GB of pixels) per step > 50 MB L2"})
     elif name == "cfg4":
         cfg.update({"tiles": 100000, "prompts": 64, "l2_policy": "every tile distinct (15 GB of uint8 tiles in HBM)",
                     "collective": "all_gather of image embeddings [12500,512] f32 per rank (NCCL)" if ws > 1 else "none"})
     elif name == "cfg5":
-        cfg.update({"gallery": 1000000, "queries": 10000,
+        cfg.update({"gallery": CFG5_GALLERY, "queries": 10000,
                     "l2_policy": "gallery tiles drawn cyclically from a resident pool of 8192 distinct uint8 tiles per rank "
-                                 "(1.2 GB >> 126 MB L2; 150 GB of distinct tiles would not fit beside the 40 GB result at N=1)",
+                                 "(1.2 GB >> 50 MB L2; 60 GB of distinct tiles would not fit beside the 16 GB result at N=1)",
                     "collective": "all_gather of query embeddings [10000/N,512] f32 per rank (NCCL)" if ws > 1 else "none"})
     return cfg
 
@@ -258,7 +261,7 @@ def metric_of(name: str):
         return METRIC, "pairs/s"
     if name == "cfg4":
         return "zero-shot classified tiles/sec (224x224 tiles x 64 prompts)", "images/s"
-    return "retrieval gallery tiles/sec (1M gallery x 10k queries, full similarity matrix)", "images/s"
+    return "retrieval gallery tiles/sec (400k gallery x 10k queries, full similarity matrix)", "images/s"
 
 
 # =================================================================================================
@@ -316,7 +319,7 @@ def kernel_bursts(eng, peaks, stream):
         ms = min(bursts)
         tf = 2.0 * M * N * K / ms / 1e9
         hbm = (M * K * 2 + N * K * 2 + (M * N * 10 if epi == 2 else M * N * 2)) / ms / 1e6
-        res.append({"kernel": f"gemm_tcgen05[{name}]", "M": M, "N": N, "K": K, "us": ms * 1e3, "tflops": tf,
+        res.append({"kernel": f"gemm_wgmma[{name}]", "M": M, "N": N, "K": K, "us": ms * 1e3, "tflops": tf,
                     "frac_of_burst_peak": tf / peaks["bf16_tflops"], "GBps": hbm, "frac_of_hbm_peak": hbm / peaks["hbm_gbs"],
                     "us_mean": sum(bursts) / len(bursts) * 1e3})
         del A, W, out, xb, st_out
@@ -349,7 +352,7 @@ def in_step_profile(eng, run_step, peaks, reps=3):
     return out
 
 
-def roofline_from_profile(prof, peaks, traffic_json):
+def roofline_from_profile(prof, peaks):
     """`roofline` = the kernel role with the largest share of the step; `roofline_worst` = the layer kernel furthest
     below its own roofline.  Both timed inside the step -> sustained tensor peak / measured HBM peak."""
     layer = [p for p in prof if p["share_of_step"] > 0.02]
@@ -359,13 +362,7 @@ def roofline_from_profile(prof, peaks, traffic_json):
     worst = min(layer, key=lambda p: p["frac_of_roofline"] or 1.0)
 
     def obj(p):
-        tr = None
-        if traffic_json:
-            key = p["kernel"].split("/", 1)[1]
-            tower = p["kernel"].split("/", 1)[0]
-            ent = traffic_json.get(f"{tower}/{key}") or traffic_json.get(key)
-            if isinstance(ent, dict) and "traffic_mb" in ent:
-                tr = ent["traffic_mb"] * 1e6
+        tr = None   # measured DRAM traffic per launch: no capture on H100
         if p["bound"] == "tensor":
             return {"bound": "tensor", "achieved": p["tflops"], "peak": peaks["bf16_tflops_sustained"], "unit": "TFLOP/s",
                     "frac": p["tflops"] / peaks["bf16_tflops_sustained"], "traffic": tr, "kernel": p["kernel"],
@@ -437,13 +434,18 @@ class Timer:
             dist.barrier()
         torch.cuda.synchronize()
 
-    def timed(self, fn, steps):
-        """barrier + sync, CUDA events on the launch stream around `steps` calls, barrier + sync, MAX over ranks (ms)."""
+    def timed(self, fn, steps, keep_last=False):
+        """barrier + sync, CUDA events on the launch stream around `steps` calls, barrier + sync, MAX over ranks (ms).
+        keep_last: what the last call returned stays in ``self.last`` (--dump-outputs)."""
         self.barrier()
+        self.last = None
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for i in range(steps):
-            fn(i)
+            if keep_last and i == steps - 1:
+                self.last = fn(i)
+            else:
+                fn(i)
         e1.record()
         self.barrier()
         ms = e0.elapsed_time(e1)
@@ -453,6 +455,29 @@ class Timer:
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
             ms = float(t.item())
         return ms
+
+
+DUMP_BUDGET = 60_000_000          # bytes of array data per --dump-outputs directory (64 MB less headroom for headers)
+
+
+def dump_outputs(dirpath, config, arrays):
+    """Write the named outputs of the last timed step as float32 (integers: float64) ``<name>.npy`` (the default
+    workload) or ``<config>_<name>.npy``, so that a comma-separated --config list can share one directory.  An output whose
+    share of DUMP_BUDGET is too small for it is cut down to a fixed, seeded sample of its rows (sorted row order)."""
+    os.makedirs(dirpath, exist_ok=True)
+    share = DUMP_BUDGET // max(1, len(arrays))
+    for name, t in arrays.items():
+        t = t.detach()
+        if t.dim() == 1:
+            t = t[:, None]
+        itemsize = 4 if t.is_floating_point() else 8
+        row_bytes = t[0].numel() * itemsize
+        if t.shape[0] * row_bytes > share:
+            keep = max(1, share // row_bytes)
+            rows = np.sort(np.random.default_rng(0).choice(t.shape[0], size=keep, replace=False))
+            t = t[torch.from_numpy(rows).to(t.device)]
+        a = t.cpu().numpy()
+        np.save(os.path.join(dirpath, (name if config == "pairs" else f"{config}_{name}") + ".npy"), a.astype(np.float32 if itemsize == 4 else np.float64))
 
 
 def run_ours(args):
@@ -499,13 +524,6 @@ def run_ours(args):
     return rc
 
 
-def traffic_json():
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "r2_traffic.json")))
-    except Exception:  # noqa: BLE001
-        return None
-
-
 def emit(ctx, value, unit, metric, ms_per_step, steps, scaling, clocks, e2e, launches, roofline, extra):
     args, ws = ctx["args"], ctx["ws"]
     line = {"metric": metric, "value": value, "unit": unit, "n_gpus": ws, "steps": steps, "warmup": args.warmup,
@@ -520,7 +538,7 @@ def bench_pairs(ctx):
     from plip_b200 import synthetic as synth
     args, rank, ws, dev, peaks = ctx["args"], ctx["rank"], ctx["ws"], ctx["dev"], ctx["peaks"]
     model, eng, sh, L, timer = ctx["model"], ctx["eng"], ctx["sh"], ctx["L"], ctx["timer"]
-    nsets = 2    # 2 alternating resident input sets (616 MB of pixels >> 126 MB L2)
+    nsets = 2    # 2 alternating resident input sets (616 MB of pixels >> 50 MB L2)
     px = [synth.pixel_values(PAIRS, seed=1234 + 17 * rank + i).to(torch.bfloat16).to(dev) for i in range(nsets)]
     ids = [synth.token_ids(PAIRS, seed=1235 + 17 * rank + i, full_length=True)[0].to(dev) for i in range(nsets)]
 
@@ -533,8 +551,11 @@ def bench_pairs(ctx):
     timer.barrier()
     launches0 = L.plip_launch_count()
     t_wall0 = time.time()
-    ms = timer.timed(step, args.steps)
+    ms = timer.timed(step, args.steps, keep_last=bool(args.dump_outputs))
     t_wall1 = time.time()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, "pairs", {"logits_per_image": timer.last})
+    timer.last = None
     launches = L.plip_launch_count() - launches0
     clocks = sampler.stop(t_wall0, t_wall1) if sampler else None
     ms_per_step = ms / args.steps
@@ -596,7 +617,7 @@ def bench_pairs(ctx):
             torch.cuda.synchronize()
         return 0
     prof = in_step_profile(eng, lambda: step(0), peaks)
-    roof, roof_worst = roofline_from_profile(prof, peaks, traffic_json())
+    roof, roof_worst = roofline_from_profile(prof, peaks)
     extra = {
         "step_tflops": (PAIRS * (FLOP_IMG + FLOP_TXT) + 2.0 * PAIRS * PAIRS * ws * 512) / (ms_per_step / 1e3) / 1e12,
         "roofline_worst": roof_worst,
@@ -713,8 +734,11 @@ def bench_cfg3(ctx):
         step(i)
     launches0 = L.plip_launch_count()
     t0 = time.time()
-    ms = timer.timed(step, args.steps)
+    ms = timer.timed(step, args.steps, keep_last=bool(args.dump_outputs))
     t1 = time.time()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, "cfg3", {"logits_per_image": timer.last})
+    timer.last = None
     launches = L.plip_launch_count() - launches0
     clocks = sampler.stop(t0, t1) if sampler else None
     tiles_h = torch.from_numpy(synth.tiles_u8(n_img, seed=100)).pin_memory()
@@ -732,7 +756,7 @@ def bench_cfg3(ctx):
         return 0
     flop = n_img * FLOP_IMG + n_txt * FLOP_TXT + 2.0 * n_img * n_txt * 512
     prof = in_step_profile(eng, lambda: step(0), peaks, reps=2)
-    roof, roof_worst = roofline_from_profile(prof, peaks, traffic_json())
+    roof, roof_worst = roofline_from_profile(prof, peaks)
     e2e = {"value": n_img * args.steps / (ms_e2e / 1e3), "unit": "pairs/s", "h2d_bytes_per_step": n_img * 150528 + n_txt * 77 * 8,
            "d2h_bytes_per_step": n_img * n_txt * 4, "ms_per_step": ms_e2e / args.steps,
            "path": "PlipCLIPModel.__call__ on pinned host uint8 tiles [4096,224,224,3] + int64 ids [1024,77] -> logits_per_image "
@@ -773,8 +797,12 @@ def bench_cfg4(ctx):
         step(i)
     launches0 = L.plip_launch_count()
     t0 = time.time()
-    ms = timer.timed(step, args.steps)
+    ms = timer.timed(step, args.steps, keep_last=bool(args.dump_outputs))
     t1 = time.time()
+    if args.dump_outputs and rank == 0:
+        pred, logits, all_img = timer.last
+        dump_outputs(args.dump_outputs, "cfg4", {"pred": pred, "logits": logits, "image_embeds": all_img})
+    timer.last = None
     launches = L.plip_launch_count() - launches0
     clocks = sampler.stop(t0, t1) if sampler else None
     # e2e: the same flow fed from a pinned host ring of 2 x 1024 tiles, H2D of every micro-batch inside the timed region
@@ -812,7 +840,7 @@ def bench_cfg5(ctx):
     from plip_b200 import distributed as D, synthetic as synth
     args, rank, ws, dev, peaks = ctx["args"], ctx["rank"], ctx["ws"], ctx["dev"], ctx["peaks"]
     eng, sh, L, timer = ctx["eng"], ctx["sh"], ctx["L"], ctx["timer"]
-    n_gal = args.tiles or 1000000
+    n_gal = args.tiles or CFG5_GALLERY
     n_q = args.queries or 10000
     lo, hi = D.shard_range(n_gal, rank, ws)
     n_local = hi - lo
@@ -839,8 +867,11 @@ def bench_cfg5(ctx):
         step(i)
     launches0 = L.plip_launch_count()
     t0 = time.time()
-    ms = timer.timed(step, args.steps)
+    ms = timer.timed(step, args.steps, keep_last=bool(args.dump_outputs))
     t1 = time.time()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, "cfg5", {"similarity_block": timer.last, "gallery_embeds": state["gal"], "query_embeds": state["q_all"]})
+    timer.last = None
     launches = L.plip_launch_count() - launches0
     clocks = sampler.stop(t0, t1) if sampler else None
     # the similarity block and the fused top-k head alone
@@ -895,17 +926,23 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", default="pairs", help="pairs (default) | cfg3 | cfg4 | cfg5, or a comma-separated list")
-    ap.add_argument("--tiles", type=int, default=0, help="cfg4 / cfg5: override the total tile count (default 100k / 1M)")
+    ap.add_argument("--tiles", type=int, default=0, help="cfg4 / cfg5: override the total tile count (default 100k / 400k)")
     ap.add_argument("--queries", type=int, default=0, help="cfg5: override the query count (default 10k)")
     ap.add_argument("--operands", default="bf16", choices=["bf16", "fp16"],
                     help="16-bit format of the GEMM / attention operands (default bf16 = BASELINE.json's dtype)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-context", action="store_true", help="skip the stock-PyTorch-on-GPU context measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned as DIR/<name>.npy (float32 / float64, "
+                         "at most 64 MB per config: larger outputs as a fixed seeded sample of rows); the inputs are seeded, so two "
+                         "builds can be compared output for output")
     ap.add_argument("--quick", action="store_true", help="skip the extras (kernels alone, product-API extras, context)")
     args = ap.parse_args()
     for c in args.config.split(","):
         if c not in WORKLOADS:
             ap.error(f"unknown config {c!r}")
+    if args.impl == "reference" and args.dump_outputs:
+        ap.error("--dump-outputs belongs to the GPU arm (the reference arm times a bounded sample of the workload)")
     if args.impl == "reference":
         args.config = args.config.split(",")[0]
         if args.steps is None:

@@ -1,7 +1,7 @@
 /*
- * plip_b200 — C ABI of the B200-native PLIP (CLIP ViT-B/32) inference engine.
+ * plip_b200 — C ABI of the H100-native PLIP (CLIP ViT-B/32) inference engine.
  *
- * One shared library (libplip_b200.so, nvcc -gencode arch=compute_100a,code=sm_100a) exports
+ * One shared library (libplip_b200.so, nvcc -gencode arch=compute_90a,code=sm_90a) exports
  * exactly the entry points below.  Plain pointers and sizes only: no torch / python types.
  *
  * The reference (PathologyFoundation/plip) has no FFI of its own — its hot path is the Python
@@ -53,9 +53,9 @@ enum plip_pixel_format {
 enum plip_id_dtype { PLIP_IDS_I32 = 0, PLIP_IDS_I64 = 1 };
 
 /* 16-bit format of every GEMM / attention OPERAND (packed weights, activations between kernels).  Accumulation, the
- * residual stream, LayerNorm statistics, softmax and the similarity head are float32 in both.  tcgen05 kind::f16
+ * residual stream, LayerNorm statistics, softmax and the similarity head are float32 in both.  wgmma
  * runs both at the same rate.  BF16 is the default (BASELINE.json's dtype).  FP16 keeps 3 more significand bits:
- * end-to-end |dlogits_per_image| is 6-8x smaller (profiles/r2_precision_study.md) — the reference's own OpenAI-clip
+ * end-to-end |dlogits_per_image| is 6-8x smaller (tools/precision_study.py) — the reference's own OpenAI-clip
  * flavour runs fp16 weights on the GPU (scripts/extract_embedding.py:94-97) — at the price of a 65504 range. */
 enum plip_operand_format { PLIP_OPERAND_BF16 = 0, PLIP_OPERAND_FP16 = 1 };
 
@@ -214,9 +214,10 @@ PLIP_API int plip_profile_read(plip_engine_t* e, plip_kernel_time_t* out, int ca
 PLIP_API int plip_dbg_set_operand_format(int operand_format);
 /* epilogue: 0 bias->bf16, 1 bias+QuickGELU->bf16, 2 x_f32 += acc+bias (optionally also xb_out bf16 copy +
  * stats_out [M,8,2] row statistics), 3 patch scatter + pos, 4 plain f32, 5/6 = 0/1 with the LayerNorm fold
- * (colsum [N], stats_in [M,8,2] with n_partials valid slots). */
+ * (colsum [N], stats_in [M,8,2] with n_partials valid slots).  cluster_size: 0 = auto, 1 / 2 = CTAs per cluster (2 = the
+ * pair shares the W tile through TMA multicast); block_n: 0 = auto, 128 / 192 / 256 = N tile. */
 PLIP_API int plip_dbg_gemm(const void* A_bf16, int lda, const void* W_bf16, int ldw, int M, int N, int K,
-                           const float* bias, void* out, int ldo, const float* pos, int epilogue, int cta_group,
+                           const float* bias, void* out, int ldo, const float* pos, int epilogue, int cluster_size,
                            int block_n, const float* colsum, const float* stats_in, int n_partials, void* xb_out,
                            float* stats_out, void* stream);
 /* Host-only: fixed-point filter row of output index xx for one axis of plip_resize_crop_u8 (the same code the

@@ -1,6 +1,6 @@
-"""plip_b200 — B200-native PLIP (CLIP ViT-B/32) inference engine.
+"""plip_b200 — H100-native PLIP (CLIP ViT-B/32) inference engine.
 
-Python host code over a hand-written sm_100a CUDA library (``libplip_b200.so``, C ABI in
+Python host code over a hand-written sm_90a CUDA library (``libplip_b200.so``, C ABI in
 ``include/plip_b200.h``).  Public surface mirrors the reference:
 
 * :class:`plip_b200.plip.PLIP` — drop-in for ``plip.PLIP`` (encode_images / encode_text / zero-shot / retrieval)

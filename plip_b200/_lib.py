@@ -105,7 +105,7 @@ def lib(strict: bool = True) -> C.CDLL:
     if not LIB_PATH.exists():
         raise RuntimeError(
             f"{LIB_PATH} is missing: build it with `python -m plip_b200.build` "
-            "(plip_b200 has no CPU fallback; the sm_100a CUDA library is the product)."
+            "(plip_b200 has no CPU fallback; the sm_90a CUDA library is the product)."
         )
     dll = C.CDLL(str(LIB_PATH))
     missing = []

@@ -1,4 +1,4 @@
-"""Build the C-ABI CUDA library (``libplip_b200.so``) in-tree with nvcc for sm_100a.
+"""Build the C-ABI CUDA library (``libplip_b200.so``) in-tree with nvcc for sm_90a.
 
 Usage: ``python -m plip_b200.build [--force] [--verbose]``.  The library has no torch / python
 dependency; it is loaded with ctypes (``plip_b200._lib``).  Objects are compiled in parallel and
@@ -20,8 +20,10 @@ OBJ_DIR = CSRC / "_build"
 LIB_PATH = PKG_DIR / "libplip_b200.so"
 INCLUDE = PKG_DIR.parent / "include"
 
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *GENCODE,
     "-O3", "-std=c++17", "-lineinfo",
     "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC",
@@ -30,7 +32,7 @@ NVCC_FLAGS = [
 ]
 
 
-NVCC_FLAGS += os.environ.get("PLIP_EXTRA_NVCC_FLAGS", "").split()   # e.g. -DPLIP_NO_RPF for an A/B build
+NVCC_FLAGS += os.environ.get("PLIP_EXTRA_NVCC_FLAGS", "").split()   # extra defines for an A/B build
 
 
 def _nvcc() -> str:
@@ -86,7 +88,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     stamp = OBJ_DIR / "link.stamp"
     want = " ".join(o.name for o in objs)
     if force or not LIB_PATH.exists() or not stamp.exists() or stamp.read_text() != want:
-        cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a",
+        cmd = [_nvcc(), "-shared", *GENCODE,
                "-o", str(LIB_PATH), *map(str, objs), "-cudart", "static", "-lpthread", "-ldl", "-lrt"]
         res = subprocess.run(cmd, capture_output=True, text=True)
         if res.returncode != 0:

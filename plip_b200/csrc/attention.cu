@@ -1,4 +1,4 @@
-// plip_b200 — fused attention core on tcgen05: S = Q K^T -> masked softmax -> O = P V, one kernel.
+// plip_b200 — fused attention core on wgmma: S = Q K^T -> masked softmax -> O = P V, one kernel.
 //
 // Replaces F.scaled_dot_product_attention / eager_attention_forward for the CLIP towers
 // (TF:integrations/sdpa_attention.py:92-101, TF:modeling_clip.py:261-279): per (sequence, head)
@@ -6,32 +6,29 @@
 // vision S = 50 without mask, text S <= 77 with the causal (+ key padding) mask (TF:546-557).
 // The dh^-0.5 = 0.125 scale is folded into the q rows of the packed QKV weights (exact: power of 2).
 //
-// Sequences are short, so G = 128 / slot sequences of one head share a 128-row UMMA tile, slot = 32 / 64 / 128 rows
+// Sequences are short, so G = 128 / slot sequences of one head share a 128-row tile, slot = 32 / 64 / 128 rows
 // (the power of two >= S), and attention between different sequences is masked out (block-diagonal: exact):
 //   TMA      per sequence a [slot x 64] box of the Q, K, V head slices of the QKV activation -> smem (128B swizzle)
-//   MMA 1    S[128x128] (TMEM, fp32) = Q (smem, K-major) x K^T (smem, K-major)         4 x UMMA 128x128x16
-//   softmax  thread == query row, a warp == one sequence: tcgen05.ld only that sequence's chunks, mask, max, exp2,
-//            row sum; P (16-bit) -> TMEM via tcgen05.st
-//   MMA 2    O[128x64] (TMEM, fp32) = P (TMEM, A operand) x V (smem, MN-major)          8 x UMMA 128x64x16
-//   epilogue tcgen05.ld O, multiply by 1/rowsum, 16-bit -> V buffer -> one TMA bulk store per sequence
-// 5 warps: warps 0-3 = softmax/epilogue (one TMEM lane quarter each), warp 4 = TMA + MMA issuer.
-// TMEM: 128 columns per CTA — P (16-bit pairs, 64 cols) is written in place over the S columns a thread
-// has already consumed, O (64 cols) reuses the upper half of S.  With single Q/K and V smem buffers
-// (48 KB; the next tile's Q,K are fetched as soon as MMA 1 retires, its V once the output store has read the buffer)
-// four CTAs co-reside per SM and hide each other's serial load -> MMA -> softmax -> MMA -> store chain.
+//   MMA 1    each of the two warpgroups owns 64 query rows: S[64 x NK] (registers, fp32) = Q (smem) x K^T (smem),
+//            NK = 64 keys (the 64-key half that holds the rows' own sequences) when slot <= 64, else all 128
+//   softmax  on the accumulator registers: mask, row max / sum over the 4 lanes of a row, exp2; the 16-bit P values
+//            are already laid out as the A fragments of MMA 2
+//   MMA 2    O[64 x 64] (registers, fp32) = P (registers) x V (smem, MN-major)
+//   epilogue O / rowsum -> 16 bit -> the warpgroup's own Q rows (free once MMA 1 retired) -> one TMA bulk store per
+//            sequence
+// One CTA runs this chain serially per tile; with 48 KB of operands several CTAs co-reside per SM and hide each
+// other's load -> MMA -> softmax -> MMA -> store latency.
 #include "kernels.cuh"
+#include "wgmma.cuh"
 
 namespace plip {
 
 namespace {
 
-constexpr int kAttThreads = 160;
+constexpr int kAttThreads = 256;
 constexpr uint32_t kTileBytes = 128 * 64 * 2;  // one [128 x 64] bf16 operand tile
 constexpr uint32_t kStageBytes = 3 * kTileBytes;
-constexpr uint32_t kAttSmem = kStageBytes + 1024 + 256;
-constexpr uint32_t kTmemCols = 128;
-constexpr uint32_t kColS = 0, kColP = 0, kColO = 64;
-constexpr int kAttCtasPerSm = 4;
+constexpr uint32_t kAttSmem = kStageBytes + 1024 + 64;
 
 // 2^x, flush-to-zero, no range fix-ups: one MUFU op (inputs are <= 0 here, -inf -> +0).
 __device__ __forceinline__ float fast_exp2(float x) {
@@ -40,24 +37,7 @@ __device__ __forceinline__ float fast_exp2(float x) {
   return y;
 }
 
-// =====================================================================================================
-// Round-2 design notes.  ncu on the round-1 kernel (one 128-row tile = floor(128 / S) sequences back to back, two-pass
-// softmax over all four chunks, row stores): ALU pipe 33 %, DRAM 42 %, tensor 16 % — it was bound by the INSTRUCTION
-// COUNT of the softmax (per-element bit tests in two passes over up to four 32-column chunks, most of them
-// belonging to the other sequence of the tile) and by 32-line-per-instruction row stores.  Changes:
-//   * slot layout: a tile holds G = 128 / slot sequences, slot = 32 / 64 / 128 rows (the power of two >= S), each
-//     loaded with its own TMA box [slot x 64] (the rows past S are the next sequence's data or zero fill: finite,
-//     masked).  A softmax warp (32 rows) then belongs to ONE sequence and touches only that sequence's
-//     ceil(S/32) column chunks — vision (S = 50): 2 chunks per warp instead of 2-4, text (S = 77): 1-3;
-//   * one pass when a warp needs <= 2 chunks: S stays in registers between max and exp (one TMEM read, no re-mask);
-//     masks are per-lane bit sets built once per kernel (only a key-padding mask refreshes them per tile) and
-//     chunks that are fully visible take a mask-free path;
-//   * the output tile is staged (bf16, 128B-swizzled) in the V buffer, which is free once P.V has retired, and
-//     leaves with one TMA bulk store per sequence (box [S x 64]) instead of 8 x 32-line STG.128 per warp; the
-//     next tile's V load waits for that store to have read the buffer (bar_vfree).
-// =====================================================================================================
 struct AttParams {
-  int64_t total_rows;   // n_seq * seq_len
   int64_t n_seq;
   int seq_len;          // S
   int slot;             // rows reserved per sequence inside a tile: 32, 64 or 128
@@ -68,282 +48,184 @@ struct AttParams {
   const int32_t* key_mask;  // [n_seq, S] or nullptr
 };
 
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&v)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(v[0]),
-               "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st16_zero(uint32_t taddr) {
-  const uint32_t z = 0u;
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1};" ::"r"(taddr),
-               "r"(z)
-               : "memory");
+template <bool F16, int NK>
+__device__ __forceinline__ void wgmma_qk(float (&s)[NK / 2], uint64_t qdesc, uint64_t kdesc, uint32_t scale_d) {
+  if constexpr (NK == 64) wgmma_ss_n64<F16>(s, qdesc, kdesc, scale_d);
+  else wgmma_ss_n128<F16>(s, qdesc, kdesc, scale_d);
 }
 
-// exp2 of one 32-column chunk held in registers (masked entries are -inf -> 0), accumulate the row sum, write P (bf16)
-template <bool F16>
-__device__ __forceinline__ void softmax_chunk_to_p(const uint32_t (&v)[32], float mx_s, float2& sum2, uint32_t p_taddr) {
-  constexpr float kLog2e = 1.4426950408889634f;
-#pragma unroll
-  for (int hv = 0; hv < 2; ++hv) {
-    uint32_t pk[8];
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      // (a packed FFMA2 / FADD2 version of this loop costs 70 more registers than the 96 available at 4 CTAs per SM)
-      const float e0 = fast_exp2(fmaf(__uint_as_float(v[16 * hv + 2 * c]), kLog2e, -mx_s));
-      const float e1 = fast_exp2(fmaf(__uint_as_float(v[16 * hv + 2 * c + 1]), kLog2e, -mx_s));
-      sum2.x += e0;
-      sum2.y += e1;
-      pk[c] = pack_op2<F16>(e0, e1);
-    }
-    tmem_st8(p_taddr + 8 * hv, pk);
-  }
-}
-
-// masked entries -> -inf (skipped when the whole warp sees every column of the chunk)
-__device__ __forceinline__ void apply_mask(uint32_t (&v)[32], uint32_t vm) {
-  if (!__all_sync(0xffffffffu, vm == 0xffffffffu)) {
-#pragma unroll
-    for (int c = 0; c < 32; ++c)
-      if (!((vm >> c) & 1u)) v[c] = 0xff800000u;  // -inf
-  }
-}
-__device__ __forceinline__ float chunk_max(const uint32_t (&v)[32], float mx) {
-#pragma unroll
-  for (int c = 0; c < 32; c += 2) mx = fmaxf(mx, fmaxf(__uint_as_float(v[c]), __uint_as_float(v[c + 1])));
-  return mx;
-}
-
-template <bool F16>
-__global__ void __launch_bounds__(kAttThreads, kAttCtasPerSm)
+template <bool F16, int NK>
+__global__ void __launch_bounds__(kAttThreads, NK == 64 ? 3 : 2)
 attention_kernel(const __grid_constant__ CUtensorMap tmLoad, const __grid_constant__ CUtensorMap tmStore,
                  const AttParams p) {
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_raw_u32 = smem_u32(smem_raw);
-  const uint32_t smem_base = (smem_raw_u32 + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + kStageBytes;
-  const uint32_t bar_qk = bar_base, bar_v = bar_base + 8;
-  const uint32_t bar_s = bar_base + 16, bar_p = bar_base + 24, bar_o = bar_base + 32, bar_e = bar_base + 40;
-  const uint32_t bar_vfree = bar_base + 48;
-  const uint32_t tmem_slot = bar_base + 56;
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t bar = smem_base + kStageBytes;
   const uint32_t sq = smem_base, sk = smem_base + kTileBytes, sv = smem_base + 2 * kTileBytes;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int hf = warp >> 2;                       // warpgroup == 64-row half of the tile
   const int D = p.heads * kHeadDim;
   const int S = p.seq_len, G = p.group, slot = p.slot;
 
-  if (warp == 4 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmLoad);
     tma_prefetch_desc(&tmStore);
-    mbar_init(bar_qk, 1);
-    mbar_init(bar_v, 1);
-    mbar_init(bar_s, 1);
-    mbar_init(bar_p, 128);
-    mbar_init(bar_o, 1);
-    mbar_init(bar_e, 128);
-    mbar_init(bar_vfree, 1);
+    mbar_init(bar, 1);
     fence_mbar_init();
   }
-  if (warp == 0) tmem_alloc<1>(tmem_slot, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base =
-      *reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_raw_u32));
 
-  const int64_t num_tiles = p.seq_tiles * p.heads;
-
-  if (warp == 4) {
-    // ===================== TMA producer + MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = make_idesc_op(128, 128, 0, 0, F16);  // S = Q K^T, both K-major
-      constexpr uint32_t idesc_o = make_idesc_op(128, 64, 0, 1, F16);   // O = P V, V is MN-major
-      const uint32_t slot_bytes = static_cast<uint32_t>(slot) * 128u;
-      auto issue_qk = [&](int64_t tile) {
-        const int64_t st = tile / p.heads;
-        const int h = (int)(tile - st * p.heads);
-        mbar_arrive_expect_tx(bar_qk, 2 * kTileBytes);
-        for (int g = 0; g < G; ++g) {
-          const int32_t row = (int32_t)((st * G + g) * S);  // past the last sequence: zero fill
-          tma_load_2d(sq + g * slot_bytes, &tmLoad, bar_qk, h * kHeadDim, row);
-          tma_load_2d(sk + g * slot_bytes, &tmLoad, bar_qk, D + h * kHeadDim, row);
-        }
-      };
-      auto issue_v = [&](int64_t tile) {
-        const int64_t st = tile / p.heads;
-        const int h = (int)(tile - st * p.heads);
-        mbar_arrive_expect_tx(bar_v, kTileBytes);
-        for (int g = 0; g < G; ++g)
-          tma_load_2d(sv + g * slot_bytes, &tmLoad, bar_v, 2 * D + h * kHeadDim, (int32_t)((st * G + g) * S));
-      };
-      int64_t tile = blockIdx.x;
-      if (tile < num_tiles) { issue_qk(tile); issue_v(tile); }
-      uint32_t it = 0;
-      const uint64_t qdesc = make_smem_desc_sw128(sq, 1024, 16);
-      const uint64_t kdesc = make_smem_desc_sw128(sk, 1024, 16);
-      for (; tile < num_tiles; tile += gridDim.x, ++it) {
-        const uint32_t par = it & 1u;
-        const int64_t next = tile + gridDim.x;
-        mbar_wait(bar_qk, par);
-        if (it > 0) mbar_wait(bar_e, par ^ 1u);  // previous tile's O (aliases S) has been read out
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_ss<1>(tmem_base + kColS, qdesc + 2 * k, kdesc + 2 * k, idesc_s, k != 0 ? 1u : 0u);
-        umma_commit<1>(bar_s);
-        if (it > 0) {                            // the previous tile's output store has read the V buffer
-          mbar_wait(bar_vfree, par ^ 1u);
-          issue_v(tile);
-        }
-        mbar_wait(bar_s, par);                   // MMA 1 retired: Q/K buffers are free
-        if (next < num_tiles) issue_qk(next);
-        mbar_wait(bar_p, par);                   // softmax warps published P in TMEM
-        mbar_wait(bar_v, par);
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          // V tile [128 keys][64 dh]: advancing 16 keys (one UMMA K) = 16 rows of 128 B
-          const uint64_t vdesc = make_smem_desc_sw128(sv + k * 2048, 1024, 1024);
-          umma_ts(tmem_base + kColO, tmem_base + kColP + k * 8, vdesc, idesc_o, k != 0 ? 1u : 0u);
-        }
-        umma_commit<1>(bar_o);
-      }
+  const int ntiles = (int)(p.seq_tiles * p.heads);
+  const uint32_t slot_bytes = static_cast<uint32_t>(slot) * 128u;
+  auto issue_loads = [&](int tile) {
+    const int64_t st = tile / p.heads;
+    const int h = (int)(tile - st * p.heads);
+    mbar_arrive_expect_tx(bar, 3 * kTileBytes);
+    for (int g = 0; g < G; ++g) {
+      const int32_t row = (int32_t)((st * G + g) * S);  // past the last sequence: zero fill
+      tma_load_2d(sq + g * slot_bytes, &tmLoad, bar, h * kHeadDim, row);
+      tma_load_2d(sk + g * slot_bytes, &tmLoad, bar, D + h * kHeadDim, row);
+      tma_load_2d(sv + g * slot_bytes, &tmLoad, bar, 2 * D + h * kHeadDim, row);
     }
-  } else {
-    // ===================== softmax + epilogue (thread == tile row) =====================
-    const int r = threadIdx.x;                    // 0..127 == TMEM lane == tile row
-    const int g = (warp * 32) / slot;             // the sequence slot this WARP belongs to
-    const int r_in = r - g * slot;                // row inside the sequence
-    const int w_in = (warp * 32 - g * slot) >> 5; // 32-row block of this warp inside its slot
-    const int ct0 = (g * slot) >> 5;              // first 32-column chunk of the slot inside the tile
-    int nch = (S + 31) >> 5;                      // chunks the sequence occupies
-    if (p.causal) nch = min(nch, w_in + 1);       // causal: nothing right of the warp's own diagonal chunk
-    if (w_in * 32 >= S) nch = 0;                  // the whole warp is padding
-    // per-lane visibility bit sets of the slot's chunks (static per thread: sequence end + causal diagonal)
-    uint32_t sm[4];
+  };
+  if (threadIdx.x == 0 && (int)blockIdx.x < ntiles) issue_loads(blockIdx.x);
+
+  // this thread's two tile rows, their sequence slot, and the keys its accumulator columns stand for
+  const int q4 = lane & 3, rr = lane >> 2;
+  const int R0 = 64 * hf + 16 * (warp & 3) + rr;  // second row: R0 + 8 (same sequence: slots are multiples of 32)
+  const int g = R0 / slot;
+  const int r_in0 = R0 - g * slot, r_in1 = r_in0 + 8;
+  const int kbase = (NK == 64) ? 64 * hf : 0;     // first key of the tile this warpgroup multiplies with
+  const int k_in_base = kbase - g * slot + 2 * q4; // + 8 j + e = index inside the sequence of column (j, e)
+  const int lim0 = r_in0 < S ? (p.causal ? r_in0 : S - 1) : -1;   // last visible key of each row
+  const int lim1 = r_in1 < S ? (p.causal ? r_in1 : S - 1) : -1;
+  constexpr float kLog2e = 1.4426950408889634f;
+
+  uint32_t it = 0;
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
+    const int st = tile / p.heads;
+    const int h = tile - st * p.heads;
+    const int64_t seq = (int64_t)st * G + g;
+
+    // keys of the sequence that exist (and are not padding): one bit per accumulator column of this thread
+    uint32_t kv = 0;
 #pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      const int hi = min(min(S, p.causal ? r_in + 1 : S) - 32 * c, 32);
-      sm[c] = (r_in < S && hi > 0) ? (hi >= 32 ? 0xffffffffu : ((1u << hi) - 1u)) : 0u;
+    for (int c = 0; c < NK / 4; ++c) {
+      const int k_in = k_in_base + 8 * (c >> 1) + (c & 1);
+      bool ok = k_in >= 0 && k_in < S;
+      if (ok && p.key_mask != nullptr) ok = seq < p.n_seq && p.key_mask[seq * S + k_in] != 0;
+      kv |= (ok ? 1u : 0u) << c;
     }
-    const uint32_t lane_base = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
-    constexpr float kLog2e = 1.4426950408889634f;
 
-    uint32_t it = 0;
-    const int ntiles = (int)num_tiles;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int st = tile / p.heads;
-      const int h = tile - st * p.heads;
-      const int64_t seq = (int64_t)st * G + g;
+    mbar_wait(bar, it & 1u);
 
-      // visibility bits of slot chunk c for this lane's row: static part & (rarely) the key-padding mask of the tile
-      auto vis = [&](int c) -> uint32_t {
-        uint32_t m = c == 0 ? sm[0] : (c == 1 ? sm[1] : (c == 2 ? sm[2] : sm[3]));
-        if (p.key_mask != nullptr) {
-          const int j = 32 * c + lane;
-          const bool kv = (j < S) && (seq < p.n_seq) && (p.key_mask[seq * S + j] != 0);
-          m &= __ballot_sync(0xffffffffu, kv);
-        }
-        return m;
-      };
-
-      mbar_wait(bar_s, it & 1u);
-      tc_fence_after();
-
-      // The LAST chunk a warp needs is the only one that can be partially visible without a key-padding mask
-      // (sequence end / causal diagonal): it is masked once and kept in registers.  Earlier chunks are read twice
-      // (max, then exp) — a TMEM load costs no ALU work, and they are mask-free unless padded keys exist.
-      float2 sum2 = make_float2(0.f, 0.f);
-      float mx = -INFINITY;
-#pragma unroll 1
-      for (int c = 0; c + 1 < nch; ++c) {
-        uint32_t v[32];
-        tmem_ld32(lane_base + kColS + 32 * (ct0 + c), v);
-        tmem_ld_wait();
-        apply_mask(v, vis(c));
-        mx = chunk_max(v, mx);
-      }
-      uint32_t last[32];
-      if (nch >= 1) {
-        tmem_ld32(lane_base + kColS + 32 * (ct0 + nch - 1), last);
-        tmem_ld_wait();
-        apply_mask(last, vis(nch - 1));
-        mx = chunk_max(last, mx);
-      }
-      const float mx_s = (mx == -INFINITY) ? 0.f : mx * kLog2e;
-      // P chunk ct overwrites S columns 16 ct .. 16 ct + 15 (= S chunk ct / 2 <= ct): in increasing ct order every
-      // S chunk is still intact when it is re-read
-#pragma unroll 1
-      for (int ct = 0; ct < 4; ++ct) {
-        const uint32_t pt = lane_base + kColP + 16 * ct;
-        const int c = ct - ct0;
-        if (c >= 0 && c + 1 < nch) {
-          uint32_t v[32];
-          tmem_ld32(lane_base + kColS + 32 * ct, v);
-          tmem_ld_wait();
-          apply_mask(v, vis(c));
-          softmax_chunk_to_p<F16>(v, mx_s, sum2, pt);
-        } else if (c >= 0 && c + 1 == nch) {
-          softmax_chunk_to_p<F16>(last, mx_s, sum2, pt);
-        } else {
-          tmem_st16_zero(pt);
-        }
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      mbar_arrive(bar_p);
-
-      // epilogue: O / rowsum -> bf16 -> V buffer (swizzled like a TMA box) -> one bulk store per sequence
-      mbar_wait(bar_o, it & 1u);
-      tc_fence_after();
-      const float sum = sum2.x + sum2.y;
-      const float inv = sum > 0.f ? 1.0f / sum : 0.f;
-      const float2 inv2 = make_float2(inv, inv);
-      const uint32_t my_row = sv + static_cast<uint32_t>(r) * 128u;
-      const int sw = r & 7;
+    // ---- S = Q K^T
+    float s[NK / 2];
+    {
+      const uint64_t qdesc = make_smem_desc_sw128(sq + hf * (64 * 128), 1024, 16);
+      const uint64_t kdesc = make_smem_desc_sw128(sk + kbase * 128, 1024, 16);
+      wgmma_pin(s);
+      wgmma_fence();
 #pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        uint32_t v[32];
-        tmem_ld32(lane_base + kColO + 32 * j, v);
-        tmem_ld_wait();
-        if (j == 1) {  // O fully read: the next tile's S = Q K^T may overwrite these columns
-          tc_fence_before();
-          mbar_arrive(bar_e);
-        }
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint32_t u[4];
-#pragma unroll
-          for (int w2 = 0; w2 < 4; ++w2) {
-            const float2 o = __fmul2_rn(make_float2(__uint_as_float(v[8 * q + 2 * w2]), __uint_as_float(v[8 * q + 2 * w2 + 1])), inv2);
-            u[w2] = pack_op2<F16>(o.x, o.y);
-          }
-          const uint32_t u0 = u[0], u1 = u[1], u2 = u[2], u3 = u[3];
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(my_row + (((4 * j + q) ^ sw) << 4)), "r"(u0),
-                       "r"(u1), "r"(u2), "r"(u3)
-                       : "memory");
-        }
-      }
-      fence_proxy_async_smem();
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (threadIdx.x == 0) {
-        for (int gg = 0; gg < G; ++gg) {
-          const int64_t sq_idx = (int64_t)st * G + gg;
-          if (sq_idx < p.n_seq)
-            tma_store_2d(&tmStore, sv + static_cast<uint32_t>(gg * slot) * 128u, h * kHeadDim, (int32_t)(sq_idx * S));
-        }
-        tma_store_commit();
-        tma_store_wait_read();   // the V buffer may be refilled
-        mbar_arrive(bar_vfree);
-      }
+      for (int k = 0; k < kHeadDim / 16; ++k) wgmma_qk<F16, NK>(s, qdesc + 2 * k, kdesc + 2 * k, k != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_pin(s);
     }
-    if (threadIdx.x == 0) tma_store_wait_all();
+
+    // ---- masked softmax on the registers (masked entries -> -inf -> exp2 = 0)
+    float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+    for (int c = 0; c < NK / 4; ++c) {
+      const int j = c >> 1, e = c & 1;
+      const int k_in = k_in_base + 8 * j + e;
+      const bool ok = (kv >> c) & 1u;
+      if (!(ok && k_in <= lim0)) s[4 * j + e] = -INFINITY;
+      if (!(ok && k_in <= lim1)) s[4 * j + 2 + e] = -INFINITY;
+      mx0 = fmaxf(mx0, s[4 * j + e]);
+      mx1 = fmaxf(mx1, s[4 * j + 2 + e]);
+    }
+#pragma unroll
+    for (int o = 1; o < 4; o <<= 1) {  // the 4 lanes that share a row
+      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, o));
+      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, o));
+    }
+    const float ms0 = (mx0 == -INFINITY) ? 0.f : mx0 * kLog2e;
+    const float ms1 = (mx1 == -INFINITY) ? 0.f : mx1 * kLog2e;
+    float sum0 = 0.f, sum1 = 0.f;
+    uint32_t pa[NK / 16][4];  // P as the A fragments of O = P V: k-step kk covers keys 16 kk .. 16 kk + 15
+#pragma unroll
+    for (int j = 0; j < NK / 8; ++j) {
+      const float e00 = fast_exp2(fmaf(s[4 * j + 0], kLog2e, -ms0)), e01 = fast_exp2(fmaf(s[4 * j + 1], kLog2e, -ms0));
+      const float e10 = fast_exp2(fmaf(s[4 * j + 2], kLog2e, -ms1)), e11 = fast_exp2(fmaf(s[4 * j + 3], kLog2e, -ms1));
+      sum0 += e00 + e01;
+      sum1 += e10 + e11;
+      pa[j >> 1][2 * (j & 1) + 0] = pack_op2<F16>(e00, e01);
+      pa[j >> 1][2 * (j & 1) + 1] = pack_op2<F16>(e10, e11);
+    }
+#pragma unroll
+    for (int o = 1; o < 4; o <<= 1) {
+      sum0 += __shfl_xor_sync(0xffffffffu, sum0, o);
+      sum1 += __shfl_xor_sync(0xffffffffu, sum1, o);
+    }
+
+    // ---- O = P V   (V tile [keys][64 dh]: advancing 16 keys = 16 rows of 128 B)
+    float o[32];
+    wgmma_pin(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < NK / 16; ++kk) {
+      const uint64_t vdesc = make_smem_desc_sw128(sv + (kbase + 16 * kk) * 128, 1024, 1024);
+      wgmma_rs_n64<F16>(o, pa[kk], vdesc, kk != 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_pin(o);
+
+    // ---- epilogue: O / rowsum -> 16 bit -> this thread's Q rows (swizzled like a TMA box) -> bulk store per sequence
+    const float inv0 = sum0 > 0.f ? 1.0f / sum0 : 0.f;
+    const float inv1 = sum1 > 0.f ? 1.0f / sum1 : 0.f;
+    const uint32_t row0 = sq + static_cast<uint32_t>(R0) * 128u, row1 = row0 + 8u * 128u;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      st_shared_b32(row0 + ((j ^ rr) << 4) + q4 * 4, pack_op2<F16>(o[4 * j + 0] * inv0, o[4 * j + 1] * inv0));
+      st_shared_b32(row1 + ((j ^ rr) << 4) + q4 * 4, pack_op2<F16>(o[4 * j + 2] * inv1, o[4 * j + 3] * inv1));
+    }
+    fence_proxy_async_smem();
+    __syncthreads();  // the output tile is complete, and both warpgroups are done with K and V
+    if (threadIdx.x == 0) {
+      for (int gg = 0; gg < G; ++gg) {
+        const int64_t sq_idx = (int64_t)st * G + gg;
+        if (sq_idx < p.n_seq)
+          tma_store_2d(&tmStore, sq + static_cast<uint32_t>(gg * slot) * 128u, h * kHeadDim, (int32_t)(sq_idx * S));
+      }
+      tma_store_commit();
+      tma_store_wait_read();   // the Q buffer may be refilled
+      if (tile + (int)gridDim.x < ntiles) issue_loads(tile + gridDim.x);
+    }
   }
+  if (threadIdx.x == 0) tma_store_wait_all();
+}
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc<1>(tmem_base, kTmemCols);
+template <bool F16, int NK>
+int launch_attention_inst(const CUtensorMap& tmL, const CUtensorMap& tmS, const AttParams& p, cudaStream_t st) {
+  auto kern = attention_kernel<F16, NK>;
+  static unsigned long long configured = 0;
+  static int grid_cap = 0;
+  if (first_use_on_device(configured)) {
+    PLIP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttSmem));
+    int dev = 0, sms = 0, per_sm = 0;
+    PLIP_CUDA_CHECK(cudaGetDevice(&dev));
+    PLIP_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    PLIP_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kAttThreads, kAttSmem));
+    grid_cap = (per_sm > 0 ? per_sm : 1) * sms;
+  }
+  const int64_t tiles = p.seq_tiles * p.heads;
+  const int grid = (int)(tiles < grid_cap ? tiles : grid_cap);
+  PLIP_CUDA_CHECK(launch_kernel(kern, dim3(grid), dim3(kAttThreads), kAttSmem, st, 1, tmL, tmS, p));
+  return 0;
 }
 
 }  // namespace
@@ -353,21 +235,10 @@ int launch_attention(const __nv_bfloat16* qkv, int64_t n_seq, int seq_len, int h
   PLIP_REQUIRE(n_seq > 0 && seq_len > 0 && seq_len <= 128, "attention: bad shape n_seq=%lld seq_len=%d",
                (long long)n_seq, seq_len);
   PLIP_REQUIRE(heads > 0 && heads <= 16, "attention: bad head count %d", heads);
-  static unsigned long long configured = 0;
-  static int grid_cap = 0;
-  if (first_use_on_device(configured)) {
-    PLIP_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttSmem));
-    PLIP_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttSmem));
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    grid_cap = kAttCtasPerSm * sms;
-  }
   const int D = heads * kHeadDim;
   const int64_t rows = n_seq * seq_len;
   PLIP_REQUIRE(rows + 128 < 0x7fffffff, "attention: too many token rows");
   AttParams p;
-  p.total_rows = rows;
   p.n_seq = n_seq;
   p.seq_len = seq_len;
   p.slot = seq_len <= 32 ? 32 : (seq_len <= 64 ? 64 : 128);
@@ -379,10 +250,11 @@ int launch_attention(const __nv_bfloat16* qkv, int64_t n_seq, int seq_len, int h
   CUtensorMap tmL, tmS;
   if (int rc = make_tmap_bf16_2d(&tmL, qkv, (uint64_t)rows, (uint64_t)3 * D, (uint64_t)3 * D * 2, (uint32_t)p.slot, 64)) return rc;
   if (int rc = make_tmap_bf16_2d(&tmS, out, (uint64_t)rows, (uint64_t)D, (uint64_t)D * 2, (uint32_t)seq_len, 64)) return rc;
-  const int64_t tiles = p.seq_tiles * heads;
-  const int grid = (int)(tiles < grid_cap ? tiles : grid_cap);
-  if (f16) PLIP_CUDA_CHECK(launch_kernel(attention_kernel<true>, dim3(grid), dim3(kAttThreads), kAttSmem, st, 1, tmL, tmS, p));
-  else PLIP_CUDA_CHECK(launch_kernel(attention_kernel<false>, dim3(grid), dim3(kAttThreads), kAttSmem, st, 1, tmL, tmS, p));
+  PLIP_REQUIRE(p.seq_tiles * heads < 0x7fffffff, "attention: too many tiles");
+  int rc;
+  if (p.slot == 128) rc = f16 ? launch_attention_inst<true, 128>(tmL, tmS, p, st) : launch_attention_inst<false, 128>(tmL, tmS, p, st);
+  else rc = f16 ? launch_attention_inst<true, 64>(tmL, tmS, p, st) : launch_attention_inst<false, 64>(tmL, tmS, p, st);
+  if (rc) return rc;
   ++g_launch_count;
   return 0;
 }

@@ -1,9 +1,7 @@
-// plip_b200 — shared device/host helpers for the sm_100a kernels.
+// plip_b200 — shared device/host helpers for the sm_90a kernels.
 //
-// Thin inline-PTX wrappers for the Blackwell primitives the engine uses:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / st),
-// cluster addressing.  No CUTLASS/CuTe dependency: the bit layouts of the UMMA
-// shared-memory descriptor and instruction descriptor are written out below.
+// Thin inline-PTX wrappers for the Hopper primitives the engine uses: mbarrier, TMA (cp.async.bulk.tensor),
+// cluster addressing.  The warpgroup MMA wrappers live in wgmma.cuh.  No CUTLASS/CuTe dependency.
 #pragma once
 
 #include <cuda.h>
@@ -71,6 +69,14 @@ inline bool first_use_on_device(unsigned long long& mask) {
   return true;
 }
 
+// SMs of the current device (grid caps of the streaming kernels).
+inline int sm_count() {
+  int dev = 0, n = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+  return n > 0 ? n : 132;
+}
+
 // Encode a 2-D bf16 row-major tensor map with 128-byte swizzle.
 // dims: inner (contiguous) extent `cols`, outer extent `rows`, row stride in bytes.
 // box: box_cols (must be 64 bf16 == 128 B for SWIZZLE_128B) x box_rows (<=256).
@@ -80,9 +86,7 @@ int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_
 #ifdef __CUDACC__
 
 // ---------------------------------------------------------------------------
-// Kernel launch helper (cluster dimension as a launch attribute).  Programmatic dependent launch was tried in
-// round 1 and measured again in round 2 (200 full steps each way: 19.55 ms with, 19.38 ms without): no gain on this
-// launch sequence, so the griddepcontrol instructions and the PLIP_PDL switch were removed.
+// Kernel launch helper (cluster dimension as a launch attribute).
 // ---------------------------------------------------------------------------
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
@@ -111,6 +115,10 @@ inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
+}
+
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
 
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
@@ -165,9 +173,8 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t byt
                : "memory");
 }
 // Arrive on a barrier that may live in another CTA of the cluster (shared::cluster address).
-// Plain (CTA-scope release) form: a .release.cluster arrive compiles to MEMBAR.ALL.GPU, which
-// drains every outstanding global store of the thread and serialised the 2-CTA pipeline (ncu r1).
-// The signals sent this way only order tcgen05 / TMA work, which has its own fences.
+// Plain (CTA-scope release) form: the signals sent this way only order wgmma reads against TMA writes of an
+// operand slot, and a .release.cluster arrive would drain every outstanding global store of the thread.
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
   asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
@@ -184,18 +191,15 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Blocking wait with a watchdog: a protocol bug traps (launch error on the host)
-// instead of hanging the GPU.  ~2^31 cycles (> 1 s) is far beyond any legal wait.
+// Blocking wait with a watchdog: a protocol bug traps (launch error on the host) instead of hanging the GPU.
+// ~2^31 cycles (> 1 s) is far beyond any legal wait.  No printf here: a function call inside a kernel that issues
+// wgmma makes ptxas serialise every wgmma.mma_async (warning C7510).
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 0x3ff) == 0 && clock64() - t0 > (1ll << 31)) {
-      printf("plip_b200: mbarrier watchdog: block %d thread %d bar 0x%x parity %u\n",
-             (int)blockIdx.x, (int)threadIdx.x, bar, parity);
-      __trap();
-    }
+    if ((++spins & 0x3ff) == 0 && clock64() - t0 > (1ll << 31)) __trap();
   }
 }
 
@@ -222,27 +226,14 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const CUtensorMap
       ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
-// 2-D tile load for a CTA pair: destination is the executing CTA's smem, completion bytes
-// are credited to `bar_cluster_addr`, which may be the peer (leader) CTA's barrier.
-__device__ __forceinline__ void tma_load_2d_cg2(uint32_t smem_dst, const CUtensorMap* tm,
-                                                uint32_t bar_cluster_addr, int32_t c0, int32_t c1) {
+// 2-D tile load, multicast: the tile lands at the same shared-memory offset of every CTA in `cta_mask` (cluster
+// ranks), and each destination CTA's barrier at `bar`'s offset is credited with the bytes.
+__device__ __forceinline__ void tma_load_2d_mc(uint32_t smem_dst, const CUtensorMap* tm, uint32_t bar, int32_t c0,
+                                               int32_t c1, uint16_t cta_mask) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar_cluster_addr), "r"(c0),
-      "r"(c1)
-      : "memory");
-}
-
-// Same, multicast: the tile lands at the same shared-memory offset of every CTA in `cta_mask` (cluster ranks), and the
-// completion bytes are credited, for each destination CTA, to the barrier at `bar_cluster_addr`'s offset in that
-// destination's pair (the even CTA when `bar_cluster_addr` names an even CTA: the pair leaders in a 2-SM pipeline).
-__device__ __forceinline__ void tma_load_2d_cg2_mc(uint32_t smem_dst, const CUtensorMap* tm, uint32_t bar_cluster_addr,
-                                                   int32_t c0, int32_t c1, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
       " [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "h"(cta_mask)
+      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
 
@@ -256,185 +247,10 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, uint32_t sme
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // all committed store groups have finished READING their shared-memory source
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// all committed store groups but the most recent one have finished reading their shared-memory source
+__device__ __forceinline__ void tma_store_wait_read_but_one() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 // all committed store groups are complete (global writes performed)
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
-// ---------------------------------------------------------------------------
-// tcgen05: TMEM allocation
-// ---------------------------------------------------------------------------
-template <int CG>
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  if constexpr (CG == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  } else {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-}
-template <int CG>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  if constexpr (CG == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-                 : "memory");
-  } else {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-                 : "memory");
-  }
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// ---------------------------------------------------------------------------
-// tcgen05: descriptors
-// ---------------------------------------------------------------------------
-// Shared-memory matrix descriptor (64 bit):
-//   [0,14)  start address >> 4        [16,30) leading byte offset >> 4
-//   [32,46) stride byte offset >> 4   [46,48) version (1 on sm_100)
-//   [49,52) base offset               [52]    LBO mode
-//   [61,64) layout: 0 none, 1 128B_base32B, 2 SWIZZLE_128B, 4 64B, 6 32B
-//
-// K-major SWIZZLE_128B tile (rows of 64 bf16 = 128 B, 8-row groups of 1024 B):
-//   SBO = 1024 (next 8-row group), LBO unused (1).
-// MN-major SWIZZLE_128B tile (k-rows of 64 bf16 along MN, 8 k-rows per 1024 B group):
-//   SBO = 1024 (next 8 k-rows), LBO = stride between 64-wide MN atoms (unused when MN == 64).
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t sbo_bytes,
-                                                         uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= 1ull << 46;  // descriptor version for Blackwell
-  d |= 2ull << 61;  // SWIZZLE_128B
-  return d;
-}
-
-// Instruction descriptor for kind::f16 (bf16 x bf16 -> fp32):
-//   [4,6) c_format (1 = F32)   [7,10) a_format (1 = BF16)   [10,13) b_format (1 = BF16)
-//   [15] a_major (0 = K)       [16] b_major (0 = K, 1 = MN)
-//   [17,23) N >> 3             [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int m, int n, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(n >> 3) << 17) |
-         (static_cast<uint32_t>(m >> 4) << 24);
-}
-// Same with IEEE half operands (a_format = b_format = 0): kind::f16 runs fp16 and bf16 at the same rate.  The
-// engine's "fp16" operand format (plip_create_ex) keeps 11 instead of 8 significand bits in every GEMM /
-// attention operand: end-to-end |dlogits| 6-8x smaller (profiles/r2_precision_study.md), range 65504.
-__host__ __device__ constexpr uint32_t make_idesc_op(int m, int n, int a_mn_major, int b_mn_major, bool f16) {
-  return f16 ? (make_idesc_bf16(m, n, a_mn_major, b_mn_major) & ~((1u << 7) | (1u << 10)))
-             : make_idesc_bf16(m, n, a_mn_major, b_mn_major);
-}
-
-// ---------------------------------------------------------------------------
-// tcgen05: MMA issue / commit
-// ---------------------------------------------------------------------------
-// D[tmem] (+)= A[smem] * B[smem]
-template <int CG>
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                        uint32_t idesc, uint32_t accumulate) {
-  if constexpr (CG == 1) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-// D[tmem] (+)= A[tmem] * B[smem]   (A operand read from tensor memory)
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc,
-                                        uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// Arrive (count 1) on `bar` once all MMAs previously issued by this thread have completed.
-// CG == 2: the arrive is multicast to the same barrier offset in both CTAs of the pair.
-template <int CG>
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  if constexpr (CG == 1) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-                 : "memory");
-  } else {
-    const uint16_t mask = 0x3;
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 "
-        "[%0], %1;" ::"r"(bar),
-        "h"(mask)
-        : "memory");
-  }
-}
-
-// cta_group::2 commit with an explicit cluster-rank mask (clusters of more than one CTA pair)
-__device__ __forceinline__ void umma_commit_mask(uint32_t bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 "
-      "[%0], %1;" ::"r"(bar),
-      "h"(mask)
-      : "memory");
-}
-
-// ---------------------------------------------------------------------------
-// tcgen05: TMEM <-> registers.  32x32b: thread t of the warp owns TMEM lane
-// (32 * (warp_id % 4) + t); xN = N consecutive 32-bit columns.
-// ---------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-        "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]),
-      "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]),
-      "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]),
-      "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]),
-      "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
 
 // ---------------------------------------------------------------------------
 // Packing / math
@@ -458,24 +274,12 @@ __device__ __forceinline__ uint32_t pack_op2_rt(float lo, float hi, int f16) {  
 }
 // QuickGELU: x * sigmoid(1.702 x)   (TF:activations.py:117-123)
 // sigmoid(y) = 0.5 * (1 + tanh(y / 2)): one MUFU op (tanh.approx.f32, max rel. error 2^-11) instead of
-// ex2 + rcp.  The fc1 epilogue is MUFU-bound (ncu r1: 128x256 tile = 4096 MUFU cycles per SM sub-partition
-// vs 6144 MMA cycles); the absolute error (<= 2.5e-4 |x|) is ~10x below the bf16 rounding of the result.
+// ex2 + rcp; the absolute error (<= 2.5e-4 |x|) is ~10x below the bf16 rounding of the result.
 __device__ __forceinline__ float quick_gelu(float x) {
   float t;
   asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.851f * x));
   const float h = 0.5f * x;
   return fmaf(h, t, h);
-}
-// Two elements at once with Blackwell's packed fp32 pipe (FMUL2 / FFMA2: one issue slot, two results).  The epilogues
-// and the softmax are FMA-pipe / issue bound next to the tensor pipe (ncu r2b: text fc1 epilogue paces the MMAs at
-// K = 512), so every scalar FFMA pair that becomes one FFMA2 shortens the co-critical path.
-__device__ __forceinline__ float2 quick_gelu2(float2 x) {
-  const float2 a = __fmul2_rn(x, make_float2(0.851f, 0.851f));
-  float2 t;
-  asm("tanh.approx.f32 %0, %1;" : "=f"(t.x) : "f"(a.x));
-  asm("tanh.approx.f32 %0, %1;" : "=f"(t.y) : "f"(a.y));
-  const float2 h = __fmul2_rn(x, make_float2(0.5f, 0.5f));
-  return __ffma2_rn(h, t, h);
 }
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

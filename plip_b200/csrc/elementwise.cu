@@ -308,7 +308,7 @@ __global__ void __launch_bounds__(kEwThreads) l2_normalize_kernel(float* __restr
 
 inline int grid_for(int64_t work_items, int per_block) {
   int64_t blocks = (work_items + per_block - 1) / per_block;
-  const int64_t cap = 148LL * 16;
+  const int64_t cap = 16LL * sm_count();
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   return (int)blocks;

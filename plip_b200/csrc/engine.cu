@@ -502,7 +502,7 @@ int grow_dev(void** p, size_t* have, size_t want) {
 // the first EOS, so captions sorted by that length can be processed bucket by bucket, each bucket only up to its own
 // longest caption.  Buckets are chosen by dynamic programming over the (<= 77) distinct lengths: cost of a bucket
 // = max(captions x prefix, kMinBucketRows) + kBucketOverheadRows token rows — a GEMM needs ~8k rows to fill the
-// 148 SMs once, and a 66-launch pass costs about as much as 2k token rows — so small or uniform batches stay in
+// SMs once, and a 66-launch pass costs about as much as 2k token rows — so small or uniform batches stay in
 // one bucket.  perm[i] = original index of the caption at sorted position i (stable); bucket k covers sorted
 // positions [start[k], start[k+1]) and is processed with prefix[k].  Returns the number of buckets.
 constexpr long long kMinBucketRows = 8192, kBucketOverheadRows = 2048;
@@ -660,7 +660,7 @@ PLIP_API int plip_create_ex(const void* host_blob, uint64_t nbytes, float logit_
   PLIP_CUDA_CHECK(cudaSetDevice(device));
   cudaDeviceProp prop;
   PLIP_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-  PLIP_REQUIRE(prop.major == 10, "plip_create: device %d is sm_%d%d; this library is built for sm_100a only",
+  PLIP_REQUIRE(prop.major == 9 && prop.minor == 0, "plip_create: device %d is sm_%d%d; this library is built for sm_90a only",
                device, prop.major, prop.minor);
   plip_engine* e = new plip_engine();
   e->device = device;
@@ -1063,7 +1063,7 @@ PLIP_API int plip_dbg_set_operand_format(int operand_format) {
 }
 
 PLIP_API int plip_dbg_gemm(const void* A_bf16, int lda, const void* W_bf16, int ldw, int M, int N, int K,
-                           const float* bias, void* out, int ldo, const float* pos, int epilogue, int cta_group,
+                           const float* bias, void* out, int ldo, const float* pos, int epilogue, int cluster_size,
                            int block_n, const float* colsum, const float* stats_in, int n_partials, void* xb_out,
                            float* stats_out, void* stream) {
   GemmArgs g;
@@ -1073,7 +1073,7 @@ PLIP_API int plip_dbg_gemm(const void* A_bf16, int lda, const void* W_bf16, int 
   g.bias = bias; g.out = out; g.ldo = ldo; g.pos = pos; g.epi = epilogue;
   g.colsum = colsum; g.stats_in = reinterpret_cast<const float2*>(stats_in); g.n_partials = n_partials;
   g.xb_out = static_cast<__nv_bfloat16*>(xb_out); g.stats_out = reinterpret_cast<float2*>(stats_out);
-  g.force_cg = cta_group; g.force_bn = block_n;
+  g.force_cg = cluster_size; g.force_bn = block_n;
   g.f16 = g_dbg_f16;
   return launch_gemm(g, static_cast<cudaStream_t>(stream));
 }

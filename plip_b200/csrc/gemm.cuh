@@ -1,4 +1,4 @@
-// plip_b200 — tcgen05 GEMM interface (host side).
+// plip_b200 — wgmma GEMM interface (host side).
 #pragma once
 #include "common.cuh"
 
@@ -16,7 +16,7 @@ enum GemmEpilogue : int {
   // partials of x come from the producing residual GEMM:  out = rstd_r (acc - mean_r colsum_n) + bias'_n.
   EPI_LN_BIAS_BF16 = 5,       // layer_norm1 + q/k/v projection            (TF:371, 310-312)
   EPI_LN_BIAS_GELU_BF16 = 6,  // layer_norm2 + fc1 + QuickGELU             (TF:380, 348-349)
-  EPI_NULL = 7,               // (diagnostic) accumulators are read from TMEM and dropped: main-loop-only rate
+  EPI_NULL = 7,               // (diagnostic) accumulators are dropped: main-loop-only rate
   // Similarity head on the tensor cores (similarity.cu): out_f32[r,c] = acc * rowscale[r] * colscale[c].  The operands
   // are fp16 hi/lo splits of power-of-two-scaled embeddings ([hi|lo|hi] x [hi|hi|lo], K = 3 x 512), the scales undo
   // the power of two and carry logit_scale and the optional 1/|x| normalisation.   (TF:modeling_clip.py:923-930)
@@ -24,7 +24,7 @@ enum GemmEpilogue : int {
   EPI_COUNT = 9
 };
 
-constexpr int kStatSlots = 8;  // per-row partial statistics slots (two per N tile of the producing GEMM: one per epilogue warp half)
+constexpr int kStatSlots = 8;  // per-row partial statistics slots (two per N tile of the producing GEMM: one per half of the tile's columns)
 
 struct GemmArgs {
   const __nv_bfloat16* A = nullptr;  // [M, K] row-major, row stride lda elements
@@ -45,8 +45,8 @@ struct GemmArgs {
   int* n_tiles_used = nullptr;       // out (host): number of statistics slots written (2 per N tile)
   int epi = EPI_F32;
   int f16 = 0;                       // 16-bit operand format of A, W and the bf16-typed outputs: 0 = bfloat16, 1 = IEEE half
-  int force_cg = 0;                  // 0 = auto; 1 / 2 = CTA-group size (test hook)
-  int force_bn = 0;                  // 0 = auto; 128 / 256 = N tile (test hook)
+  int force_cg = 0;                  // 0 = auto; 1 / 2 = CTAs per cluster (test hook)
+  int force_bn = 0;                  // 0 = auto; 128 / 192 / 256 = N tile (test hook)
 };
 
 // Enqueue the GEMM on `stream`.  Returns 0 on success (see last_error otherwise).

@@ -18,7 +18,7 @@
 // vertical pass runs out of that strip, one thread per 4 output bytes.
 // Source pixels are read once per strip (strips overlap by the filter support; L2 absorbs the re-reads); the
 // roofline is HBM (source bytes + 150,528 tile bytes per image) but the kernel is issue-bound: H_src x 224 x 3 x
-// taps integer MACs per image with ~3 instructions each (profiles/r1_resize_probe.json).
+// taps integer MACs per image with ~3 instructions each.
 #include "kernels.cuh"
 
 #include <math.h>
@@ -316,7 +316,7 @@ static int plan_image(const plip_resize_desc_t& s, long long idx, size_t src_byt
   const size_t tb = table_bytes(ksh, ksv);
   // Strip height: taller strips re-read fewer source rows (adjacent strips overlap by the filter support),
   // shorter ones need less shared memory and keep more CTAs per SM.  Relative throughput by resident CTAs
-  // measured on B200 (profiles/r1_resize_probe.json); registers cap residency at 5.
+  // (tools/resize_probe.py measures it; these weights have not been re-measured on H100); registers cap residency at 5.
   static const double kThroughput[6] = {0.0, 1.0, 1.12, 1.21, 1.57, 1.70};
   const double vscale = (double)s.height / (double)s.new_height, fs = vscale < 1.0 ? 1.0 : vscale;
   int rp = 0, rows = 0;

@@ -344,7 +344,7 @@ similarity_topk_tiled_kernel(const float* __restrict__ Q, int64_t n, const float
 
 
 // ---- similarity on the tensor cores ------------------------------------------------------------------------------
-// scale * norm(a) . norm(b)^T as ONE tcgen05 GEMM with fp32-class accuracy: every embedding row is scaled by a power
+// scale * norm(a) . norm(b)^T as ONE wgmma GEMM with fp32-class accuracy: every embedding row is scaled by a power
 // of two to max|x| in [32, 64) and split into fp16 hi + lo (22 significand bits, every fp16 x fp16 product exact in the
 // fp32 accumulator); with A' = [hi | lo | hi] and B' = [hi | hi | lo] (K = 3 x 512) the GEMM sums hi.hi + lo.hi + hi.lo
 // (the dropped lo.lo term is 2^-22 relative).  Row / column scale vectors undo the powers of two and carry logit_scale
@@ -439,7 +439,8 @@ int launch_similarity_tc(const float* a, int64_t n, const float* b, int64_t m, f
   __half* asplit = reinterpret_cast<__half*>(base + bytes_b);
   float* cscale = reinterpret_cast<float*>(base + bytes_b + bytes_a);
   float* rscale = cscale + m_pad;
-  auto grid_for_rows = [](int64_t r) { int64_t g = (r + 7) / 8; return (int)(g < 1 ? 1 : (g > 148 * 8 ? 148 * 8 : g)); };
+  const int64_t row_grid_cap = 8LL * sm_count();
+  auto grid_for_rows = [row_grid_cap](int64_t r) { int64_t g = (r + 7) / 8; return (int)(g < 1 ? 1 : (g > row_grid_cap ? row_grid_cap : g)); };
   PLIP_CUDA_CHECK(launch_kernel(split_embed_kernel, dim3(grid_for_rows(m_pad)), dim3(256), 0, st, 1, b, m, m_pad,
                                 norm_b ? 1 : 0, 1, 1.0f, bsplit, cscale));
   ++g_launch_count;
@@ -611,7 +612,7 @@ int launch_similarity_topk(const float* q, int64_t n, const float* s, int64_t m,
   }
   const int64_t row_tiles = (n + TM - 1) / TM, space_tiles = (m + TN - 1) / TN;
   PLIP_REQUIRE(row_tiles <= 0x7fffffff, "similarity_topk: too many queries");
-  int64_t splits = (2 * 148 + row_tiles - 1) / row_tiles;  // aim at ~2 CTAs per SM
+  int64_t splits = (2 * sm_count() + row_tiles - 1) / row_tiles;  // aim at ~2 CTAs per SM
   if (splits > space_tiles) splits = space_tiles;
   if (splits > 64) splits = 64;
   if (splits < 1) splits = 1;

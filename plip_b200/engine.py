@@ -65,7 +65,7 @@ def similarity_topk(query: torch.Tensor, space: torch.Tensor, k: int, scale: flo
     """``plip_similarity_topk`` needs no engine handle (no weights involved): fused scores + top-k over ``space`` rows on
     ``device`` (default: the current CUDA device).  Returns ``(idx int32 [n,k], val f32 [n,k])``, best first."""
     if not torch.cuda.is_available():
-        raise RuntimeError("plip_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise RuntimeError("plip_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
     dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
     L = lib()
     q = query.to(torch.float32).to(dev, non_blocking=True).contiguous()
@@ -91,7 +91,7 @@ class Engine:
         ``"fp16"`` (same speed, 3 more significand bits: 6-8x smaller end-to-end logits error, 65504 range; what the
         reference's OpenAI-clip flavour runs on a GPU).  Accumulation / residual stream / softmax are fp32 in both."""
         if not torch.cuda.is_available():
-            raise RuntimeError("plip_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("plip_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self._L = lib()
         dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         if dev.type != "cuda":

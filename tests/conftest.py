@@ -9,11 +9,11 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-GOLDEN = os.path.join(ROOT, "tests", "golden", "clip_golden.npz")
+GOLDEN = [os.path.join(ROOT, "tests", "golden", name) for name in ("clip_golden.npz", "processor_golden.npz")]
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box: pytest -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (pytest -m gpu on an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -27,7 +27,10 @@ def pytest_collection_modifyitems(config, items):
 
 @pytest.fixture(scope="session")
 def golden():
-    return dict(np.load(GOLDEN, allow_pickle=False))
+    out = {}
+    for path in GOLDEN:
+        out.update(np.load(path, allow_pickle=False))
+    return out
 
 
 @pytest.fixture(scope="session")

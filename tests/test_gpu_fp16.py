@@ -1,6 +1,6 @@
 """The fp16 operand format (``Engine(..., operand_dtype="fp16")`` / ``plip_create_ex``): same kernels with IEEE-half
 GEMM / attention operands.  Bounds are 2-3x what the CPU emulation of this contract gives
-(tools/precision_study.py, profiles/r2_precision_study.md: 1-cos 9e-8 / 4e-7, |dlogits| 1.7e-3 max over 64 x 32)."""
+(tools/precision_study.py: 1-cos 9e-8 / 4e-7, |dlogits| 1.7e-3 max over 64 x 32)."""
 import pytest
 import torch
 

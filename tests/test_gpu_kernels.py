@@ -197,7 +197,7 @@ def test_attention(L, n_seq, S, heads, causal, use_mask):
 
 
 def test_similarity_tensor_core_path(L):
-    """Wide score matrices (>= 256 columns) run as one tcgen05 GEMM on fp16 hi/lo splits (similarity.cu): fp32-class
+    """Wide score matrices (>= 256 columns) run as one wgmma GEMM on fp16 hi/lo splits (similarity.cu): fp32-class
     accuracy at PLIP's largest trained logit scale (100), with and without on-the-fly normalisation, ragged sizes."""
     g = torch.Generator().manual_seed(5)
     for n, m, na, nb, mag in ((1000, 777, True, True, 1.0), (130, 300, False, False, 1.0), (257, 1024, True, False, 37.0)):

@@ -1,4 +1,4 @@
-"""The CPU emulation behind DESIGN.md §2 / profiles/r2_precision_study.md stays runnable and keeps telling the same
+"""The CPU emulation behind DESIGN.md §2 stays runnable and keeps telling the same
 story on a tiny sample: fp16 operands beat bf16 by ~an order of magnitude in logits error, the 3-term split is exact
 to ~1e-5, and the LayerNorm fold does not cost accuracy on the outlier weights."""
 import json

@@ -11,7 +11,7 @@ applied before the operand rounding (``r(LN(x)) r(W)^T``).  It answers, without 
   2. whether the LayerNorm fold loses precision on trained-CLIP-like residual streams (``mode="outlier"`` weights);
   3. what a "centred" fold (operand = r(x - shift_r)) buys.
 
-    python tools/precision_study.py [--images 64 --captions 32 --out profiles/r2_precision_study.json]
+    python tools/precision_study.py [--images 64 --captions 32 --out precision_study.json]
 """
 from __future__ import annotations
 
@@ -57,7 +57,7 @@ def ln_linear(x, gamma, beta, w, b, c: Cfg, shift=None):
         return rnd(O.layer_norm(x, gamma, beta), c.act) @ rnd(w, c.wgt).t() + b
     K = x.shape[-1]
     mean = x.sum(-1, keepdim=True) / K
-    var = (x * x).sum(-1, keepdim=True) / K - mean * mean          # one-pass, fp32 (gemm_tcgen05.cu epilogue)
+    var = (x * x).sum(-1, keepdim=True) / K - mean * mean          # one-pass, fp32 (gemm_wgmma.cu epilogue)
     rstd = torch.rsqrt(var.clamp_min(0) + EPS)
     wf = rnd(w * gamma[None, :], c.wgt)
     colsum = wf.sum(1)
@@ -138,7 +138,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--images", type=int, default=64)
     ap.add_argument("--captions", type=int, default=32)
-    ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "r2_precision_study.json"))
+    ap.add_argument("--out", default="precision_study.json")
     ap.add_argument("--modes", default="rich,outlier")
     args = ap.parse_args()
     torch.set_grad_enabled(False)

@@ -1,4 +1,4 @@
-"""Run a few vision (and text) forwards at batch 1024 for ncu launch lists / captures (no timing here)."""
+"""Run a few vision (and text) forwards at batch 1024 for a profiler to attach to (no timing here)."""
 import os
 import sys
 
