@@ -251,12 +251,8 @@ int launch_attention(const __nv_bfloat16* qkv, int64_t n_seq, int seq_len, int h
   if (int rc = make_tmap_bf16_2d(&tmL, qkv, (uint64_t)rows, (uint64_t)3 * D, (uint64_t)3 * D * 2, (uint32_t)p.slot, 64)) return rc;
   if (int rc = make_tmap_bf16_2d(&tmS, out, (uint64_t)rows, (uint64_t)D, (uint64_t)D * 2, (uint32_t)seq_len, 64)) return rc;
   PLIP_REQUIRE(p.seq_tiles * heads < 0x7fffffff, "attention: too many tiles");
-  int rc;
-  if (p.slot == 128) rc = f16 ? launch_attention_inst<true, 128>(tmL, tmS, p, st) : launch_attention_inst<false, 128>(tmL, tmS, p, st);
-  else rc = f16 ? launch_attention_inst<true, 64>(tmL, tmS, p, st) : launch_attention_inst<false, 64>(tmL, tmS, p, st);
-  if (rc) return rc;
-  ++g_launch_count;
-  return 0;
+  if (p.slot == 128) return f16 ? launch_attention_inst<true, 128>(tmL, tmS, p, st) : launch_attention_inst<false, 128>(tmL, tmS, p, st);
+  return f16 ? launch_attention_inst<true, 64>(tmL, tmS, p, st) : launch_attention_inst<false, 64>(tmL, tmS, p, st);
 }
 
 }  // namespace plip

@@ -11,6 +11,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <atomic>
+
 namespace plip {
 
 // ---------------------------------------------------------------------------
@@ -58,6 +60,10 @@ void set_last_error(const char* fmt, ...);
     }                                                                                \
   } while (0)
 
+// Kernels enqueued for execution since load (plip_launch_count): launch_kernel counts each launch, a stream capture
+// takes back the kernels it recorded (nothing runs), and a graph replay adds its kernel nodes.
+inline std::atomic<unsigned long long> g_launch_count{0};
+
 // cudaFuncSetAttribute is per device: returns true the first time it is called for the current device with
 // a given per-kernel mask (a process that drives several GPUs configures each kernel once per GPU).
 inline bool first_use_on_device(unsigned long long& mask) {
@@ -86,7 +92,7 @@ int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_
 #ifdef __CUDACC__
 
 // ---------------------------------------------------------------------------
-// Kernel launch helper (cluster dimension as a launch attribute).
+// Kernel launch helper (cluster dimension as a launch attribute); counts the launch in g_launch_count.
 // ---------------------------------------------------------------------------
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
@@ -107,7 +113,9 @@ inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block
   }
   cfg.attrs = attr;
   cfg.numAttrs = na;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+  const cudaError_t err = cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+  if (err == cudaSuccess) g_launch_count.fetch_add(1, std::memory_order_relaxed);
+  return err;
 }
 
 // ---------------------------------------------------------------------------

@@ -328,7 +328,6 @@ int launch_im2col(const void* pixels, int fmt, int64_t n, __nv_bfloat16* out, in
     default: set_last_error("im2col: unknown pixel format %d", fmt); return -2;
   }
   PLIP_CUDA_CHECK(cudaGetLastError());
-  ++g_launch_count;
   return 0;
 }
 
@@ -347,7 +346,6 @@ int launch_layernorm(const float* x, const int32_t* row_index, int64_t in_row_st
     return -2;
   }
   PLIP_CUDA_CHECK(cudaGetLastError());
-  ++g_launch_count;
   return 0;
 }
 
@@ -362,7 +360,6 @@ int launch_rowstats_cast(const float* x, int64_t rows, int dim, __nv_bfloat16* x
     set_last_error("rowstats_cast: unsupported dim %d", dim);
     return -2;
   }
-  ++g_launch_count;
   return 0;
 }
 
@@ -384,7 +381,6 @@ int launch_text_embed(const void* ids, int ids_dtype, int64_t n, int seq_len, in
     return -2;
   }
   PLIP_CUDA_CHECK(cudaGetLastError());
-  g_launch_count += 2;
   return 0;
 }
 
@@ -396,14 +392,12 @@ int launch_mask_to_i32(const void* mask, int dtype, int64_t count, int seq_len, 
   else
     PLIP_CUDA_CHECK(launch_kernel(mask_to_i32_kernel<int>, dim3(grid), dim3(kEwThreads), 0, st, 1, static_cast<const int*>(mask), count, seq_len, stride, out));
   PLIP_CUDA_CHECK(cudaGetLastError());
-  ++g_launch_count;
   return 0;
 }
 
 int launch_cls_rows(const float* cls, const float* pos, int64_t n, float* x, cudaStream_t st) {
   PLIP_CUDA_CHECK(launch_kernel(cls_rows_kernel, dim3(grid_for(n * (kVisDim / 4), kEwThreads)), dim3(kEwThreads), 0, st, 1, cls, pos, n, x));
   PLIP_CUDA_CHECK(cudaGetLastError());
-  ++g_launch_count;
   return 0;
 }
 
@@ -415,7 +409,6 @@ int launch_gather_rows(const __nv_bfloat16* a16, const float* x32, const int32_t
                                 reinterpret_cast<const uint4*>(a16), reinterpret_cast<const uint4*>(x32), row_index,
                                 row_stride, n, dim, reinterpret_cast<uint4*>(a16_out), reinterpret_cast<uint4*>(x32_out)));
   PLIP_CUDA_CHECK(cudaGetLastError());
-  ++g_launch_count;
   return 0;
 }
 
@@ -423,7 +416,6 @@ int launch_l2_normalize(float* x, int64_t rows, int dim, cudaStream_t st) {
   PLIP_REQUIRE(rows > 0 && dim > 0, "l2_normalize: bad shape");
   PLIP_CUDA_CHECK(launch_kernel(l2_normalize_kernel, dim3(grid_for(rows, kEwThreads / 32)), dim3(kEwThreads), 0, st, 1, x, rows, dim));
   PLIP_CUDA_CHECK(cudaGetLastError());
-  ++g_launch_count;
   return 0;
 }
 

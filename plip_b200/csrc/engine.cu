@@ -17,6 +17,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <array>
 #include <map>
 #include <string>
 #include <tuple>
@@ -116,6 +117,23 @@ size_t pixel_bytes(int fmt) {
   return fmt == PLIP_PIX_F32_NCHW ? px * 4 : (fmt == PLIP_PIX_BF16_NCHW ? px * 2 : px);
 }
 
+// Everything a captured launch sequence bakes in (the engine's buffers aside).  Unused fields are 0.
+struct GraphKey {
+  int tower;  // 0 vision, 1 text
+  int n;
+  int format;  // pixel format / ids dtype
+  int normalize, seq_len, prefix_len, has_mask, pool_argmax, prune;
+  auto fields() const {
+    return std::tie(tower, n, format, normalize, seq_len, prefix_len, has_mask, pool_argmax, prune);
+  }
+  bool operator<(const GraphKey& o) const { return fields() < o.fields(); }
+};
+
+struct Graph {
+  cudaGraphExec_t exec = nullptr;
+  unsigned long long kernels = 0;  // kernel nodes: what one replay adds to g_launch_count
+};
+
 }  // namespace
 }  // namespace plip
 
@@ -162,18 +180,16 @@ struct plip_engine {
   size_t d_out_bytes = 0;
   void* d_aux = nullptr;  // ids + mask for the text host path
   size_t d_aux_bytes = 0;
-  // small-batch path: the ~67 launches of a tower are replayed as ONE CUDA graph per (tower, n, input format ...) on
-  // engine-owned staging buffers (inputs are copied in, the [n,512] result copied out), which removes the host-side
-  // launch cost that dominates when a forward is only a few hundred microseconds of GPU work (reference default:
+  // small-batch path: the ~67 launches of a tower are replayed as ONE CUDA graph per GraphKey on engine-owned
+  // staging buffers (inputs are copied in, the [n,512] result copied out), which removes the host-side launch cost
+  // that dominates when a forward is only a few hundred microseconds of GPU work (reference default:
   // batch_size = 8, plip.py:95-97).  PLIP_GRAPH_MAX (default 128, 0 = off) bounds n.
   int graph_max_n = 128;
   cudaStream_t s_cap = nullptr;
-  void* g_in = nullptr;        // staged pixels / ids
-  size_t g_in_bytes = 0;
-  void* g_mask = nullptr;
-  size_t g_mask_bytes = 0;
+  void* g_in[2] = {nullptr, nullptr};  // staged pixels / ids, attention mask
+  size_t g_in_bytes[2] = {0, 0};
   float* g_out = nullptr;      // [graph_max_n, 512]
-  std::map<std::tuple<int, int, int, int, int, int, int>, cudaGraphExec_t> graphs;
+  std::map<GraphKey, Graph> graphs;
   // in-step kernel timing (plip_profile_*): a CUDA event pair around every launch of a forward pass, recorded on
   // the launch stream, so bench.py can report each kernel's average duration INSIDE the step it belongs to
   bool prof_on = false;
@@ -262,6 +278,40 @@ WsLayout ws_layout(int mb) {
   return w;
 }
 
+// One GEMM of a forward pass in the engine's operand format, profiled as `kind` with its algorithmic work
+// (DESIGN.md §4): 2·M·N·K FLOPs; A and W read once, the output written once (an fp32 residual read and written),
+// plus the 16-bit copy of the updated rows when the residual epilogue emits one.
+int gemm(plip_engine* e, int kind, GemmArgs g, cudaStream_t st) {
+  g.f16 = e->f16;
+  const double M = g.M, N = g.N, K = g.K;
+  const double out_elem = g.epi == EPI_BIAS_RESID_F32 ? 8 : (g.epi == EPI_F32 || g.epi == EPI_PATCH_F32 ? 4 : 2);
+  ProfScope ps(e, st, kind, 2 * M * N * K, M * K * 2 + N * K * 2 + M * N * out_elem + (g.xb_out ? M * N * 2 : 0));
+  return launch_gemm(g, st);
+}
+
+// The rest of an encoder layer after attention, on `rows` rows of the attention output `ao` and the fp32 residual
+// stream `x`:  x = x + out_proj(ao);  x = x + fc2(quick_gelu(fc1(LN2(x))))            TF:modeling_clip.py:370-382
+// The residual GEMMs leave Xn / stats (the input of the next LayerNorm-folded GEMM) and the number of statistics
+// partials in np; the last layer's fc2 does not, its output only feeds the pooled-row LayerNorm (fp32 x).
+int layer_tail(plip_engine* e, const LayerW& w, int rows, int D, int FF, const __nv_bfloat16* ao, float* x, bool last,
+               int& np, cudaStream_t st) {
+  GemmArgs g;
+  g.A = ao; g.lda = D; g.W = w.wo; g.ldw = D; g.M = rows; g.N = D; g.K = D;
+  g.bias = w.bo; g.out = x; g.ldo = D; g.epi = EPI_BIAS_RESID_F32;
+  g.xb_out = e->Xn; g.stats_out = e->stats; g.n_tiles_used = &np;
+  if (int rc = gemm(e, PK_OUT, g, st)) return rc;
+  g = GemmArgs();
+  g.A = e->Xn; g.lda = D; g.W = w.w1; g.ldw = D; g.M = rows; g.N = FF; g.K = D;
+  g.bias = w.b1; g.colsum = w.s1; g.stats_in = e->stats; g.n_partials = np;
+  g.out = e->H; g.ldo = FF; g.epi = EPI_LN_BIAS_GELU_BF16;
+  if (int rc = gemm(e, PK_FC1, g, st)) return rc;
+  g = GemmArgs();
+  g.A = e->H; g.lda = FF; g.W = w.w2; g.ldw = FF; g.M = rows; g.N = D; g.K = FF;
+  g.bias = w.b2; g.out = x; g.ldo = D; g.epi = EPI_BIAS_RESID_F32;
+  if (!last) { g.xb_out = e->Xn; g.stats_out = e->stats; g.n_tiles_used = &np; }
+  return gemm(e, PK_FC2, g, st);
+}
+
 // Encoder layers with both LayerNorms folded into the consuming GEMMs.  On entry X holds the residual
 // stream; Xn / stats are (re)derived from it here and afterwards maintained by the residual epilogues.
 //
@@ -277,103 +327,39 @@ int run_layers(plip_engine* e, const LayerW* L, int64_t n_seq, int S, int D, int
   const int64_t M = n_seq * S;
   PLIP_REQUIRE(M <= 0x7fffffff / 4, "micro-batch too large");
   if (num_layers <= 0) return 0;
-  const double dM = (double)M, dD = (double)D, dF = (double)FF;
   {
-    ProfScope ps(e, st, PK_ROWSTATS, 0, dM * dD * 6 + dM * 8);
+    ProfScope ps(e, st, PK_ROWSTATS, 0, (double)M * D * 6 + (double)M * 8);
     if (int rc = launch_rowstats_cast(e->X, M, D, e->Xn, e->stats, e->f16, st)) return rc;
   }
-  // algorithmic HBM bytes per launch (DESIGN.md §4): operands read once, outputs written once
-  const double b_qkv = dM * dD * 2 + 3 * dD * dD * 2 + dM * 3 * dD * 2;
-  const double b_att = dM * 3 * dD * 2 + dM * dD * 2;
-  const double b_out = dM * dD * 2 + dD * dD * 2 + dM * dD * (4 + 4 + 2);
-  const double b_fc1 = dM * dD * 2 + dD * dF * 2 + dM * dF * 2;
-  const double b_fc2 = dM * dF * 2 + dD * dF * 2 + dM * dD * (4 + 4 + 2);
+  const double b_att = (double)M * 3 * D * 2 + (double)M * D * 2;
   const double f_att = 4.0 * (double)n_seq * heads * S * S * kHeadDim;
   int np = 1;
   for (int l = 0; l < num_layers; ++l) {
     const LayerW& w = L[l];
-    // x = x + out_proj(attn(LN1(x)))                                     TF:modeling_clip.py:370-377
+    const bool last = l + 1 == num_layers;
+    // LN1 + q/k/v projection, attention                                   TF:modeling_clip.py:370-376
     GemmArgs g;
-    g.f16 = e->f16;
     g.A = e->Xn; g.lda = D; g.W = w.wqkv; g.ldw = D; g.M = (int)M; g.N = 3 * D; g.K = D;
     g.bias = w.bqkv; g.colsum = w.sqkv; g.stats_in = e->stats; g.n_partials = np;
     g.out = e->QKV; g.ldo = 3 * D; g.epi = EPI_LN_BIAS_BF16;
-    {
-      ProfScope ps(e, st, PK_QKV, 2.0 * dM * 3 * dD * dD, b_qkv);
-      if (int rc = launch_gemm(g, st)) return rc;
-    }
+    if (int rc = gemm(e, PK_QKV, g, st)) return rc;
     {
       ProfScope ps(e, st, PK_ATTN, f_att, b_att);
       if (int rc = launch_attention(e->QKV, n_seq, S, heads, causal, kmask, e->AO, e->f16, st)) return rc;
     }
-    if (prune && l + 1 == num_layers) {
-      // compact copies of the pooled rows: attention output -> head of the (now free) QKV buffer, residual rows behind it
-      const double dn = (double)n_seq;
-      __nv_bfloat16* ao_p = e->QKV;
-      float* x_p = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(e->QKV) + (((size_t)n_seq * D * 2 + 1023) & ~(size_t)1023));
-      {
-        ProfScope ps(e, st, PK_MISC, 0, dn * dD * 12);
-        if (int rc = launch_gather_rows(e->AO, e->X, pool_idx, S, n_seq, D, ao_p, x_p, st)) return rc;
-      }
-      g = GemmArgs();
-      g.f16 = e->f16;
-      g.A = ao_p; g.lda = D; g.W = w.wo; g.ldw = D; g.M = (int)n_seq; g.N = D; g.K = D;
-      g.bias = w.bo; g.out = x_p; g.ldo = D; g.epi = EPI_BIAS_RESID_F32;
-      g.xb_out = e->Xn; g.stats_out = e->stats; g.n_tiles_used = &np;
-      {
-        ProfScope ps(e, st, PK_OUT, 2.0 * dn * dD * dD, dn * dD * 12 + dD * dD * 2);
-        if (int rc = launch_gemm(g, st)) return rc;
-      }
-      g = GemmArgs();
-      g.f16 = e->f16;
-      g.A = e->Xn; g.lda = D; g.W = w.w1; g.ldw = D; g.M = (int)n_seq; g.N = FF; g.K = D;
-      g.bias = w.b1; g.colsum = w.s1; g.stats_in = e->stats; g.n_partials = np;
-      g.out = e->H; g.ldo = FF; g.epi = EPI_LN_BIAS_GELU_BF16;
-      {
-        ProfScope ps(e, st, PK_FC1, 2.0 * dn * dD * dF, dn * dD * 2 + dD * dF * 2 + dn * dF * 2);
-        if (int rc = launch_gemm(g, st)) return rc;
-      }
-      g = GemmArgs();
-      g.f16 = e->f16;
-      g.A = e->H; g.lda = FF; g.W = w.w2; g.ldw = FF; g.M = (int)n_seq; g.N = D; g.K = FF;
-      g.bias = w.b2; g.out = x_p; g.ldo = D; g.epi = EPI_BIAS_RESID_F32;
-      {
-        ProfScope ps(e, st, PK_FC2, 2.0 * dn * dD * dF, dn * dF * 2 + dD * dF * 2 + dn * dD * 8);
-        if (int rc = launch_gemm(g, st)) return rc;
-      }
-      e->pooled_x = x_p;
-      break;
+    if (!(prune && last)) {
+      if (int rc = layer_tail(e, w, (int)M, D, FF, e->AO, e->X, last, np, st)) return rc;
+      continue;
     }
-    g = GemmArgs();
-    g.f16 = e->f16;
-    g.A = e->AO; g.lda = D; g.W = w.wo; g.ldw = D; g.M = (int)M; g.N = D; g.K = D;
-    g.bias = w.bo; g.out = e->X; g.ldo = D; g.epi = EPI_BIAS_RESID_F32;
-    g.xb_out = e->Xn; g.stats_out = e->stats; g.n_tiles_used = &np;
+    // compact copies of the pooled rows: attention output -> head of the (now free) QKV buffer, residual rows behind it
+    __nv_bfloat16* ao_p = e->QKV;
+    float* x_p = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(e->QKV) + (((size_t)n_seq * D * 2 + 1023) & ~(size_t)1023));
     {
-      ProfScope ps(e, st, PK_OUT, 2.0 * dM * dD * dD, b_out);
-      if (int rc = launch_gemm(g, st)) return rc;
+      ProfScope ps(e, st, PK_MISC, 0, (double)n_seq * D * 12);
+      if (int rc = launch_gather_rows(e->AO, e->X, pool_idx, S, n_seq, D, ao_p, x_p, st)) return rc;
     }
-    // x = x + fc2(quick_gelu(fc1(LN2(x))))                                TF:modeling_clip.py:379-382
-    g = GemmArgs();
-    g.f16 = e->f16;
-    g.A = e->Xn; g.lda = D; g.W = w.w1; g.ldw = D; g.M = (int)M; g.N = FF; g.K = D;
-    g.bias = w.b1; g.colsum = w.s1; g.stats_in = e->stats; g.n_partials = np;
-    g.out = e->H; g.ldo = FF; g.epi = EPI_LN_BIAS_GELU_BF16;
-    {
-      ProfScope ps(e, st, PK_FC1, 2.0 * dM * dD * dF, b_fc1);
-      if (int rc = launch_gemm(g, st)) return rc;
-    }
-    g = GemmArgs();
-    g.f16 = e->f16;
-    g.A = e->H; g.lda = FF; g.W = w.w2; g.ldw = FF; g.M = (int)M; g.N = D; g.K = FF;
-    g.bias = w.b2; g.out = e->X; g.ldo = D; g.epi = EPI_BIAS_RESID_F32;
-    if (l + 1 < num_layers) {  // the last layer's output only feeds the pooled-row LayerNorm (fp32 X)
-      g.xb_out = e->Xn; g.stats_out = e->stats; g.n_tiles_used = &np;
-    }
-    {
-      ProfScope ps(e, st, PK_FC2, 2.0 * dM * dD * dF, b_fc2);
-      if (int rc = launch_gemm(g, st)) return rc;
-    }
+    if (int rc = layer_tail(e, w, (int)n_seq, D, FF, ao_p, x_p, true, np, st)) return rc;
+    e->pooled_x = x_p;
   }
   return 0;
 }
@@ -388,15 +374,10 @@ int vision_trunk(plip_engine* e, const void* pixels, int fmt, int64_t mb, int nu
     if (int rc = launch_im2col(pixels, fmt, mb, e->H, e->f16, st)) return rc;
   }
   GemmArgs g;
-  g.f16 = e->f16;
   g.A = e->H; g.lda = kPatchK; g.W = e->v_patch_w; g.ldw = kPatchK;
   g.M = (int)(mb * kPatches); g.N = kVisDim; g.K = kPatchK;
   g.out = e->X; g.ldo = kVisDim; g.pos = e->v_pos; g.epi = EPI_PATCH_F32;
-  {
-    ProfScope ps(e, st, PK_PATCH, 2.0 * dmb * kPatches * kVisDim * kPatchK,
-                 dmb * kPatches * kPatchK * 2 + (double)kVisDim * kPatchK * 2 + dmb * kPatches * kVisDim * 4);
-    if (int rc = launch_gemm(g, st)) return rc;
-  }
+  if (int rc = gemm(e, PK_PATCH, g, st)) return rc;
   {
     ProfScope ps(e, st, PK_MISC, 0, dmb * kVisDim * 4);
     if (int rc = launch_cls_rows(e->v_cls, e->v_pos, mb, e->X, st)) return rc;
@@ -409,29 +390,33 @@ int vision_trunk(plip_engine* e, const void* pixels, int fmt, int64_t mb, int nu
   return run_layers(e, e->vis, mb, kVisSeq, kVisDim, kVisFF, kVisHeads, false, nullptr, num_layers, st, prune, nullptr);
 }
 
-int vision_forward(plip_engine* e, const void* pixels, int fmt, int64_t mb, float* out, int normalize,
-                   cudaStream_t st) {
-  if (int rc = vision_trunk(e, pixels, fmt, mb, kLayers, st, e->prune_last != 0)) return rc;
-  // pooled = post_layernorm(last_hidden_state[:, 0, :])                  TF:modeling_clip.py:685-686
+// Tower head: LayerNorm of the pooled rows -> projection [-> L2 normalise].  The pooled rows are the compact
+// e->pooled_x rows when the last layer was pruned, else rows pool_idx[i] of X (null: row i*S).
+int pooled_head(plip_engine* e, const int32_t* pool_idx, int64_t mb, int S, int D, const float* gamma,
+                const float* beta, const __nv_bfloat16* proj, float* out, int normalize, cudaStream_t st) {
   {
-    ProfScope ps(e, st, PK_LN, 0, (double)mb * kVisDim * 6);
-    const float* src = e->pooled_x ? e->pooled_x : e->X;  // compact CLS rows when the last layer was pruned
-    if (int rc = launch_layernorm(src, nullptr, e->pooled_x ? (int64_t)kVisDim : (int64_t)kVisSeq * kVisDim, mb, kVisDim,
-                                  e->v_post_g, e->v_post_b, nullptr, e->pooled, e->f16, st)) return rc;
+    ProfScope ps(e, st, PK_LN, 0, (double)mb * D * 6);
+    const bool compact = e->pooled_x != nullptr;
+    if (int rc = launch_layernorm(compact ? e->pooled_x : e->X, compact ? nullptr : pool_idx,
+                                  compact || pool_idx ? (int64_t)D : (int64_t)S * D, mb, D, gamma, beta, nullptr,
+                                  e->pooled, e->f16, st)) return rc;
   }
   GemmArgs g;
-  g.f16 = e->f16;
-  g.A = e->pooled; g.lda = kVisDim; g.W = e->v_proj; g.ldw = kVisDim;
-  g.M = (int)mb; g.N = kProj; g.K = kVisDim; g.out = out; g.ldo = kProj; g.epi = EPI_F32;
-  {
-    ProfScope ps(e, st, PK_PROJ, 2.0 * (double)mb * kProj * kVisDim, (double)mb * (kVisDim * 2 + kProj * 4) + (double)kProj * kVisDim * 2);
-    if (int rc = launch_gemm(g, st)) return rc;
-  }
+  g.A = e->pooled; g.lda = D; g.W = proj; g.ldw = D;
+  g.M = (int)mb; g.N = kProj; g.K = D; g.out = out; g.ldo = kProj; g.epi = EPI_F32;
+  if (int rc = gemm(e, PK_PROJ, g, st)) return rc;
   if (normalize) {
     ProfScope ps(e, st, PK_MISC, 0, (double)mb * kProj * 8);
     return launch_l2_normalize(out, mb, kProj, st);
   }
   return 0;
+}
+
+int vision_forward(plip_engine* e, const void* pixels, int fmt, int64_t mb, float* out, int normalize,
+                   cudaStream_t st) {
+  if (int rc = vision_trunk(e, pixels, fmt, mb, kLayers, st, e->prune_last != 0)) return rc;
+  // pooled = post_layernorm(last_hidden_state[:, 0, :])                  TF:modeling_clip.py:685-686
+  return pooled_head(e, nullptr, mb, kVisSeq, kVisDim, e->v_post_g, e->v_post_b, e->v_proj, out, normalize, st);
 }
 
 // S = number of leading token positions actually processed (<= stride, the row length of ids / mask).
@@ -457,25 +442,7 @@ int text_forward(plip_engine* e, const void* ids, int ids_dtype, const void* mas
                  float* out, int normalize, cudaStream_t st) {
   if (int rc = text_trunk(e, ids, ids_dtype, mask, mb, S, stride, kLayers, st, e->prune_last != 0)) return rc;
   // pooled = final_layer_norm(last_hidden_state)[b, first eos]            TF:modeling_clip.py:562-584
-  {
-    ProfScope ps(e, st, PK_LN, 0, (double)mb * kTxtDim * 6);
-    const float* src = e->pooled_x ? e->pooled_x : e->X;  // compact EOS rows when the last layer was pruned
-    if (int rc = launch_layernorm(src, e->pooled_x ? nullptr : e->row_idx, kTxtDim, mb, kTxtDim, e->t_fin_g, e->t_fin_b,
-                                  nullptr, e->pooled, e->f16, st)) return rc;
-  }
-  GemmArgs g;
-  g.f16 = e->f16;
-  g.A = e->pooled; g.lda = kTxtDim; g.W = e->t_proj; g.ldw = kTxtDim;
-  g.M = (int)mb; g.N = kProj; g.K = kTxtDim; g.out = out; g.ldo = kProj; g.epi = EPI_F32;
-  {
-    ProfScope ps(e, st, PK_PROJ, 2.0 * (double)mb * kProj * kTxtDim, (double)mb * (kTxtDim * 2 + kProj * 4) + (double)kProj * kTxtDim * 2);
-    if (int rc = launch_gemm(g, st)) return rc;
-  }
-  if (normalize) {
-    ProfScope ps(e, st, PK_MISC, 0, (double)mb * kProj * 8);
-    return launch_l2_normalize(out, mb, kProj, st);
-  }
-  return 0;
+  return pooled_head(e, e->row_idx, mb, S, kTxtDim, e->t_fin_g, e->t_fin_b, e->t_proj, out, normalize, st);
 }
 
 int ensure_host_path(plip_engine* e) {
@@ -575,20 +542,41 @@ bool is_pinned(const void* p) {
 
 namespace {
 
-// Capture `body` (stream-ordered launches on e->s_cap, nothing executes) into an executable graph.
+// Kernel nodes of a captured graph.
+int count_kernel_nodes(cudaGraph_t g, unsigned long long* kernels) {
+  size_t n = 0;
+  PLIP_CUDA_CHECK(cudaGraphGetNodes(g, nullptr, &n));
+  std::vector<cudaGraphNode_t> nodes(n);
+  PLIP_CUDA_CHECK(cudaGraphGetNodes(g, nodes.data(), &n));
+  *kernels = 0;
+  for (cudaGraphNode_t node : nodes) {
+    cudaGraphNodeType type;
+    PLIP_CUDA_CHECK(cudaGraphNodeGetType(node, &type));
+    *kernels += type == cudaGraphNodeTypeKernel;
+  }
+  return 0;
+}
+
+// Capture `body` (stream-ordered launches on e->s_cap, nothing executes) into an executable graph.  The captured
+// launches were counted by launch_kernel but do not run: they come off g_launch_count and are added per replay.
 template <typename F>
-int capture_graph(plip_engine* e, F&& body, cudaGraphExec_t* out) {
+int capture_graph(plip_engine* e, F&& body, Graph* out) {
   if (!e->s_cap) PLIP_CUDA_CHECK(cudaStreamCreateWithFlags(&e->s_cap, cudaStreamNonBlocking));
   PLIP_CUDA_CHECK(cudaStreamBeginCapture(e->s_cap, cudaStreamCaptureModeThreadLocal));
-  const int rc = body(e->s_cap);
+  int rc = body(e->s_cap);
   cudaGraph_t g = nullptr;
   const cudaError_t ce = cudaStreamEndCapture(e->s_cap, &g);
+  if (g) {
+    const int rc_count = count_kernel_nodes(g, &out->kernels);
+    if (rc == 0) rc = rc_count;
+    g_launch_count.fetch_sub(out->kernels, std::memory_order_relaxed);
+  }
   if (rc != 0) {
     if (g) cudaGraphDestroy(g);
     return rc;
   }
   PLIP_CUDA_CHECK(ce);
-  const cudaError_t ci = cudaGraphInstantiate(out, g, 0);
+  const cudaError_t ci = cudaGraphInstantiate(&out->exec, g, 0);
   cudaGraphDestroy(g);
   PLIP_CUDA_CHECK(ci);
   return 0;
@@ -603,8 +591,46 @@ constexpr size_t kMaxGraphs = 96;
 void trim_graphs(plip_engine* e) {
   if (e->graphs.size() < kMaxGraphs) return;
   cudaDeviceSynchronize();  // none of them may still be running
-  for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);
+  for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);
   e->graphs.clear();
+}
+
+// A caller's input buffer of a graph-replayed call (src null: absent); input i is staged in e->g_in[i].
+struct Staged {
+  const void* src;
+  size_t bytes;
+};
+
+// Small-batch path (graph_eligible): the first call of a key runs forward(stream, in0, in1, out) eagerly on the
+// caller's buffers, which also configures every kernel, then records it as a graph on the staging buffers.  Later
+// calls copy the inputs in, replay the graph and copy the [n, 512] result out.
+template <typename F>
+int graph_call(plip_engine* e, const GraphKey& key, std::array<Staged, 2> in, float* out, cudaStream_t st,
+               F&& forward) {
+  auto it = e->graphs.find(key);
+  if (it == e->graphs.end()) {
+    const size_t stage_bytes[2] = {(size_t)e->graph_max_n * pixel_bytes(PLIP_PIX_F32_NCHW),
+                                   (size_t)e->graph_max_n * kTxtSeq * 8};
+    for (int i = 0; i < 2; ++i)
+      if (in[i].src)
+        if (int rc = grow_dev(&e->g_in[i], &e->g_in_bytes[i], stage_bytes[i])) return rc;
+    if (!e->g_out) PLIP_CUDA_CHECK(cudaMalloc(&e->g_out, (size_t)e->graph_max_n * kProj * 4));
+    if (int rc = forward(st, in[0].src, in[1].src, out)) return rc;
+    Graph graph;
+    if (int rc = capture_graph(e, [&](cudaStream_t cs) {
+          return forward(cs, in[0].src ? e->g_in[0] : nullptr, in[1].src ? e->g_in[1] : nullptr, e->g_out);
+        }, &graph)) return rc;
+    trim_graphs(e);
+    e->graphs.emplace(key, graph);
+  } else {
+    for (int i = 0; i < 2; ++i)
+      if (in[i].src) PLIP_CUDA_CHECK(cudaMemcpyAsync(e->g_in[i], in[i].src, in[i].bytes, cudaMemcpyDeviceToDevice, st));
+    PLIP_CUDA_CHECK(cudaGraphLaunch(it->second.exec, st));
+    PLIP_CUDA_CHECK(cudaMemcpyAsync(out, e->g_out, (size_t)key.n * kProj * 4, cudaMemcpyDeviceToDevice, st));
+    g_launch_count.fetch_add(it->second.kernels, std::memory_order_relaxed);
+  }
+  PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
+  return 0;
 }
 
 }  // namespace
@@ -616,7 +642,7 @@ extern "C" {
 
 PLIP_API const char* plip_last_error(void) { return plip::get_last_error(); }
 PLIP_API int plip_abi_version(void) { return PLIP_B200_ABI_VERSION; }
-PLIP_API uint64_t plip_launch_count(void) { return plip::g_launch_count; }
+PLIP_API uint64_t plip_launch_count(void) { return plip::g_launch_count.load(std::memory_order_relaxed); }
 
 PLIP_API int plip_weights_num_tensors(void) { return (int)specs().size(); }
 
@@ -718,9 +744,9 @@ PLIP_API int plip_destroy(plip_engine_t* e) {
   if (e->d_out) cudaFree(e->d_out);
   if (e->d_aux) cudaFree(e->d_aux);
   if (e->ev_last) cudaEventDestroy(e->ev_last);
-  for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);
-  if (e->g_in) cudaFree(e->g_in);
-  if (e->g_mask) cudaFree(e->g_mask);
+  for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);
+  for (void* p : e->g_in)
+    if (p) cudaFree(p);
   if (e->g_out) cudaFree(e->g_out);
   if (e->s_cap) cudaStreamDestroy(e->s_cap);
   for (cudaEvent_t ev : e->prof_ev) cudaEventDestroy(ev);
@@ -793,25 +819,11 @@ PLIP_API int plip_encode_images(plip_engine_t* e, const void* pixels_dev, int pi
   PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_last, 0));  // calls on different streams share one workspace
   const size_t pb = pixel_bytes(pixel_format);
   if (graph_eligible(e, n)) {
-    const auto key = std::make_tuple(0 + 4 * e->prune_last, (int)n, pixel_format, normalize ? 1 : 0, 0, 0, 0);
-    auto it = e->graphs.find(key);
-    if (it == e->graphs.end()) {
-      // first call of this shape: run it eagerly (this also configures every kernel), then record the graph
-      if (int rc = grow_dev(&e->g_in, &e->g_in_bytes, (size_t)e->graph_max_n * pixel_bytes(PLIP_PIX_F32_NCHW))) return rc;
-      if (!e->g_out) PLIP_CUDA_CHECK(cudaMalloc(&e->g_out, (size_t)e->graph_max_n * kProj * 4));
-      if (int rc = vision_forward(e, pixels_dev, pixel_format, n, out_dev, normalize, st)) return rc;
-      cudaGraphExec_t ge = nullptr;
-      if (int rc = capture_graph(e, [&](cudaStream_t cs) { return vision_forward(e, e->g_in, pixel_format, n, e->g_out, normalize, cs); }, &ge)) return rc;
-      trim_graphs(e);
-      e->graphs.emplace(key, ge);
-    } else {
-      PLIP_CUDA_CHECK(cudaMemcpyAsync(e->g_in, pixels_dev, (size_t)n * pb, cudaMemcpyDeviceToDevice, st));
-      PLIP_CUDA_CHECK(cudaGraphLaunch(it->second, st));
-      PLIP_CUDA_CHECK(cudaMemcpyAsync(out_dev, e->g_out, (size_t)n * kProj * 4, cudaMemcpyDeviceToDevice, st));
-      g_launch_count += 67 + e->prune_last;
-    }
-    PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
-    return 0;
+    const GraphKey key{0, (int)n, pixel_format, normalize ? 1 : 0, 0, 0, 0, 0, e->prune_last};
+    return graph_call(e, key, {{{pixels_dev, (size_t)n * pb}, {nullptr, 0}}}, out_dev, st,
+                      [&](cudaStream_t s, const void* pixels, const void*, float* out) {
+                        return vision_forward(e, pixels, pixel_format, n, out, normalize, s);
+                      });
   }
   for (int64_t i = 0; i < n; i += e->max_mb) {
     const int64_t mb = (n - i < e->max_mb) ? (n - i) : e->max_mb;
@@ -843,32 +855,13 @@ PLIP_API int plip_encode_text_prefix(plip_engine_t* e, const void* ids_dev, int 
   PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_last, 0));
   const size_t isz = ids_dtype == PLIP_IDS_I64 ? 8 : 4;
   if (graph_eligible(e, n)) {
-    // everything a captured launch sequence bakes in is part of the key (incl. the pooling convention)
-    const auto key = std::make_tuple(1 + 2 * e->text_pool_argmax + 4 * e->prune_last, (int)n, ids_dtype, normalize ? 1 : 0, seq_len, prefix_len,
-                                     attention_mask_dev ? 1 : 0);
+    const GraphKey key{1, (int)n, ids_dtype, normalize ? 1 : 0, seq_len, prefix_len, attention_mask_dev ? 1 : 0,
+                       e->text_pool_argmax, e->prune_last};
     const size_t ib = (size_t)n * seq_len * isz;
-    auto it = e->graphs.find(key);
-    if (it == e->graphs.end()) {
-      if (int rc = grow_dev(&e->g_in, &e->g_in_bytes, (size_t)e->graph_max_n * pixel_bytes(PLIP_PIX_F32_NCHW))) return rc;
-      if (int rc = grow_dev(&e->g_mask, &e->g_mask_bytes, (size_t)e->graph_max_n * kTxtSeq * 8)) return rc;
-      if (!e->g_out) PLIP_CUDA_CHECK(cudaMalloc(&e->g_out, (size_t)e->graph_max_n * kProj * 4));
-      if (int rc = text_forward(e, ids_dev, ids_dtype, attention_mask_dev, n, prefix_len, seq_len, out_dev, normalize, st)) return rc;
-      cudaGraphExec_t ge = nullptr;
-      if (int rc = capture_graph(e, [&](cudaStream_t cs) {
-            return text_forward(e, e->g_in, ids_dtype, attention_mask_dev ? e->g_mask : nullptr, n, prefix_len, seq_len,
-                                e->g_out, normalize, cs);
-          }, &ge)) return rc;
-      trim_graphs(e);
-      e->graphs.emplace(key, ge);
-    } else {
-      PLIP_CUDA_CHECK(cudaMemcpyAsync(e->g_in, ids_dev, ib, cudaMemcpyDeviceToDevice, st));
-      if (attention_mask_dev) PLIP_CUDA_CHECK(cudaMemcpyAsync(e->g_mask, attention_mask_dev, ib, cudaMemcpyDeviceToDevice, st));
-      PLIP_CUDA_CHECK(cudaGraphLaunch(it->second, st));
-      PLIP_CUDA_CHECK(cudaMemcpyAsync(out_dev, e->g_out, (size_t)n * kProj * 4, cudaMemcpyDeviceToDevice, st));
-      g_launch_count += 66 + e->prune_last;
-    }
-    PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
-    return 0;
+    return graph_call(e, key, {{{ids_dev, ib}, {attention_mask_dev, ib}}}, out_dev, st,
+                      [&](cudaStream_t s, const void* ids, const void* mask, float* out) {
+                        return text_forward(e, ids, ids_dtype, mask, n, prefix_len, seq_len, out, normalize, s);
+                      });
   }
   for (int64_t i = 0; i < n; i += e->max_mb) {
     const int64_t mb = (n - i < e->max_mb) ? (n - i) : e->max_mb;

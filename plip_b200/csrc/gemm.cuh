@@ -52,7 +52,4 @@ struct GemmArgs {
 // Enqueue the GEMM on `stream`.  Returns 0 on success (see last_error otherwise).
 int launch_gemm(const GemmArgs& g, cudaStream_t stream);
 
-// Number of kernel launches issued by this translation unit since load (bench accounting).
-extern unsigned long long g_launch_count;
-
 }  // namespace plip

@@ -25,8 +25,6 @@
 
 namespace plip {
 
-unsigned long long g_launch_count = 0;
-
 namespace {
 
 constexpr int BM = 128;  // rows per CTA tile: 64 per consumer warpgroup
@@ -401,7 +399,6 @@ int launch_inst(const GemmArgs& g, cudaStream_t stream) {
   const int num_tiles = ((g.M + BM * CG - 1) / (BM * CG)) * (g.N / BN);
   const int groups = max_groups < num_tiles ? max_groups : num_tiles;
   PLIP_CUDA_CHECK(launch_kernel(kern, dim3(groups * CG), dim3(kThreads), C::SMEM_BYTES, stream, CG, tmA, tmB, tmC, p));
-  ++g_launch_count;
   return 0;
 }
 

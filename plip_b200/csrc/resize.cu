@@ -367,7 +367,6 @@ int launch_resize_crop(const uint8_t* src, size_t src_bytes, const plip_resize_d
     }
     PLIP_CUDA_CHECK(launch_kernel(resize_crop_kernel, dim3(kImage / kRsRowsPerCta, cnt), dim3(kRsThreads), smem, st, 1,
                                src, (uint64_t)src_bytes, tiles, b, base));
-    ++g_launch_count;
   }
   return 0;
 }

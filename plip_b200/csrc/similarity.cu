@@ -4,13 +4,13 @@
 // and the numpy heads  key.dot(space.T) + argmax / argsort top-k
 //   (plip.py:73-87,99-102; evaluation/zero_shot/zero_shot.py:12-13; evaluation/retrieval/retrieval.py:13-16).
 //
-// The [n,512] x [m,512]^T product is kept in fp32 FMA arithmetic (K = 512 only): the |dlogits| <= 1e-3
-// bar at logit scales up to 100 rules out 16-bit operands (SURVEY.md §7).  The row norms are
-// accumulated from the same operand tiles that feed the product, so each input is read once per tile.
+// The [n,512] x [m,512]^T product needs fp32-class accuracy: the |dlogits| <= 1e-3 bar at logit scales up to 100
+// rules out plain 16-bit operands (SURVEY.md §7).  Wide score matrices and big top-k problems run it on the tensor
+// cores with operands split into fp16 hi + lo parts; the other cases use fp32 FMA kernels that accumulate the row
+// norms from the same operand tiles that feed the product, so each input is read once per tile.
 #include "kernels.cuh"
 
 #include <cuda_fp16.h>
-#include <stdlib.h>
 
 #include <mutex>
 
@@ -402,14 +402,61 @@ split_embed_kernel(const float* __restrict__ x, int64_t n, int64_t n_pad, int no
   }
 }
 
-// grow-only per-device scratch for the split operands and the scale vectors (plip_similarity has no engine handle)
-struct SimScratch {
+// Grow-only per-device scratch: these entry points have no engine handle to hang a workspace on, and nothing is
+// allocated once the buffers are warm.  A lease holds its slot's lock for the whole call, so concurrent calls on
+// different streams take turns; the stream waits for the previous user's kernels, and the lease records the slot's
+// event for the next one when it ends.  Each pool has its own lock, so one lease may enclose a lease of another pool.
+struct ScratchSlot {
+  std::mutex mu;
   void* p = nullptr;
   size_t bytes = 0;
   cudaEvent_t ev = nullptr;
 };
-SimScratch g_sim_pool[64];
-std::mutex g_sim_mu;
+using ScratchPool = ScratchSlot[64];
+
+class ScratchLease {
+ public:
+  ScratchLease(ScratchPool& pool, cudaStream_t st) : st_(st) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    slot_ = &pool[dev & 63];
+    slot_->mu.lock();
+  }
+  ~ScratchLease() {
+    if (acquired_) cudaEventRecord(slot_->ev, st_);
+    slot_->mu.unlock();
+  }
+  ScratchLease(const ScratchLease&) = delete;
+  ScratchLease& operator=(const ScratchLease&) = delete;
+
+  // At least `bytes` of scratch at *out; a buffer that is too small is replaced (by one 1.5x as large with `slack`)
+  // once its last user has finished.
+  int acquire(size_t bytes, void** out, bool slack = false) {
+    ScratchSlot& s = *slot_;
+    if (!s.ev) PLIP_CUDA_CHECK(cudaEventCreateWithFlags(&s.ev, cudaEventDisableTiming));
+    if (s.bytes < bytes) {
+      if (s.p) {
+        PLIP_CUDA_CHECK(cudaEventSynchronize(s.ev));
+        PLIP_CUDA_CHECK(cudaFree(s.p));
+        s.p = nullptr; s.bytes = 0;
+      }
+      const size_t want = slack ? bytes + bytes / 2 : bytes;
+      PLIP_CUDA_CHECK(cudaMalloc(&s.p, want));
+      s.bytes = want;
+    }
+    PLIP_CUDA_CHECK(cudaStreamWaitEvent(st_, s.ev, 0));
+    acquired_ = true;
+    *out = s.p;
+    return 0;
+  }
+
+ private:
+  ScratchSlot* slot_ = nullptr;
+  cudaStream_t st_;
+  bool acquired_ = false;
+};
+
+ScratchPool g_sim_pool, g_topk_tc_pool, g_topk_tiled_pool;
 
 constexpr int64_t kSimRowChunk = 131072;  // A rows split + multiplied per pass (403 MB of fp16 operand scratch)
 
@@ -418,23 +465,10 @@ int launch_similarity_tc(const float* a, int64_t n, const float* b, int64_t m, f
   const int64_t m_pad = (m + 127) / 128 * 128;
   const int64_t rows = n < kSimRowChunk ? n : kSimRowChunk;
   const size_t bytes_b = (size_t)m_pad * kSplitK * 2, bytes_a = (size_t)rows * kSplitK * 2;
-  const size_t want = bytes_b + bytes_a + (size_t)(m_pad + rows) * 4 + 1024;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  std::lock_guard<std::mutex> lk(g_sim_mu);
-  SimScratch& sc = g_sim_pool[dev & 63];
-  if (!sc.ev) PLIP_CUDA_CHECK(cudaEventCreateWithFlags(&sc.ev, cudaEventDisableTiming));
-  if (sc.bytes < want) {
-    if (sc.p) {
-      PLIP_CUDA_CHECK(cudaEventSynchronize(sc.ev));
-      PLIP_CUDA_CHECK(cudaFree(sc.p));
-      sc.p = nullptr; sc.bytes = 0;
-    }
-    PLIP_CUDA_CHECK(cudaMalloc(&sc.p, want));
-    sc.bytes = want;
-  }
-  PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, sc.ev, 0));
-  uint8_t* base = static_cast<uint8_t*>(sc.p);
+  ScratchLease lease(g_sim_pool, st);
+  void* scratch = nullptr;
+  if (int rc = lease.acquire(bytes_b + bytes_a + (size_t)(m_pad + rows) * 4 + 1024, &scratch)) return rc;
+  uint8_t* base = static_cast<uint8_t*>(scratch);
   __half* bsplit = reinterpret_cast<__half*>(base);
   __half* asplit = reinterpret_cast<__half*>(base + bytes_b);
   float* cscale = reinterpret_cast<float*>(base + bytes_b + bytes_a);
@@ -443,12 +477,10 @@ int launch_similarity_tc(const float* a, int64_t n, const float* b, int64_t m, f
   auto grid_for_rows = [row_grid_cap](int64_t r) { int64_t g = (r + 7) / 8; return (int)(g < 1 ? 1 : (g > row_grid_cap ? row_grid_cap : g)); };
   PLIP_CUDA_CHECK(launch_kernel(split_embed_kernel, dim3(grid_for_rows(m_pad)), dim3(256), 0, st, 1, b, m, m_pad,
                                 norm_b ? 1 : 0, 1, 1.0f, bsplit, cscale));
-  ++g_launch_count;
   for (int64_t i = 0; i < n; i += rows) {
     const int64_t cnt = n - i < rows ? n - i : rows;
     PLIP_CUDA_CHECK(launch_kernel(split_embed_kernel, dim3(grid_for_rows(cnt)), dim3(256), 0, st, 1, a + i * kProj, cnt, cnt,
                                   norm_a ? 1 : 0, 0, scale, asplit, rscale));
-    ++g_launch_count;
     GemmArgs g;
     g.f16 = 1;
     g.A = reinterpret_cast<const __nv_bfloat16*>(asplit); g.lda = kSplitK;
@@ -458,7 +490,6 @@ int launch_similarity_tc(const float* a, int64_t n, const float* b, int64_t m, f
     g.out = out + i * ldo; g.ldo = (int)ldo; g.epi = EPI_SIM_F32;
     if (int rc = launch_gemm(g, st)) return rc;
   }
-  PLIP_CUDA_CHECK(cudaEventRecord(sc.ev, st));
   return 0;
 }
 
@@ -523,8 +554,6 @@ rowwise_topk_merge_kernel(const float* __restrict__ S, int64_t n, int64_t cols, 
   }
 }
 
-SimScratch g_topk_tc_pool[64];
-
 int launch_similarity_topk_tc(const float* q, int64_t n, const float* s, int64_t m, float scale, bool norm_q,
                               bool norm_s, int k, int32_t* idx, float* val, cudaStream_t st) {
   // chunk of the space: <= 256 MB of fp32 scores for all n queries, a multiple of 256 columns
@@ -533,35 +562,18 @@ int launch_similarity_topk_tc(const float* q, int64_t n, const float* s, int64_t
   if (gc > 32768) gc = 32768;
   if (gc > (m + 255) / 256 * 256) gc = (m + 255) / 256 * 256;
   const size_t score_bytes = (size_t)n * gc * 4, val_bytes = val ? 0 : (size_t)n * k * 4;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  SimScratch& sc = g_topk_tc_pool[dev & 63];
-  {
-    std::lock_guard<std::mutex> lk(g_sim_mu);
-    if (!sc.ev) PLIP_CUDA_CHECK(cudaEventCreateWithFlags(&sc.ev, cudaEventDisableTiming));
-    if (sc.bytes < score_bytes + val_bytes + 256) {
-      if (sc.p) {
-        PLIP_CUDA_CHECK(cudaEventSynchronize(sc.ev));
-        PLIP_CUDA_CHECK(cudaFree(sc.p));
-        sc.p = nullptr; sc.bytes = 0;
-      }
-      PLIP_CUDA_CHECK(cudaMalloc(&sc.p, score_bytes + val_bytes + 256));
-      sc.bytes = score_bytes + val_bytes + 256;
-    }
-    PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, sc.ev, 0));
-  }
-  float* scores = static_cast<float*>(sc.p);
-  float* vals = val ? val : reinterpret_cast<float*>(static_cast<uint8_t*>(sc.p) + score_bytes);
+  ScratchLease lease(g_topk_tc_pool, st);
+  void* scratch = nullptr;
+  if (int rc = lease.acquire(score_bytes + val_bytes + 256, &scratch)) return rc;
+  float* scores = static_cast<float*>(scratch);
+  float* vals = val ? val : reinterpret_cast<float*>(static_cast<uint8_t*>(scratch) + score_bytes);
   const unsigned grid = (unsigned)((n + kMergeWarps - 1) / kMergeWarps);
   for (int64_t c0 = 0; c0 < m; c0 += gc) {
     const int64_t cols = m - c0 < gc ? m - c0 : gc;
     if (int rc = launch_similarity_tc(q, n, s + c0 * kProj, cols, scale, norm_q, norm_s, scores, gc, st)) return rc;
     PLIP_CUDA_CHECK(launch_kernel(rowwise_topk_merge_kernel, dim3(grid), dim3(kMergeWarps * 32), 0, st, 1, scores, n, cols,
                                   gc, c0, k, c0 == 0 ? 1 : 0, idx, vals));
-    ++g_launch_count;
   }
-  std::lock_guard<std::mutex> lk(g_sim_mu);
-  PLIP_CUDA_CHECK(cudaEventRecord(sc.ev, st));
   return 0;
 }
 
@@ -575,17 +587,15 @@ int launch_similarity(const float* a, int64_t n, const float* b, int64_t m, floa
                (reinterpret_cast<uintptr_t>(out) & 15) == 0, "similarity: operands must be 16-byte aligned");
   // Tensor-core path for wide score matrices (>= 256 columns) whenever the output rows can take the 128-column
   // padding of the GEMM tile (plip_b200's own callers allocate ld_logits that way).
-  static const int sim_simt = [] { const char* v = getenv("PLIP_SIM_SIMT"); return (v && v[0] == '1') ? 1 : 0; }();
   const int64_t m_pad = (m + 127) / 128 * 128;
   // (the choice depends on m only, so a row-sharded call computes bit-identical rows to the unsharded one)
-  if (!sim_simt && m >= 256 && ldo >= m_pad && ldo % 4 == 0 && ldo < 0x7fffffff)
+  if (m >= 256 && ldo >= m_pad && ldo % 4 == 0 && ldo < 0x7fffffff)
     return launch_similarity_tc(a, n, b, m, scale, norm_a, norm_b, out, ldo, st);
   const int64_t gy = (n + TM - 1) / TM, gx = (m + TN - 1) / TN;
   PLIP_REQUIRE(gy <= 65535, "similarity: n=%lld too large for one launch (chunk rows)", (long long)n);
   dim3 grid((unsigned)gx, (unsigned)gy);
   PLIP_CUDA_CHECK(launch_kernel(similarity_kernel, grid, dim3(kSimThreads), 0, st, 1, a, n, b, m, (int)kProj, scale,
                              norm_a ? 1 : 0, norm_b ? 1 : 0, out, ldo));
-  ++g_launch_count;
   return 0;
 }
 
@@ -594,14 +604,12 @@ int launch_similarity_topk(const float* q, int64_t n, const float* s, int64_t m,
   PLIP_REQUIRE(n > 0 && m > 0, "similarity_topk: empty operand");
   PLIP_REQUIRE(k >= 1 && k <= kTopkMax, "similarity_topk: k=%d out of range [1,%d]", k, kTopkMax);
   PLIP_REQUIRE(n <= 0x7fffffff && m <= 0x7fffffff, "similarity_topk: operand too large");
-  static const int topk_simt = [] { const char* v = getenv("PLIP_SIM_SIMT"); return (v && v[0] == '1') ? 1 : 0; }();
-  if (!topk_simt && n >= 256 && m >= 8192)  // big retrieval problems: scores from the tensor cores, chunk by chunk
+  if (n >= 256 && m >= 8192)  // big retrieval problems: scores from the tensor cores, chunk by chunk
     return launch_similarity_topk_tc(q, n, s, m, scale, norm_q, norm_s, k, idx, val, st);
   if (n * m < (int64_t)1 << 16) {
     // tiny problems (e.g. a handful of class prompts): one CTA per query streaming the space
     PLIP_CUDA_CHECK(launch_kernel(similarity_topk_kernel, dim3((unsigned)n), dim3(kTopkThreads), 0, st, 1, q, n, s, m,
                                (int)kProj, scale, norm_q ? 1 : 0, norm_s ? 1 : 0, k, idx, val));
-    ++g_launch_count;
     return 0;
   }
   static unsigned long long configured = 0;
@@ -621,48 +629,20 @@ int launch_similarity_topk(const float* q, int64_t n, const float* s, int64_t m,
   float* scratch_v = nullptr;
   int* scratch_i = nullptr;
   unsigned* tickets = nullptr;
-  if (splits > 1) {
-    // Partial lists of the space splits: a per-device buffer that only ever grows (no allocation once warm;
-    // this function has no engine handle to hang a workspace on).  Calls that share it are ordered by `ev`.
-    struct Scratch { void* p = nullptr; size_t bytes = 0; cudaEvent_t ev = nullptr; };
-    static Scratch pool[64];
-    static std::mutex mu;
+  ScratchLease lease(g_topk_tiled_pool, st);
+  if (splits > 1) {  // partial lists of the space splits + one merge ticket per query tile
     const size_t ent = (size_t)splits * row_tiles * TM * k;
-    const size_t bytes = ent * 8 + (size_t)row_tiles * 4;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    std::lock_guard<std::mutex> lk(mu);
-    Scratch& sc = pool[dev & 63];
-    if (!sc.ev) PLIP_CUDA_CHECK(cudaEventCreateWithFlags(&sc.ev, cudaEventDisableTiming));
-    if (sc.bytes < bytes) {
-      if (sc.p) {
-        PLIP_CUDA_CHECK(cudaEventSynchronize(sc.ev));  // last user of the old buffer
-        PLIP_CUDA_CHECK(cudaFree(sc.p));
-        sc.p = nullptr; sc.bytes = 0;
-      }
-      const size_t want = bytes + bytes / 2;
-      PLIP_CUDA_CHECK(cudaMalloc(&sc.p, want));
-      sc.bytes = want;
-    }
-    PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, sc.ev, 0));  // a call on another stream may still be merging
-    void* scratch = sc.p;
+    void* scratch = nullptr;
+    if (int rc = lease.acquire(ent * 8 + (size_t)row_tiles * 4, &scratch, true)) return rc;
     scratch_v = static_cast<float*>(scratch);
     scratch_i = reinterpret_cast<int*>(scratch_v + ent);
     tickets = reinterpret_cast<unsigned*>(scratch_i + ent);
     PLIP_CUDA_CHECK(cudaMemsetAsync(tickets, 0, (size_t)row_tiles * 4, st));
-    dim3 grid((unsigned)row_tiles, (unsigned)splits);
-    PLIP_CUDA_CHECK(launch_kernel(similarity_topk_tiled_kernel, grid, dim3(kTkThreads), smem, st, 1, q, n, s, m, (int)kProj,
-                               scale, norm_q ? 1 : 0, norm_s ? 1 : 0, k, tiles_per_split, scratch_v, scratch_i, tickets,
-                               idx, val));
-    PLIP_CUDA_CHECK(cudaEventRecord(sc.ev, st));
-    ++g_launch_count;
-    return 0;
   }
   dim3 grid((unsigned)row_tiles, (unsigned)splits);
   PLIP_CUDA_CHECK(launch_kernel(similarity_topk_tiled_kernel, grid, dim3(kTkThreads), smem, st, 1, q, n, s, m, (int)kProj,
                              scale, norm_q ? 1 : 0, norm_s ? 1 : 0, k, tiles_per_split, scratch_v, scratch_i, tickets,
                              idx, val));
-  ++g_launch_count;
   return 0;
 }
 
