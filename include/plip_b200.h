@@ -124,6 +124,18 @@ PLIP_API int plip_last_layer_pruning(const plip_engine_t* e);
 PLIP_API int plip_encode_images(plip_engine_t* e, const void* pixels_dev, int pixel_format, int64_t n,
                                 float* out_dev, int normalize, void* stream);
 
+/* Same at any image size: CLIPModel.get_image_features(pixel_values, interpolate_pos_encoding=True) (TF:161-218,
+ * 832-856).  pixels_dev holds n images of height x width in pixel_format ([n,3,H,W] or [n,H,W,3] for u8).  The patch
+ * grid is gh = height / 32 by gw = width / 32 (remainder pixels on the right and bottom are ignored, as by the
+ * stride-32 conv), S = gh * gw + 1 tokens, and the 7 x 7 position table is resized to gh x gw bicubically (A = -0.75,
+ * align_corners = False, as F.interpolate).  Requires 32 <= height, width and gh, gw <= 32 (up to 1024 pixels per side),
+ * and S <= 50 * max_micro_batch (the workspace's token rows): a pass holds min(max_micro_batch,
+ * floor(50 * max_micro_batch / S)) images.  A 7 x 7 grid uses the stored table, so 224 <= height, width <= 255 give
+ * exactly the 224 x 224 result; 224 x 224 is plip_encode_images itself.  Sequences longer than 128 tokens (more than
+ * 8 x 16 patches) run the long-sequence attention kernel (profile role "vision/attention[long]"). */
+PLIP_API int plip_encode_images_hw(plip_engine_t* e, const void* pixels_dev, int pixel_format, int64_t n, int height,
+                                   int width, float* out_dev, int normalize, void* stream);
+
 /* Text tower + text_projection: replaces CLIPModel.get_text_features (TF:793-825, called at
  * plip.py:68) and model.encode_text (embedders/plip.py:66).
  * ids_dev: [n,seq_len] token ids (seq_len <= 77); attention_mask_dev: optional [n,seq_len] of the
@@ -234,9 +246,17 @@ PLIP_API int plip_dbg_rowstats_cast(const float* x, int64_t rows, int dim, void*
 PLIP_API int plip_dbg_layernorm(const float* x, int64_t rows, int dim, int64_t in_row_stride,
                                 const float* gamma, const float* beta, float* out_f32, void* out_bf16,
                                 void* stream);
+/* seq_len <= 128: any causal / key_mask; 128 < seq_len <= 1025 (long-sequence kernel): causal = 0, key_mask = NULL. */
 PLIP_API int plip_dbg_attention(const void* qkv_bf16, int64_t n_seq, int seq_len, int heads, int causal,
                                 const int32_t* key_mask, void* out_bf16, void* stream);
 PLIP_API int plip_dbg_im2col(const void* pixels, int pixel_format, int64_t n, void* out_bf16, void* stream);
+/* The vision position table pos_dev (float32 [50,768]) resized to a grid_h x grid_w patch grid as
+ * plip_encode_images_hw does it: out_dev float32 [1 + grid_h * grid_w, 768]; 1 <= grid_h, grid_w <= 32. */
+PLIP_API int plip_dbg_pos_interp(const float* pos_dev, int grid_h, int grid_w, float* out_dev, void* stream);
+/* Vision tower at any image size (plip_encode_images_hw geometry): the fp32 residual stream [n*S, 768] after
+ * `num_layers` layers; n must fit one pass. */
+PLIP_API int plip_dbg_hidden_states_hw(plip_engine_t* e, const void* pixels_dev, int pixel_format, int64_t n,
+                                       int height, int width, int num_layers, float* hidden_dev, void* stream);
 /* Run one tower and copy the fp32 residual stream [n*S, D] after `num_layers` encoder layers
  * (0 = after embeddings / pre-LN) into hidden_dev.  tower: 0 = vision (input pixels), 1 = text. */
 PLIP_API int plip_dbg_hidden_states(plip_engine_t* e, int tower, const void* input_dev, int input_format,

@@ -74,6 +74,7 @@ SIGNATURES = {
     "plip_logit_scale_exp": (_f, [_vp]),
     "plip_max_micro_batch": (_i, [_vp]),
     "plip_encode_images": (_i, [_vp, _vp, _i, _i64, _fp, _i, _vp]),
+    "plip_encode_images_hw": (_i, [_vp, _vp, _i, _i64, _i, _i, _fp, _i, _vp]),
     "plip_encode_text": (_i, [_vp, _vp, _i, _vp, _i64, _i, _fp, _i, _vp]),
     "plip_encode_text_prefix": (_i, [_vp, _vp, _i, _vp, _i64, _i, _i, _fp, _i, _vp]),
     "plip_similarity": (_i, [_fp, _i64, _fp, _i64, _f, _i, _i, _fp, _i64, _vp]),
@@ -92,6 +93,8 @@ SIGNATURES = {
     "plip_dbg_attention": (_i, [_vp, _i64, _i, _i, _i, _vp, _vp, _vp]),
     "plip_dbg_im2col": (_i, [_vp, _i, _i64, _vp, _vp]),
     "plip_dbg_hidden_states": (_i, [_vp, _i, _vp, _i, _vp, _i64, _i, _fp, _vp]),
+    "plip_dbg_pos_interp": (_i, [_fp, _i, _i, _fp, _vp]),
+    "plip_dbg_hidden_states_hw": (_i, [_vp, _vp, _i, _i64, _i, _i, _i, _fp, _vp]),
 }
 
 _LIB = None

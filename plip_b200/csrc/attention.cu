@@ -18,6 +18,7 @@
 //            sequence
 // One CTA runs this chain serially per tile; with 48 KB of operands several CTAs co-reside per SM and hide each
 // other's load -> MMA -> softmax -> MMA -> store latency.
+// Sequences longer than 128 (vision at more than 256 x 256 pixels) go to attention_long_kernel below.
 #include "kernels.cuh"
 #include "wgmma.cuh"
 
@@ -228,13 +229,234 @@ int launch_attention_inst(const CUtensorMap& tmL, const CUtensorMap& tmS, const 
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Long sequences (S > 128: vision at more than 256 x 256 pixels, interpolated position table), non-causal and
+// unmasked only.  Flash-style online softmax over blocks of 64 keys, one CTA per (sequence, head, 128-query block):
+//   warp 8       producer: TMA of the Q block (once) and of the K / V blocks into a two-stage ring (full / empty
+//                mbarriers), so block j + 1 lands while block j is multiplied
+//   warpgroups   each owns 64 query rows:  S = Q K^T (wgmma m64n64k16, ss) -> keys >= S masked to -inf -> running
+//   0 - 1        row max / sum in fp32 (O rescaled by 2^(m_old - m_new)) -> P packed straight into the A fragments
+//                of O += P V (wgmma rs, P never leaves the registers) -> after the last block O / l -> 16 bit -> the
+//                warpgroup's own Q rows -> one TMA store
+// The 3-D tensor maps ([n_seq][S][cols], box {64, rows, 1}) zero-fill rows past a sequence's end on load and clip
+// them on store: no tail code, and no row of the next sequence is read or written.  Key blocks are consumed in a
+// fixed order: the result is bitwise reproducible.
+constexpr int kLongThreads = 288;                 // two consumer warpgroups + one producer warp
+constexpr int kLongKeys = 64;                     // keys per block
+constexpr uint32_t kLongQBytes = 128 * 64 * 2;    // [128 queries x 64 dh]
+constexpr uint32_t kLongKVBytes = kLongKeys * 64 * 2;
+constexpr int kLongStages = 2;
+constexpr uint32_t kLongSmem = kLongQBytes + kLongStages * 2 * kLongKVBytes + 1024 + 64;
+
+struct LongAttParams {
+  int seq_len;
+  int heads;
+  int q_blocks;  // ceil(S / 128)
+};
+
+template <bool F16>
+__global__ void __launch_bounds__(kLongThreads, 2)
+attention_long_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmO,
+                      const LongAttParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t sq = smem_base;
+  auto sk = [&](int s) { return smem_base + kLongQBytes + (uint32_t)s * 2u * kLongKVBytes; };
+  auto sv = [&](int s) { return sk(s) + kLongKVBytes; };
+  const uint32_t bar = smem_base + kLongQBytes + kLongStages * 2 * kLongKVBytes;
+  const uint32_t q_bar = bar;
+  auto full_bar = [&](int s) { return bar + 8u * (1 + s); };
+  auto empty_bar = [&](int s) { return bar + 8u * (1 + kLongStages + s); };
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int wg = warp >> 2;
+  const int S = p.seq_len, D = p.heads * kHeadDim;
+  const int qb = blockIdx.x % p.q_blocks;
+  const int bh = blockIdx.x / p.q_blocks;
+  const int h = bh % p.heads;
+  const int seq = bh / p.heads;
+  const int q0 = qb * 128;
+  const int n_kb = (S + kLongKeys - 1) / kLongKeys;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmQKV);
+    tma_prefetch_desc(&tmO);
+    mbar_init(q_bar, 1);
+    for (int s = 0; s < kLongStages; ++s) {
+      mbar_init(full_bar(s), 1);
+      mbar_init(empty_bar(s), 2);  // one arrive per consumer warpgroup
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (wg == 2) {
+    // ===================== TMA producer =====================
+    if (lane == 0) {
+      mbar_arrive_expect_tx(q_bar, kLongQBytes);
+      tma_load_3d(sq, &tmQKV, q_bar, h * kHeadDim, q0, seq);
+      tma_load_3d(sq + kLongQBytes / 2, &tmQKV, q_bar, h * kHeadDim, q0 + 64, seq);
+      for (int kb = 0; kb < n_kb; ++kb) {
+        const int s = kb % kLongStages;
+        if (kb >= kLongStages) mbar_wait(empty_bar(s), (uint32_t)((kb / kLongStages - 1) & 1));
+        mbar_arrive_expect_tx(full_bar(s), 2 * kLongKVBytes);
+        tma_load_3d(sk(s), &tmQKV, full_bar(s), D + h * kHeadDim, kb * kLongKeys, seq);
+        tma_load_3d(sv(s), &tmQKV, full_bar(s), 2 * D + h * kHeadDim, kb * kLongKeys, seq);
+      }
+    }
+    return;
+  }
+
+  // ===================== consumers =====================
+  const int q4 = lane & 3, rr = lane >> 2;
+  const int R0 = 64 * wg + 16 * (warp & 3) + rr;  // this thread's tile rows R0 and R0 + 8
+  constexpr float kLog2e = 1.4426950408889634f;
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY;  // running row max (raw scores)
+  float l0 = 0.f, l1 = 0.f;              // this thread's share of the running row sum
+  const uint64_t qdesc = make_smem_desc_sw128(sq + wg * (64 * 128), 1024, 16);
+  mbar_wait(q_bar, 0);
+
+  for (int kb = 0; kb < n_kb; ++kb) {
+    const int s = kb % kLongStages;
+    mbar_wait(full_bar(s), (uint32_t)((kb / kLongStages) & 1));
+
+    // ---- S = Q K^T
+    float sc[32];
+    {
+      const uint64_t kdesc = make_smem_desc_sw128(sk(s), 1024, 16);
+      wgmma_pin(sc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kHeadDim / 16; ++k) wgmma_ss_n64<F16>(sc, qdesc + 2 * k, kdesc + 2 * k, k != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_pin(sc);
+    }
+
+    // ---- online softmax on the registers
+    const int kbase = kb * kLongKeys + 2 * q4;  // + 8 j + e = key of column (j, e)
+    if (kb * kLongKeys + kLongKeys > S) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (kbase + 8 * j + e >= S) {
+            sc[4 * j + e] = -INFINITY;
+            sc[4 * j + 2 + e] = -INFINITY;
+          }
+    }
+    float mx0 = m0, mx1 = m1;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      mx0 = fmaxf(mx0, fmaxf(sc[4 * j + 0], sc[4 * j + 1]));
+      mx1 = fmaxf(mx1, fmaxf(sc[4 * j + 2], sc[4 * j + 3]));
+    }
+#pragma unroll
+    for (int off = 1; off < 4; off <<= 1) {  // the 4 lanes that share a row
+      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, off));
+      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, off));
+    }
+    // every block holds at least one real key, so mx is finite; m_old = -inf (first block) gives alpha = 0
+    const float ms0 = mx0 * kLog2e, ms1 = mx1 * kLog2e;
+    const float alpha0 = fast_exp2(fmaf(m0, kLog2e, -ms0)), alpha1 = fast_exp2(fmaf(m1, kLog2e, -ms1));
+    m0 = mx0;
+    m1 = mx1;
+    l0 *= alpha0;
+    l1 *= alpha1;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      o[4 * j + 0] *= alpha0; o[4 * j + 1] *= alpha0;
+      o[4 * j + 2] *= alpha1; o[4 * j + 3] *= alpha1;
+    }
+    uint32_t pa[4][4];  // P as the A fragments of O += P V: k-step kk covers keys 16 kk .. 16 kk + 15 of the block
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float e00 = fast_exp2(fmaf(sc[4 * j + 0], kLog2e, -ms0)), e01 = fast_exp2(fmaf(sc[4 * j + 1], kLog2e, -ms0));
+      const float e10 = fast_exp2(fmaf(sc[4 * j + 2], kLog2e, -ms1)), e11 = fast_exp2(fmaf(sc[4 * j + 3], kLog2e, -ms1));
+      l0 += e00 + e01;
+      l1 += e10 + e11;
+      pa[j >> 1][2 * (j & 1) + 0] = pack_op2<F16>(e00, e01);
+      pa[j >> 1][2 * (j & 1) + 1] = pack_op2<F16>(e10, e11);
+    }
+
+    // ---- O += P V   (V block [keys][64 dh]: advancing 16 keys = 16 rows of 128 B)
+    wgmma_pin(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kLongKeys / 16; ++kk) {
+      const uint64_t vdesc = make_smem_desc_sw128(sv(s) + 16 * kk * 128, 1024, 1024);
+      wgmma_rs_n64<F16>(o, pa[kk], vdesc, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_pin(o);
+    if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar(s));  // this warpgroup is done with K / V of the stage
+  }
+
+  // ---- epilogue: O / l -> 16 bit -> this warpgroup's Q rows (swizzled like a TMA box) -> one TMA store
+#pragma unroll
+  for (int off = 1; off < 4; off <<= 1) {
+    l0 += __shfl_xor_sync(0xffffffffu, l0, off);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, off);
+  }
+  const float inv0 = l0 > 0.f ? 1.0f / l0 : 0.f;
+  const float inv1 = l1 > 0.f ? 1.0f / l1 : 0.f;
+  const uint32_t row0 = sq + static_cast<uint32_t>(R0) * 128u, row1 = row0 + 8u * 128u;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    st_shared_b32(row0 + ((j ^ rr) << 4) + q4 * 4, pack_op2<F16>(o[4 * j + 0] * inv0, o[4 * j + 1] * inv0));
+    st_shared_b32(row1 + ((j ^ rr) << 4) + q4 * 4, pack_op2<F16>(o[4 * j + 2] * inv1, o[4 * j + 3] * inv1));
+  }
+  fence_proxy_async_smem();
+  if (wg == 0) named_barrier_sync<1, 128>();  // the warpgroup's 64 output rows are staged
+  else named_barrier_sync<2, 128>();
+  if ((threadIdx.x & 127) == 0 && q0 + 64 * wg < S) {
+    tma_store_3d(&tmO, sq + wg * (64 * 128), h * kHeadDim, q0 + 64 * wg, seq);
+    tma_store_commit();
+    tma_store_wait_all();
+  }
+}
+
+template <bool F16>
+int launch_attention_long(const CUtensorMap& tmQKV, const CUtensorMap& tmO, const LongAttParams& p, int64_t blocks,
+                          cudaStream_t st) {
+  auto kern = attention_long_kernel<F16>;
+  static unsigned long long configured = 0;
+  if (first_use_on_device(configured))
+    PLIP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLongSmem));
+  PLIP_CUDA_CHECK(launch_kernel(kern, dim3((unsigned)blocks), dim3(kLongThreads), kLongSmem, st, 1, tmQKV, tmO, p));
+  return 0;
+}
+
 }  // namespace
 
 int launch_attention(const __nv_bfloat16* qkv, int64_t n_seq, int seq_len, int heads, bool causal,
                      const int32_t* key_mask, __nv_bfloat16* out, int f16, cudaStream_t st) {
-  PLIP_REQUIRE(n_seq > 0 && seq_len > 0 && seq_len <= 128, "attention: bad shape n_seq=%lld seq_len=%d",
+  PLIP_REQUIRE(n_seq > 0 && seq_len > 0 && seq_len <= kMaxVisSeq, "attention: bad shape n_seq=%lld seq_len=%d",
                (long long)n_seq, seq_len);
   PLIP_REQUIRE(heads > 0 && heads <= 16, "attention: bad head count %d", heads);
+  if (seq_len > 128) {
+    PLIP_REQUIRE(!causal && key_mask == nullptr,
+                 "attention: seq_len %d > 128 is supported without causal or key mask only", seq_len);
+    const int D = heads * kHeadDim;
+    LongAttParams p;
+    p.seq_len = seq_len;
+    p.heads = heads;
+    p.q_blocks = (seq_len + 127) / 128;
+    const int64_t blocks = n_seq * heads * p.q_blocks;
+    PLIP_REQUIRE(blocks < 0x7fffffff && n_seq < 0x7fffffff, "attention: too many sequences");
+    CUtensorMap tmQKV, tmO;
+    if (int rc = make_tmap_bf16_3d(&tmQKV, qkv, (uint64_t)n_seq, (uint64_t)seq_len, (uint64_t)3 * D,
+                                   (uint64_t)3 * D * 2, (uint64_t)seq_len * 3 * D * 2, 64, 64)) return rc;
+    if (int rc = make_tmap_bf16_3d(&tmO, out, (uint64_t)n_seq, (uint64_t)seq_len, (uint64_t)D, (uint64_t)D * 2,
+                                   (uint64_t)seq_len * D * 2, 64, 64)) return rc;
+    return f16 ? launch_attention_long<true>(tmQKV, tmO, p, blocks, st)
+               : launch_attention_long<false>(tmQKV, tmO, p, blocks, st);
+  }
   const int D = heads * kHeadDim;
   const int64_t rows = n_seq * seq_len;
   PLIP_REQUIRE(rows + 128 < 0x7fffffff, "attention: too many token rows");

@@ -23,6 +23,9 @@ constexpr int kPatch = 32;
 constexpr int kGrid = 7;           // 224 / 32
 constexpr int kPatches = 49;
 constexpr int kVisSeq = 50;        // 49 patches + class token
+// Inputs other than 224 x 224 (interpolated position table): patch grid gh x gw up to kMaxGrid per side.
+constexpr int kMaxGrid = 32;       // 1024 pixels
+constexpr int kMaxVisSeq = kMaxGrid * kMaxGrid + 1;
 constexpr int kVisDim = 768;
 constexpr int kVisHeads = 12;
 constexpr int kVisFF = 3072;
@@ -88,6 +91,11 @@ inline int sm_count() {
 // box: box_cols (must be 64 bf16 == 128 B for SWIZZLE_128B) x box_rows (<=256).
 int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
                       uint64_t row_stride_bytes, uint32_t box_rows, uint32_t box_cols);
+// Encode a 3-D bf16 tensor map [mats][rows][cols] with 128-byte swizzle and a {box_cols, box_rows, 1} box: a box
+// that reaches past `rows` is zero-filled on load and clipped on store inside its own matrix, never spilling into the
+// next one.
+int make_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t mats, uint64_t rows, uint64_t cols,
+                      uint64_t row_stride_bytes, uint64_t mat_stride_bytes, uint32_t box_rows, uint32_t box_cols);
 
 #ifdef __CUDACC__
 
@@ -251,6 +259,27 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, uint32_t sme
                    reinterpret_cast<uint64_t>(tm)),
                "r"(smem_src), "r"(c0), "r"(c1)
                : "memory");
+}
+// 3-D tile load / store (make_tmap_bf16_3d maps): c0 column, c1 row inside matrix c2.
+__device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const CUtensorMap* tm, uint32_t bar, int32_t c0,
+                                            int32_t c1, int32_t c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%3, %4, %5}], [%2];"
+      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* tm, uint32_t smem_src, int32_t c0, int32_t c1,
+                                             int32_t c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(tm)),
+               "r"(smem_src), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+// Barrier over THREADS threads of the CTA (a warpgroup), ID 1..15 (0 is __syncthreads).
+template <int ID, int THREADS>
+__device__ __forceinline__ void named_barrier_sync() {
+  asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(THREADS) : "memory");
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // all committed store groups have finished READING their shared-memory source

@@ -24,32 +24,50 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8], int f16) {
 // Restates nn.Conv2d(3,768,32,32,bias=False) input gathering (TF:modeling_clip.py:148-154,209-210);
 // the uint8 path fuses CLIPImageProcessor's rescale + normalise (TF:image_processing_clip.py:50-62).
 // One thread moves 8 consecutive x of one image row.
+// Any image size (interpolated position table): the image is H x W, the patch grid gh x gw (the H % 32 bottom rows
+// and W % 32 right columns are never read, as with the stride-32 conv).  FIXED = the 224 x 224 geometry as
+// compile-time constants.  vec = 0 (rows whose start is not aligned for the vector loads, e.g. W = 250): the same
+// pixels read one value at a time.
 // ------------------------------------------------------------------------------------------------
-template <int FMT>
+struct ImGeom {
+  int H, W, gh, gw;
+};
+
+template <int FMT, bool FIXED>
 __global__ void __launch_bounds__(kEwThreads) im2col_kernel(const void* __restrict__ pixels,
-                                                            __nv_bfloat16* __restrict__ out, int64_t n, int f16) {
-  constexpr int kX8 = kImage / 8;  // 28 groups of 8 pixels per image row
-  const int64_t total = (FMT == PLIP_PIX_U8_NHWC) ? n * kImage * kX8 : n * 3 * kImage * kX8;
+                                                            __nv_bfloat16* __restrict__ out, int64_t n, int f16,
+                                                            ImGeom geo, int vec) {
+  const int H = FIXED ? kImage : geo.H, W = FIXED ? kImage : geo.W;
+  const int gw = FIXED ? kGrid : geo.gw, patches = FIXED ? kPatches : geo.gh * geo.gw;
+  const int rows = FIXED ? kImage : geo.gh * 32;  // image rows that reach a patch
+  const int kX8 = FIXED ? kImage / 8 : geo.gw * 4;  // groups of 8 pixels per image row (28 at 224)
+  const bool vload = FIXED || vec != 0;
+  const int64_t total = (FMT == PLIP_PIX_U8_NHWC) ? n * rows * kX8 : n * 3 * rows * kX8;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
        i += (int64_t)gridDim.x * blockDim.x) {
     const int x8 = (int)(i % kX8);
     int64_t r = i / kX8;
-    const int y = (int)(r % kImage);
-    r /= kImage;
+    const int y = (int)(r % rows);
+    r /= rows;
     const int x = x8 * 8;
     const int py = y >> 5, ky = y & 31, px = x >> 5, kx = x & 31;
     if constexpr (FMT == PLIP_PIX_U8_NHWC) {
       const int64_t b = r;
-      const uint8_t* src = static_cast<const uint8_t*>(pixels) + ((b * kImage + y) * kImage + x) * 3;
-      const uint2* s2 = reinterpret_cast<const uint2*>(src);  // 24 bytes, 8-byte aligned
-      uint2 w0 = __ldg(s2), w1 = __ldg(s2 + 1), w2 = __ldg(s2 + 2);
+      const uint8_t* src = static_cast<const uint8_t*>(pixels) + ((b * H + y) * W + x) * 3;
       uint8_t bytes[24];
-      *reinterpret_cast<uint2*>(bytes) = w0;
-      *reinterpret_cast<uint2*>(bytes + 8) = w1;
-      *reinterpret_cast<uint2*>(bytes + 16) = w2;
+      if (vload) {
+        const uint2* s2 = reinterpret_cast<const uint2*>(src);  // 24 bytes, 8-byte aligned
+        uint2 w0 = __ldg(s2), w1 = __ldg(s2 + 1), w2 = __ldg(s2 + 2);
+        *reinterpret_cast<uint2*>(bytes) = w0;
+        *reinterpret_cast<uint2*>(bytes + 8) = w1;
+        *reinterpret_cast<uint2*>(bytes + 16) = w2;
+      } else {
+#pragma unroll
+        for (int j = 0; j < 24; ++j) bytes[j] = __ldg(src + j);
+      }
       const float mean[3] = {0.48145466f, 0.4578275f, 0.40821073f};
       const float istd[3] = {1.0f / 0.26862954f, 1.0f / 0.26130258f, 1.0f / 0.27577711f};
-      __nv_bfloat16* dst = out + (b * kPatches + py * kGrid + px) * (int64_t)kPatchK + ky * 32 + kx;
+      __nv_bfloat16* dst = out + (b * patches + py * gw + px) * (int64_t)kPatchK + ky * 32 + kx;
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
         float f[8];
@@ -60,16 +78,33 @@ __global__ void __launch_bounds__(kEwThreads) im2col_kernel(const void* __restri
     } else {
       const int c = (int)(r % 3);
       const int64_t b = r / 3;
-      const int64_t src_off = ((b * 3 + c) * kImage + y) * kImage + x;
+      const int64_t src_off = ((b * 3 + c) * H + y) * W + x;
       __nv_bfloat16* dst =
-          out + (b * kPatches + py * kGrid + px) * (int64_t)kPatchK + c * 1024 + ky * 32 + kx;
+          out + (b * patches + py * gw + px) * (int64_t)kPatchK + c * 1024 + ky * 32 + kx;
       if constexpr (FMT == PLIP_PIX_F32_NCHW) {
-        const float4* s4 = reinterpret_cast<const float4*>(static_cast<const float*>(pixels) + src_off);
-        const float4 a = __ldg(s4), bq = __ldg(s4 + 1);
-        const float f[8] = {a.x, a.y, a.z, a.w, bq.x, bq.y, bq.z, bq.w};
+        const float* s = static_cast<const float*>(pixels) + src_off;
+        float f[8];
+        if (vload) {
+          const float4* s4 = reinterpret_cast<const float4*>(s);
+          const float4 a = __ldg(s4), bq = __ldg(s4 + 1);
+          f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = bq.x; f[5] = bq.y; f[6] = bq.z; f[7] = bq.w;
+        } else {
+#pragma unroll
+          for (int j = 0; j < 8; ++j) f[j] = __ldg(s + j);
+        }
         *reinterpret_cast<uint4*>(dst) = pack8(f, f16);
       } else {  // bf16 NCHW: straight 16-byte copy (re-rounded to half for the fp16 operand format)
-        uint4 w = __ldg(reinterpret_cast<const uint4*>(static_cast<const __nv_bfloat16*>(pixels) + src_off));
+        const __nv_bfloat16* s = static_cast<const __nv_bfloat16*>(pixels) + src_off;
+        uint4 w;
+        if (vload) {
+          w = __ldg(reinterpret_cast<const uint4*>(s));
+        } else {
+          const unsigned short* s16 = reinterpret_cast<const unsigned short*>(s);
+          uint32_t u[4];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) u[j] = (uint32_t)__ldg(s16 + 2 * j) | ((uint32_t)__ldg(s16 + 2 * j + 1) << 16);
+          w = make_uint4(u[0], u[1], u[2], u[3]);
+        }
         if (f16) {
           const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&w);
           float f[8];
@@ -257,9 +292,9 @@ __global__ void __launch_bounds__(kEwThreads) mask_to_i32_kernel(const IdT* __re
     out[i] = m[(i / seq_len) * stride + (i % seq_len)] != 0 ? 1 : 0;
 }
 
-// Class-token rows: x[b*50] = class_embedding + position_embedding[0]   (TF:212-217).
+// Class-token rows: x[b*S] = class_embedding + position_embedding[0]   (TF:212-217), S = 50 at 224 x 224.
 __global__ void __launch_bounds__(kEwThreads) cls_rows_kernel(const float* __restrict__ cls,
-                                                              const float* __restrict__ pos, int64_t n,
+                                                              const float* __restrict__ pos, int64_t n, int seq,
                                                               float* __restrict__ x) {
   constexpr int V = kVisDim / 4;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n * V;
@@ -268,8 +303,53 @@ __global__ void __launch_bounds__(kEwThreads) cls_rows_kernel(const float* __res
     const int j = (int)(i % V);
     const float4 c = __ldg(reinterpret_cast<const float4*>(cls) + j);
     const float4 p = __ldg(reinterpret_cast<const float4*>(pos) + j);
-    reinterpret_cast<float4*>(x + b * kVisSeq * kVisDim)[j] =
+    reinterpret_cast<float4*>(x + b * seq * kVisDim)[j] =
         make_float4(c.x + p.x, c.y + p.y, c.z + p.z, c.w + p.w);
+  }
+}
+
+// Position table of a gh x gw patch grid (TF:modeling_clip.py:161-200, interpolate_pos_encoding): row 0 (class) is
+// copied; rows 1..49 of the stored table, viewed as [768, 7, 7], are resized to [768, gh, gw] the way
+// F.interpolate(mode="bicubic", align_corners=False) does it: cubic convolution with A = -0.75, source coordinate
+// (i + 0.5) * 7 / g - 0.5, taps clamped to [0, 6], no antialias; out row 1 + y * gw + x.  One thread per output value.
+__device__ __forceinline__ void cubic_taps(int g, int i, int (&idx)[4], float (&w)[4]) {
+  constexpr float A = -0.75f;
+  const float scale = (float)kGrid / (float)g;
+  const float real = scale * ((float)i + 0.5f) - 0.5f;
+  const float fl = floorf(real);
+  const float t = real - fl;
+  const float t1 = t + 1.f, t2 = 1.f - t, t3 = 2.f - t;
+  w[0] = ((A * t1 - 5.f * A) * t1 + 8.f * A) * t1 - 4.f * A;
+  w[1] = ((A + 2.f) * t - (A + 3.f)) * t * t + 1.f;
+  w[2] = ((A + 2.f) * t2 - (A + 3.f)) * t2 * t2 + 1.f;
+  w[3] = ((A * t3 - 5.f * A) * t3 + 8.f * A) * t3 - 4.f * A;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) idx[k] = min(max((int)fl - 1 + k, 0), kGrid - 1);
+}
+
+__global__ void __launch_bounds__(kEwThreads) pos_interp_kernel(const float* __restrict__ pos, int gh, int gw,
+                                                                float* __restrict__ out) {
+  const int total = (1 + gh * gw) * kVisDim;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    const int row = i / kVisDim, c = i - row * kVisDim;
+    if (row == 0) {
+      out[i] = __ldg(pos + c);
+      continue;
+    }
+    const int y = (row - 1) / gw, x = (row - 1) - y * gw;
+    int iy[4], ix[4];
+    float wy[4], wx[4];
+    cubic_taps(gh, y, iy, wy);
+    cubic_taps(gw, x, ix, wx);
+    float acc = 0.f;
+#pragma unroll
+    for (int a = 0; a < 4; ++a) {
+      float t = 0.f;
+#pragma unroll
+      for (int b = 0; b < 4; ++b) t += __ldg(pos + (size_t)(1 + iy[a] * kGrid + ix[b]) * kVisDim + c) * wx[b];
+      acc += t * wy[a];
+    }
+    out[i] = acc;
   }
 }
 
@@ -316,17 +396,43 @@ inline int grid_for(int64_t work_items, int per_block) {
 
 }  // namespace
 
-int launch_im2col(const void* pixels, int fmt, int64_t n, __nv_bfloat16* out, int f16, cudaStream_t st) {
+int launch_im2col(const void* pixels, int fmt, int64_t n, int height, int width, __nv_bfloat16* out, int f16,
+                  cudaStream_t st) {
   PLIP_REQUIRE(n > 0, "im2col: n must be positive");
-  PLIP_REQUIRE((reinterpret_cast<uintptr_t>(pixels) & 15) == 0, "im2col: pixels must be 16-byte aligned");
-  const int64_t items = (fmt == PLIP_PIX_U8_NHWC ? 1 : 3) * n * kImage * (kImage / 8);
+  PLIP_REQUIRE(height >= kPatch && width >= kPatch && height / kPatch <= kMaxGrid && width / kPatch <= kMaxGrid,
+               "im2col: image size %dx%d out of range", height, width);
+  const bool fixed = height == kImage && width == kImage;
+  const uintptr_t addr = reinterpret_cast<uintptr_t>(pixels);
+  PLIP_REQUIRE(!fixed || (addr & 15) == 0, "im2col: pixels must be 16-byte aligned");
+  // vector loads need every row start aligned: f32 16 B (W % 4 == 0), bf16 16 B (W % 8), u8 8 B (3 W % 8)
+  const bool aligned = (addr & (fmt == PLIP_PIX_U8_NHWC ? 7 : 15)) == 0;
+  const int vec = aligned && width % (fmt == PLIP_PIX_F32_NCHW ? 4 : 8) == 0 ? 1 : 0;
+  const ImGeom geo{height, width, height / kPatch, width / kPatch};
+  const int64_t items = (fmt == PLIP_PIX_U8_NHWC ? 1 : 3) * n * (geo.gh * 32) * (geo.gw * 4);
   const int grid = grid_for(items, kEwThreads);
+#define PLIP_IM2COL(F)                                                                                                 \
+  PLIP_CUDA_CHECK(fixed ? launch_kernel(im2col_kernel<F, true>, dim3(grid), dim3(kEwThreads), 0, st, 1, pixels, out, n, \
+                                        f16, geo, vec)                                                                 \
+                        : launch_kernel(im2col_kernel<F, false>, dim3(grid), dim3(kEwThreads), 0, st, 1, pixels, out,  \
+                                        n, f16, geo, vec))
   switch (fmt) {
-    case PLIP_PIX_F32_NCHW: PLIP_CUDA_CHECK(launch_kernel(im2col_kernel<PLIP_PIX_F32_NCHW>, dim3(grid), dim3(kEwThreads), 0, st, 1, pixels, out, n, f16)); break;
-    case PLIP_PIX_BF16_NCHW: PLIP_CUDA_CHECK(launch_kernel(im2col_kernel<PLIP_PIX_BF16_NCHW>, dim3(grid), dim3(kEwThreads), 0, st, 1, pixels, out, n, f16)); break;
-    case PLIP_PIX_U8_NHWC: PLIP_CUDA_CHECK(launch_kernel(im2col_kernel<PLIP_PIX_U8_NHWC>, dim3(grid), dim3(kEwThreads), 0, st, 1, pixels, out, n, f16)); break;
+    case PLIP_PIX_F32_NCHW: PLIP_IM2COL(PLIP_PIX_F32_NCHW); break;
+    case PLIP_PIX_BF16_NCHW: PLIP_IM2COL(PLIP_PIX_BF16_NCHW); break;
+    case PLIP_PIX_U8_NHWC: PLIP_IM2COL(PLIP_PIX_U8_NHWC); break;
     default: set_last_error("im2col: unknown pixel format %d", fmt); return -2;
   }
+#undef PLIP_IM2COL
+  PLIP_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+int launch_pos_interp(const float* pos, int gh, int gw, float* out, cudaStream_t st) {
+  PLIP_REQUIRE(pos && out, "pos_interp: null argument");
+  PLIP_REQUIRE(gh >= 1 && gw >= 1 && gh <= kMaxGrid && gw <= kMaxGrid, "pos_interp: grid %dx%d out of [1,%d]", gh, gw,
+               kMaxGrid);
+  const int64_t items = (int64_t)(1 + gh * gw) * kVisDim;
+  PLIP_CUDA_CHECK(launch_kernel(pos_interp_kernel, dim3(grid_for(items, kEwThreads)), dim3(kEwThreads), 0, st, 1, pos,
+                                gh, gw, out));
   PLIP_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -395,8 +501,8 @@ int launch_mask_to_i32(const void* mask, int dtype, int64_t count, int seq_len, 
   return 0;
 }
 
-int launch_cls_rows(const float* cls, const float* pos, int64_t n, float* x, cudaStream_t st) {
-  PLIP_CUDA_CHECK(launch_kernel(cls_rows_kernel, dim3(grid_for(n * (kVisDim / 4), kEwThreads)), dim3(kEwThreads), 0, st, 1, cls, pos, n, x));
+int launch_cls_rows(const float* cls, const float* pos, int64_t n, int seq, float* x, cudaStream_t st) {
+  PLIP_CUDA_CHECK(launch_kernel(cls_rows_kernel, dim3(grid_for(n * (kVisDim / 4), kEwThreads)), dim3(kEwThreads), 0, st, 1, cls, pos, n, seq, x));
   PLIP_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

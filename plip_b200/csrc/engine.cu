@@ -107,14 +107,33 @@ struct LayerW {
 constexpr int kEosId = 49407;  // TF:configuration_clip.py:63 (eos_token_id)
 
 enum ProfKind { PK_QKV = 0, PK_ATTN, PK_OUT, PK_FC1, PK_FC2, PK_PATCH, PK_IM2COL, PK_LN, PK_ROWSTATS, PK_EMBED, PK_PROJ,
-                PK_MISC, PK_COUNT };
+                PK_MISC, PK_ATTN_LONG, PK_COUNT };
 const char* const kProfNames[PK_COUNT] = {"gemm[ln1+qkv]", "attention", "gemm[out_proj+resid]", "gemm[ln2+fc1+gelu]",
                                           "gemm[fc2+resid]", "gemm[patch_embed]", "im2col", "layernorm",
-                                          "rowstats_cast", "text_embed", "gemm[projection]", "misc"};
+                                          "rowstats_cast", "text_embed", "gemm[projection]", "misc", "attention[long]"};
 
-size_t pixel_bytes(int fmt) {
-  const size_t px = (size_t)3 * kImage * kImage;
+size_t pixel_bytes(int fmt, int height = kImage, int width = kImage) {
+  const size_t px = (size_t)3 * height * width;
   return fmt == PLIP_PIX_F32_NCHW ? px * 4 : (fmt == PLIP_PIX_BF16_NCHW ? px * 2 : px);
+}
+
+// Input geometry of the vision tower: H x W pixels -> gh x gw patches (the H % 32 / W % 32 remainder is ignored, as by
+// the stride-32 conv), S = gh * gw + 1 tokens.  224 x 224 (7 x 7, S = 50) uses the stored position table; any other
+// grid an interpolated one (TF:modeling_clip.py:161-218, interpolate_pos_encoding).
+struct VisGeom {
+  int H = kImage, W = kImage, gh = kGrid, gw = kGrid, S = kVisSeq;
+};
+
+VisGeom vis_geom(int height, int width) {
+  VisGeom g;
+  g.H = height; g.W = width; g.gh = height / kPatch; g.gw = width / kPatch; g.S = g.gh * g.gw + 1;
+  return g;
+}
+
+// The workspace holds kVisSeq * max_mb vision token rows (and max_mb pooled rows): images per pass at S tokens each.
+int64_t images_per_pass(int max_mb, int S) {
+  const int64_t n = (int64_t)kVisSeq * max_mb / S;
+  return n < max_mb ? n : max_mb;
 }
 
 // Everything a captured launch sequence bakes in (the engine's buffers aside).  Unused fields are 0.
@@ -344,7 +363,7 @@ int run_layers(plip_engine* e, const LayerW* L, int64_t n_seq, int S, int D, int
     g.out = e->QKV; g.ldo = 3 * D; g.epi = EPI_LN_BIAS_BF16;
     if (int rc = gemm(e, PK_QKV, g, st)) return rc;
     {
-      ProfScope ps(e, st, PK_ATTN, f_att, b_att);
+      ProfScope ps(e, st, S > 128 ? PK_ATTN_LONG : PK_ATTN, f_att, b_att);
       if (int rc = launch_attention(e->QKV, n_seq, S, heads, causal, kmask, e->AO, e->f16, st)) return rc;
     }
     if (!(prune && last)) {
@@ -364,30 +383,40 @@ int run_layers(plip_engine* e, const LayerW* L, int64_t n_seq, int S, int D, int
   return 0;
 }
 
-// Vision tower up to (and including) `num_layers` encoder layers; X holds the residual stream.
-int vision_trunk(plip_engine* e, const void* pixels, int fmt, int64_t mb, int num_layers, cudaStream_t st,
-                 bool prune = false) {
+// Vision tower up to (and including) `num_layers` encoder layers; X holds the residual stream [mb * geo.S, 768].
+int vision_trunk(plip_engine* e, const void* pixels, int fmt, int64_t mb, const VisGeom& geo, int num_layers,
+                 cudaStream_t st, bool prune = false) {
   e->prof_tower = 0;
   const double dmb = (double)mb;
+  const int patches = geo.gh * geo.gw;
+  // Position table of the grid.  An interpolated one goes to the QKV buffer, which nothing reads before the first
+  // layer's QKV GEMM: [geo.S, 768] fp32 fits, since S <= kVisSeq * max_mb and QKV holds that many rows of 2 x 2304 B.
+  const float* pos = e->v_pos;
+  if (geo.gh != kGrid || geo.gw != kGrid) {
+    float* table = reinterpret_cast<float*>(e->QKV);
+    ProfScope ps(e, st, PK_MISC, 0, (double)kVisSeq * kVisDim * 4 + (double)geo.S * kVisDim * 4);
+    if (int rc = launch_pos_interp(e->v_pos, geo.gh, geo.gw, table, st)) return rc;
+    pos = table;
+  }
   {
-    ProfScope ps(e, st, PK_IM2COL, 0, dmb * (double)pixel_bytes(fmt) + dmb * kPatches * kPatchK * 2);
-    if (int rc = launch_im2col(pixels, fmt, mb, e->H, e->f16, st)) return rc;
+    ProfScope ps(e, st, PK_IM2COL, 0, dmb * (double)pixel_bytes(fmt, geo.H, geo.W) + dmb * patches * kPatchK * 2);
+    if (int rc = launch_im2col(pixels, fmt, mb, geo.H, geo.W, e->H, e->f16, st)) return rc;
   }
   GemmArgs g;
   g.A = e->H; g.lda = kPatchK; g.W = e->v_patch_w; g.ldw = kPatchK;
-  g.M = (int)(mb * kPatches); g.N = kVisDim; g.K = kPatchK;
-  g.out = e->X; g.ldo = kVisDim; g.pos = e->v_pos; g.epi = EPI_PATCH_F32;
+  g.M = (int)(mb * patches); g.N = kVisDim; g.K = kPatchK;
+  g.out = e->X; g.ldo = kVisDim; g.pos = pos; g.patches = patches; g.seq = geo.S; g.epi = EPI_PATCH_F32;
   if (int rc = gemm(e, PK_PATCH, g, st)) return rc;
   {
     ProfScope ps(e, st, PK_MISC, 0, dmb * kVisDim * 4);
-    if (int rc = launch_cls_rows(e->v_cls, e->v_pos, mb, e->X, st)) return rc;
+    if (int rc = launch_cls_rows(e->v_cls, pos, mb, geo.S, e->X, st)) return rc;
   }
-  const int64_t M = mb * kVisSeq;
+  const int64_t M = mb * geo.S;
   {
     ProfScope ps(e, st, PK_LN, 0, (double)M * kVisDim * 8);
     if (int rc = launch_layernorm(e->X, nullptr, kVisDim, M, kVisDim, e->v_pre_g, e->v_pre_b, e->X, nullptr, e->f16, st)) return rc;
   }
-  return run_layers(e, e->vis, mb, kVisSeq, kVisDim, kVisFF, kVisHeads, false, nullptr, num_layers, st, prune, nullptr);
+  return run_layers(e, e->vis, mb, geo.S, kVisDim, kVisFF, kVisHeads, false, nullptr, num_layers, st, prune, nullptr);
 }
 
 // Tower head: LayerNorm of the pooled rows -> projection [-> L2 normalise].  The pooled rows are the compact
@@ -413,10 +442,10 @@ int pooled_head(plip_engine* e, const int32_t* pool_idx, int64_t mb, int S, int 
 }
 
 int vision_forward(plip_engine* e, const void* pixels, int fmt, int64_t mb, float* out, int normalize,
-                   cudaStream_t st) {
-  if (int rc = vision_trunk(e, pixels, fmt, mb, kLayers, st, e->prune_last != 0)) return rc;
+                   cudaStream_t st, const VisGeom& geo = VisGeom()) {
+  if (int rc = vision_trunk(e, pixels, fmt, mb, geo, kLayers, st, e->prune_last != 0)) return rc;
   // pooled = post_layernorm(last_hidden_state[:, 0, :])                  TF:modeling_clip.py:685-686
-  return pooled_head(e, nullptr, mb, kVisSeq, kVisDim, e->v_post_g, e->v_post_b, e->v_proj, out, normalize, st);
+  return pooled_head(e, nullptr, mb, geo.S, kVisDim, e->v_post_g, e->v_post_b, e->v_proj, out, normalize, st);
 }
 
 // S = number of leading token positions actually processed (<= stride, the row length of ids / mask).
@@ -579,6 +608,26 @@ int capture_graph(plip_engine* e, F&& body, Graph* out) {
   const cudaError_t ci = cudaGraphInstantiate(&out->exec, g, 0);
   cudaGraphDestroy(g);
   PLIP_CUDA_CHECK(ci);
+  return 0;
+}
+
+// Arguments of a vision call at any image size (interpolate_pos_encoding): 32 <= H, W and a patch grid of at most
+// kMaxGrid x kMaxGrid, and one image's tokens must fit the workspace's kVisSeq * max_micro_batch token rows.  The
+// shape is checked before the handle, so a bad size is reported as such whatever else is wrong.
+int check_hw_call(const char* fn, const plip_engine* e, const void* in, const void* out, int fmt, int64_t n,
+                  int height, int width) {
+  PLIP_REQUIRE(in && out, "%s: null argument", fn);
+  PLIP_REQUIRE(n > 0, "%s: n must be positive (got %lld)", fn, (long long)n);
+  PLIP_REQUIRE(fmt >= 0 && fmt <= 2, "%s: unknown pixel format %d", fn, fmt);
+  PLIP_REQUIRE(height >= kPatch && width >= kPatch && height / kPatch <= kMaxGrid && width / kPatch <= kMaxGrid,
+               "%s: image size %dx%d out of range (32 <= height, width and at most %d patches of 32 per side)", fn,
+               height, width, kMaxGrid);
+  PLIP_REQUIRE(e != nullptr, "%s: null engine", fn);
+  const int S = (height / kPatch) * (width / kPatch) + 1;
+  PLIP_REQUIRE(S <= (int64_t)kVisSeq * e->max_mb,
+               "%s: a %dx%d image has %d tokens, more than the %lld token rows of the workspace "
+               "(%d x max_micro_batch %d); create the engine with max_micro_batch >= %d",
+               fn, height, width, S, (long long)kVisSeq * e->max_mb, kVisSeq, e->max_mb, (S + kVisSeq - 1) / kVisSeq);
   return 0;
 }
 
@@ -829,6 +878,25 @@ PLIP_API int plip_encode_images(plip_engine_t* e, const void* pixels_dev, int pi
     const int64_t mb = (n - i < e->max_mb) ? (n - i) : e->max_mb;
     if (int rc = vision_forward(e, static_cast<const uint8_t*>(pixels_dev) + i * pb, pixel_format, mb,
                                 out_dev + i * kProj, normalize, st)) return rc;
+  }
+  PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
+  return 0;
+}
+
+PLIP_API int plip_encode_images_hw(plip_engine_t* e, const void* pixels_dev, int pixel_format, int64_t n, int height,
+                                   int width, float* out_dev, int normalize, void* stream) {
+  if (int rc = check_hw_call("plip_encode_images_hw", e, pixels_dev, out_dev, pixel_format, n, height, width)) return rc;
+  if (height == kImage && width == kImage)
+    return plip_encode_images(e, pixels_dev, pixel_format, n, out_dev, normalize, stream);
+  const VisGeom geo = vis_geom(height, width);
+  const int64_t per_pass = images_per_pass(e->max_mb, geo.S);
+  const size_t pb = pixel_bytes(pixel_format, height, width);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_last, 0));  // calls on different streams share one workspace
+  for (int64_t i = 0; i < n; i += per_pass) {
+    const int64_t mb = (n - i < per_pass) ? (n - i) : per_pass;
+    if (int rc = vision_forward(e, static_cast<const uint8_t*>(pixels_dev) + i * pb, pixel_format, mb,
+                                out_dev + i * kProj, normalize, st, geo)) return rc;
   }
   PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
   return 0;
@@ -1089,8 +1157,12 @@ PLIP_API int plip_dbg_attention(const void* qkv_bf16, int64_t n_seq, int seq_len
 }
 
 PLIP_API int plip_dbg_im2col(const void* pixels, int pixel_format, int64_t n, void* out_bf16, void* stream) {
-  return launch_im2col(pixels, pixel_format, n, static_cast<__nv_bfloat16*>(out_bf16), g_dbg_f16,
+  return launch_im2col(pixels, pixel_format, n, kImage, kImage, static_cast<__nv_bfloat16*>(out_bf16), g_dbg_f16,
                        static_cast<cudaStream_t>(stream));
+}
+
+PLIP_API int plip_dbg_pos_interp(const float* pos_dev, int grid_h, int grid_w, float* out_dev, void* stream) {
+  return launch_pos_interp(pos_dev, grid_h, grid_w, out_dev, static_cast<cudaStream_t>(stream));
 }
 
 PLIP_API int plip_dbg_hidden_states(plip_engine_t* e, int tower, const void* input_dev, int input_format,
@@ -1102,13 +1174,30 @@ PLIP_API int plip_dbg_hidden_states(plip_engine_t* e, int tower, const void* inp
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   size_t bytes;
   if (tower == 0) {
-    if (int rc = vision_trunk(e, input_dev, input_format, n, num_layers, st)) return rc;
+    if (int rc = vision_trunk(e, input_dev, input_format, n, VisGeom(), num_layers, st)) return rc;
     bytes = (size_t)n * kVisSeq * kVisDim * 4;
   } else {
     if (int rc = text_trunk(e, input_dev, input_format, attention_mask_dev, n, kTxtSeq, kTxtSeq, num_layers, st)) return rc;
     bytes = (size_t)n * kTxtSeq * kTxtDim * 4;
   }
   PLIP_CUDA_CHECK(cudaMemcpyAsync(hidden_dev, e->X, bytes, cudaMemcpyDeviceToDevice, st));
+  PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
+  return 0;
+}
+
+PLIP_API int plip_dbg_hidden_states_hw(plip_engine_t* e, const void* pixels_dev, int pixel_format, int64_t n,
+                                       int height, int width, int num_layers, float* hidden_dev, void* stream) {
+  if (int rc = check_hw_call("plip_dbg_hidden_states_hw", e, pixels_dev, hidden_dev, pixel_format, n, height, width))
+    return rc;
+  const VisGeom geo = vis_geom(height, width);
+  PLIP_REQUIRE(n <= images_per_pass(e->max_mb, geo.S),
+               "plip_dbg_hidden_states_hw: n=%lld images of %d tokens exceed one pass (%lld images)", (long long)n,
+               geo.S, (long long)images_per_pass(e->max_mb, geo.S));
+  PLIP_REQUIRE(num_layers >= 0 && num_layers <= kLayers, "plip_dbg_hidden_states_hw: num_layers %d", num_layers);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_last, 0));
+  if (int rc = vision_trunk(e, pixels_dev, pixel_format, n, geo, num_layers, st)) return rc;
+  PLIP_CUDA_CHECK(cudaMemcpyAsync(hidden_dev, e->X, (size_t)n * geo.S * kVisDim * 4, cudaMemcpyDeviceToDevice, st));
   PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
   return 0;
 }

@@ -9,7 +9,7 @@ enum GemmEpilogue : int {
   EPI_BIAS_BF16 = 0,       // out_bf16 = acc + bias                     (QKV projection, TF:modeling_clip.py:310-312)
   EPI_BIAS_GELU_BF16 = 1,  // out_bf16 = quick_gelu(acc + bias)         (fc1, TF:modeling_clip.py:348-349)
   EPI_BIAS_RESID_F32 = 2,  // x_f32   += acc + bias  (in place)         (out_proj / fc2 + residual, :334,:377,:350,:382)
-  EPI_PATCH_F32 = 3,       // x_f32[b*50+1+p] = acc + pos[1+p]          (patch conv + position embedding, :209-217)
+  EPI_PATCH_F32 = 3,       // x_f32[b*S+1+p] = acc + pos[1+p]           (patch conv + position embedding, :209-217)
   EPI_F32 = 4,             // out_f32 = acc                             (visual/text projection, :861,:823)
   // LayerNorm folded into the consuming GEMM (DESIGN.md §4.1): A holds bf16(x) (un-normalised), W holds
   // bf16(gamma o W), colsum[n] = sum_k W'[n,k], bias' = bias + W beta, and per-row (sum, sum of squares)
@@ -36,7 +36,9 @@ struct GemmArgs {
   const float* rowscale = nullptr;   // [M]   EPI_SIM_F32 only
   void* out = nullptr;               // bf16 or fp32 depending on epilogue; row stride ldo elements
   int ldo = 0;
-  const float* pos = nullptr;        // EPI_PATCH_F32: vision position embedding [50, N]
+  const float* pos = nullptr;        // EPI_PATCH_F32: vision position embedding [seq, N]
+  int patches = kPatches;            // EPI_PATCH_F32: patches per image (A row r = patch r % patches of image r / patches)
+  int seq = kVisSeq;                 // EPI_PATCH_F32: rows per image in out (class row + patches)
   const float* colsum = nullptr;     // EPI_LN_*: [N] row sums of the folded bf16 weight
   const float2* stats_in = nullptr;  // EPI_LN_*: [M, kStatSlots] partial (sum, sumsq) of the fp32 rows behind A
   int n_partials = 0;                // EPI_LN_*: valid slots in stats_in

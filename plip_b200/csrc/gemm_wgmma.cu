@@ -53,6 +53,7 @@ struct GemmDev {
   void* out;
   int ldo;
   const float* pos;
+  int patches, seq;
   const float* colsum;
   const float2* stats_in;
   int n_partials;
@@ -158,11 +159,11 @@ __device__ __forceinline__ void epilogue_warp(const GemmDev& p, const CUtensorMa
     size_t q0 = 0, q1 = 0;  // EPI_PATCH_F32: rows of the position embedding
     if constexpr (EPI == EPI_PATCH_F32) {
       const int r0 = ok0 ? row0 : 0, r1 = ok1 ? row1 : 0;
-      const int b0 = r0 / kPatches, b1 = r1 / kPatches;
-      o0 = static_cast<size_t>(b0 * kVisSeq + 1 + (r0 - b0 * kPatches)) * p.ldo;
-      o1 = static_cast<size_t>(b1 * kVisSeq + 1 + (r1 - b1 * kPatches)) * p.ldo;
-      q0 = static_cast<size_t>(1 + (r0 - b0 * kPatches)) * p.N;
-      q1 = static_cast<size_t>(1 + (r1 - b1 * kPatches)) * p.N;
+      const int b0 = r0 / p.patches, b1 = r1 / p.patches;
+      o0 = static_cast<size_t>(b0 * p.seq + 1 + (r0 - b0 * p.patches)) * p.ldo;
+      o1 = static_cast<size_t>(b1 * p.seq + 1 + (r1 - b1 * p.patches)) * p.ldo;
+      q0 = static_cast<size_t>(1 + (r0 - b0 * p.patches)) * p.N;
+      q1 = static_cast<size_t>(1 + (r1 - b1 * p.patches)) * p.N;
     }
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
@@ -392,6 +393,7 @@ int launch_inst(const GemmArgs& g, cudaStream_t stream) {
   GemmDev p;
   p.M = g.M; p.N = g.N; p.K = g.K;
   p.bias = g.bias; p.rowscale = g.rowscale; p.out = g.out; p.ldo = g.ldo; p.pos = g.pos;
+  p.patches = g.patches; p.seq = g.seq;
   p.colsum = g.colsum; p.stats_in = g.stats_in; p.n_partials = g.n_partials;
   p.xb_out = g.xb_out; p.stats_out = g.stats_out;
   if (g.n_tiles_used) *g.n_tiles_used = 2 * (g.N / BN);
@@ -438,6 +440,9 @@ int launch_gemm(const GemmArgs& g, cudaStream_t stream) {
                  "launch_gemm: LayerNorm-folded epilogue needs colsum, stats and 1..%d partials", kStatSlots);
   if (g.epi == EPI_SIM_F32)
     PLIP_REQUIRE(g.bias && g.rowscale, "launch_gemm: the similarity epilogue needs row and column scales");
+  if (g.epi == EPI_PATCH_F32)
+    PLIP_REQUIRE(g.patches >= 1 && g.seq == g.patches + 1, "launch_gemm: patch epilogue with %d patches, %d rows",
+                 g.patches, g.seq);
   if (g.xb_out || g.stats_out)
     PLIP_REQUIRE(g.epi == EPI_BIAS_RESID_F32 && g.xb_out && g.stats_out,
                  "launch_gemm: xb/stats outputs belong to the residual epilogue");

@@ -8,7 +8,12 @@
 namespace plip {
 
 // elementwise.cu  (f16 = 1: 16-bit outputs are IEEE half instead of bfloat16; the pointer type stays a 16-bit tag)
-int launch_im2col(const void* pixels, int fmt, int64_t n, __nv_bfloat16* out, int f16, cudaStream_t st);
+// pixels: n images of height x width (224 x 224 unless the position table is interpolated) -> the patch matrix
+// [n * gh * gw, 3072], gh = height / 32, gw = width / 32.
+int launch_im2col(const void* pixels, int fmt, int64_t n, int height, int width, __nv_bfloat16* out, int f16,
+                  cudaStream_t st);
+// The vision position table resized to a gh x gw patch grid: fp32 [1 + gh * gw, 768] (bicubic, as HF).
+int launch_pos_interp(const float* pos, int gh, int gw, float* out, cudaStream_t st);
 int launch_layernorm(const float* x, const int32_t* row_index, int64_t in_row_stride, int64_t rows, int dim,
                      const float* gamma, const float* beta, float* out_f32, __nv_bfloat16* out_bf16, int f16,
                      cudaStream_t st);
@@ -17,7 +22,7 @@ int launch_text_embed(const void* ids, int ids_dtype, int64_t n, int seq_len, in
                       const float* pos, float* x, int32_t* eos_rows, int eos_id, int no_eos_argmax, cudaStream_t st);
 int launch_mask_to_i32(const void* mask, int dtype, int64_t count, int seq_len, int stride, int32_t* out,
                        cudaStream_t st);
-int launch_cls_rows(const float* cls, const float* pos, int64_t n, float* x, cudaStream_t st);
+int launch_cls_rows(const float* cls, const float* pos, int64_t n, int seq, float* x, cudaStream_t st);
 int launch_l2_normalize(float* x, int64_t rows, int dim, cudaStream_t st);
 // rows idx(i) (= row_index[i], or i * row_stride) of a 16-bit [*, dim] and an fp32 [*, dim] matrix -> compact [n, dim]
 int launch_gather_rows(const __nv_bfloat16* a16, const float* x32, const int32_t* row_index, int64_t row_stride,
@@ -31,6 +36,7 @@ int resize_filter_host(int in_size, int out_size, int xx, int32_t* k, int k_cap,
 
 // attention.cu: softmax(q k^T [+causal/padding mask]) v per (sequence, head); q pre-scaled by dh^-0.5.
 // qkv: bf16 [n_seq*seq_len, 3*heads*64]; key_mask: optional int32 [n_seq, seq_len] (0 = masked key).
+// seq_len > 128 (up to kMaxVisSeq) runs the long-sequence kernel: no causal mask, no key mask.
 // f16 = 1: q, k, v, P and the output are IEEE half instead of bfloat16 (the engine's operand format).
 int launch_attention(const __nv_bfloat16* qkv, int64_t n_seq, int seq_len, int heads, bool causal,
                      const int32_t* key_mask, __nv_bfloat16* out, int f16, cudaStream_t st);

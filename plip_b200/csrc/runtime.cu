@@ -90,6 +90,27 @@ int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_
   return 0;
 }
 
+// Not cached: one launch of the long-sequence attention kernel encodes two.
+int make_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t mats, uint64_t rows, uint64_t cols,
+                      uint64_t row_stride_bytes, uint64_t mat_stride_bytes, uint32_t box_rows, uint32_t box_cols) {
+  EncodeTiledFn enc = resolve_encode();
+  if (!enc) return -1;
+  cuuint64_t gdim[3] = {cols, rows, mats};
+  cuuint64_t gstr[2] = {row_stride_bytes, mat_stride_bytes};
+  cuuint32_t box[3] = {box_cols, box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), gdim, gstr, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_last_error("cuTensorMapEncodeTiled (3-D) failed (%d): base=%p mats=%llu rows=%llu cols=%llu box=%ux%u",
+                   (int)r, base, (unsigned long long)mats, (unsigned long long)rows, (unsigned long long)cols,
+                   box_rows, box_cols);
+    return -1;
+  }
+  return 0;
+}
+
 static int encode_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
                                uint64_t row_stride_bytes, uint32_t box_rows, uint32_t box_cols) {
   EncodeTiledFn enc = resolve_encode();

@@ -18,24 +18,46 @@ IMAGE_SIZE = 224
 MAX_TEXT_LEN = 77
 
 
-def _pixel_format(t: Union[torch.Tensor, np.ndarray]) -> int:
-    """Validate an image batch and return its C-ABI pixel format (error text mirrors TF:204-207)."""
+PATCH = 32
+MAX_GRID = 32  # interpolate_pos_encoding: at most 32 x 32 patches (1024 px per side, 1025 tokens)
+
+
+def _check_size(h: int, w: int, interpolate_pos_encoding: bool) -> None:
+    if not interpolate_pos_encoding:
+        if h != IMAGE_SIZE or w != IMAGE_SIZE:
+            raise ValueError(f"Input image size ({h}*{w}) doesn't match model (224*224).")  # TF:204-207
+    elif not (h >= PATCH and w >= PATCH and h // PATCH <= MAX_GRID and w // PATCH <= MAX_GRID):
+        raise ValueError(f"Input image size ({h}*{w}) out of range for interpolate_pos_encoding: height and width "
+                         f"must be >= {PATCH} with at most {MAX_GRID} patches of {PATCH} per side (<= 1055 px)")
+
+
+def _pixel_format(t: Union[torch.Tensor, np.ndarray], interpolate_pos_encoding: bool = False) -> int:
+    """Validate an image batch and return its C-ABI pixel format (error text mirrors TF:204-207).  With
+    ``interpolate_pos_encoding`` any height / width with ``32 <= H, W`` and ``H // 32, W // 32 <= 32`` is accepted."""
     shape, dtype = tuple(t.shape), t.dtype
     if dtype in (torch.uint8, np.dtype("uint8")):
         if len(shape) != 4 or shape[3] != 3:
             raise ValueError(f"uint8 images must be [n,224,224,3] (NHWC), got {shape}")
-        if shape[1] != IMAGE_SIZE or shape[2] != IMAGE_SIZE:
-            raise ValueError(f"Input image size ({shape[1]}*{shape[2]}) doesn't match model (224*224).")
+        _check_size(shape[1], shape[2], interpolate_pos_encoding)
         return PIX_U8_NHWC
     if len(shape) != 4 or shape[1] != 3:
         raise ValueError(f"pixel_values must be [n,3,224,224], got {shape}")
-    if shape[2] != IMAGE_SIZE or shape[3] != IMAGE_SIZE:
-        raise ValueError(f"Input image size ({shape[2]}*{shape[3]}) doesn't match model (224*224).")
+    _check_size(shape[2], shape[3], interpolate_pos_encoding)
     if dtype in (torch.float32, np.dtype("float32")):
         return PIX_F32_NCHW
     if dtype == torch.bfloat16:
         return PIX_BF16_NCHW
     raise TypeError(f"unsupported pixel dtype {dtype} (float32, bfloat16 or uint8)")
+
+
+def _pixel_hw(t: Union[torch.Tensor, np.ndarray], fmt: int) -> Tuple[int, int]:
+    """``(height, width)`` of a batch ``_pixel_format`` accepted as ``fmt``."""
+    return (int(t.shape[1]), int(t.shape[2])) if fmt == PIX_U8_NHWC else (int(t.shape[2]), int(t.shape[3]))
+
+
+def vision_seq_len(height: int, width: int) -> int:
+    """Tokens of one image: ``(H // 32) * (W // 32)`` patches + the class token (50 at 224 x 224)."""
+    return (height // PATCH) * (width // PATCH) + 1
 
 
 def _ids_dtype(dtype) -> int:
@@ -158,17 +180,28 @@ class Engine:
 
     # ---- device-tensor API -------------------------------------------------------------------
     @torch.no_grad()
-    def encode_images(self, pixels: torch.Tensor, normalize: bool = False) -> torch.Tensor:
-        """``get_image_features``: ``[n,3,224,224]`` f32/bf16 or ``[n,224,224,3]`` u8 -> ``[n,512]`` f32 (device)."""
-        fmt = _pixel_format(pixels)
+    def encode_images(self, pixels: torch.Tensor, normalize: bool = False,
+                      interpolate_pos_encoding: bool = False) -> torch.Tensor:
+        """``get_image_features``: ``[n,3,224,224]`` f32/bf16 or ``[n,224,224,3]`` u8 -> ``[n,512]`` f32 (device).
+
+        ``interpolate_pos_encoding=True``: any ``[n,3,H,W]`` / ``[n,H,W,3]`` with ``32 <= H, W`` and at most 32 patches
+        of 32 pixels per side; the position table is resized bicubically to the patch grid, as HF does
+        (``plip_encode_images_hw``).  An image's ``(H // 32) * (W // 32) + 1`` tokens must fit the workspace's
+        ``50 * max_micro_batch`` token rows."""
+        fmt = _pixel_format(pixels, interpolate_pos_encoding)
         n = int(pixels.shape[0])
         if n == 0:
             return torch.empty(0, EMBED_DIM, device=self.device)
         pixels = self._dev(pixels)
         out = torch.empty(n, EMBED_DIM, device=self.device, dtype=torch.float32)
         with torch.cuda.device(self.device):
-            check(self._L.plip_encode_images(self._h, pixels.data_ptr(), fmt, n, out.data_ptr(), int(normalize),
-                                             self._stream()), "plip_encode_images")
+            if interpolate_pos_encoding:
+                h, w = _pixel_hw(pixels, fmt)
+                check(self._L.plip_encode_images_hw(self._h, pixels.data_ptr(), fmt, n, h, w, out.data_ptr(),
+                                                    int(normalize), self._stream()), "plip_encode_images_hw")
+            else:
+                check(self._L.plip_encode_images(self._h, pixels.data_ptr(), fmt, n, out.data_ptr(), int(normalize),
+                                                 self._stream()), "plip_encode_images")
         return out
 
     @torch.no_grad()
@@ -296,10 +329,20 @@ class Engine:
     # ---- test hook ---------------------------------------------------------------------------
     @torch.no_grad()
     def hidden_states(self, tower: str, inputs: torch.Tensor, num_layers: int,
-                      attention_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """Residual stream after ``num_layers`` encoder layers (fp32), for layer-wise parity tests."""
+                      attention_mask: Optional[torch.Tensor] = None,
+                      interpolate_pos_encoding: bool = False) -> torch.Tensor:
+        """Residual stream after ``num_layers`` encoder layers (fp32), for layer-wise parity tests.  Vision with
+        ``interpolate_pos_encoding``: any accepted image size, ``[n, S, 768]`` with ``S = vision_seq_len(H, W)``."""
         x = self._dev(inputs)
         n = int(x.shape[0])
+        if tower == "vision" and interpolate_pos_encoding:
+            fmt = _pixel_format(x, True)
+            h, w = _pixel_hw(x, fmt)
+            out = torch.empty((n, vision_seq_len(h, w), 768), device=self.device, dtype=torch.float32)
+            with torch.cuda.device(self.device):
+                check(self._L.plip_dbg_hidden_states_hw(self._h, x.data_ptr(), fmt, n, h, w, int(num_layers),
+                                                        out.data_ptr(), self._stream()), "plip_dbg_hidden_states_hw")
+            return out
         if tower == "vision":
             fmt, t, shape = _pixel_format(x), 0, (n, 50, 768)
         else:

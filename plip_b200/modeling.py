@@ -101,11 +101,13 @@ class PlipCLIPModel:
         return self.engine.logit_scale_exp
 
     # ---- HF surface ---------------------------------------------------------------------------
-    def get_image_features(self, pixel_values: torch.Tensor = None, **_ignored) -> torch.Tensor:
-        """TF:829-863 — vision tower + visual_projection, un-normalised ``[n,512]`` float32."""
+    def get_image_features(self, pixel_values: torch.Tensor = None, interpolate_pos_encoding: bool = False,
+                           **_ignored) -> torch.Tensor:
+        """TF:829-863 — vision tower + visual_projection, un-normalised ``[n,512]`` float32.
+        ``interpolate_pos_encoding=True`` accepts other image sizes (TF:161-218; ``Engine.encode_images``)."""
         if pixel_values is None:
             raise ValueError("You have to specify pixel_values")
-        return self.engine.encode_images(pixel_values)
+        return self.engine.encode_images(pixel_values, interpolate_pos_encoding=interpolate_pos_encoding)
 
     def get_text_features(self, input_ids: torch.Tensor = None, attention_mask: Optional[torch.Tensor] = None,
                           **_ignored) -> torch.Tensor:
@@ -116,12 +118,13 @@ class PlipCLIPModel:
 
     def forward(self, input_ids: torch.Tensor = None, pixel_values: torch.Tensor = None,
                 attention_mask: Optional[torch.Tensor] = None, return_loss: Optional[bool] = None,
-                **_ignored) -> CLIPOutput:
+                interpolate_pos_encoding: bool = False, **_ignored) -> CLIPOutput:
         """TF:867-944 — both towers, L2-normalise, ``exp(logit_scale) * I . T^T``."""
         if input_ids is None:
             raise ValueError("You have to specify input_ids")
         if pixel_values is None:
             raise ValueError("You have to specify pixel_values")
+        ipe = interpolate_pos_encoding
         if not pixel_values.is_cuda:
             # host inputs (an extension: HF would raise on a device mismatch): the pixel upload runs on the engine's
             # copy stream while the text tower computes, so ~3 ms of PCIe time per 1024 uint8 tiles stay hidden
@@ -133,10 +136,10 @@ class PlipCLIPModel:
             embs = []
             for chunk, uploaded in parts:
                 torch.cuda.current_stream(self.device).wait_event(uploaded)
-                embs.append(self.engine.encode_images(chunk, normalize=True))
+                embs.append(self.engine.encode_images(chunk, normalize=True, interpolate_pos_encoding=ipe))
             img = embs[0] if len(embs) == 1 else torch.cat(embs, dim=0)
         else:
-            img = self.engine.encode_images(pixel_values, normalize=True)
+            img = self.engine.encode_images(pixel_values, normalize=True, interpolate_pos_encoding=ipe)
             txt = self.engine.encode_text(input_ids, attention_mask, normalize=True)
         lpi = self.engine.similarity(img, txt, normalize_image=False, normalize_text=False)
         loss = None

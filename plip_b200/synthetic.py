@@ -139,6 +139,16 @@ def pixel_values(n: int, seed: int = 1234) -> torch.Tensor:
     return (x - mean) / std
 
 
+def pixel_values_hw(n: int, h: int, w: int, seed: int = 4321) -> torch.Tensor:
+    """Normalised pixels of any size (``interpolate_pos_encoding`` inputs): fp32 [n,3,h,w], drawn like
+    :func:`pixel_values`."""
+    g = torch.Generator().manual_seed(seed)
+    x = torch.rand(n, 3, h, w, generator=g)
+    mean = torch.tensor((0.48145466, 0.4578275, 0.40821073)).view(1, 3, 1, 1)
+    std = torch.tensor((0.26862954, 0.26130258, 0.27577711)).view(1, 3, 1, 1)
+    return (x - mean) / std
+
+
 def token_ids(n: int, seed: int = 1235, full_length: bool = False, min_len: int = 8):
     """cfg3: random caption ids [n,77] int64 with bos at 0, first eos at len-1, eos padding after it
     (what the CLIP tokenizer emits), plus the matching attention_mask (1 up to and incl. the eos)."""
