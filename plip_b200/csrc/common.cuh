@@ -233,6 +233,15 @@ __device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* tm, int32_
                : "memory");
 }
 
+__device__ __forceinline__ float2 ld_shared_f32x2(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_shared_f32x2(uint32_t addr, float2 v) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v.x), "f"(v.y) : "memory");
+}
+
 // 2-D tile load, completion on an mbarrier of the executing CTA.
 __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const CUtensorMap* tm, uint32_t bar,
                                             int32_t c0, int32_t c1) {

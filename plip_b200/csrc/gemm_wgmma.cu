@@ -34,12 +34,22 @@ constexpr int kConsumerWarps = 8;
 constexpr uint32_t A_STAGE = BM * BK * 2;
 constexpr uint32_t kStoreStageBytes = 16 * 128;  // one [16 rows x 64 bf16] TMA store box
 
-template <int BN>
+// Staging blocks (2 KB each) per consumer warp.  The 16-bit epilogues alternate two store boxes.  The fp32 residual
+// epilogue streams x in and y out through them, one box per block in flight: two blocks at BN 256 and 128, three at
+// BN 192 (which still leaves 4 ring stages).  Each count divides the tile's BN / 32 boxes, so every tile starts at
+// block 0.  Four blocks at BN 256 would cost a ring stage (4 -> 3) and measured slower (tools/gemm_epilogue_probe.py:
+// out_proj 378 vs 351 us, fc2 638 vs 581 us on an H100 80GB HBM3 at 700 W).
+constexpr int x_boxes(int BN, int EPI) {
+  return EPI != EPI_BIAS_RESID_F32 ? 2 : BN == 192 ? 3 : 2;
+}
+
+template <int BN, int EPI>
 struct Cfg {
   static constexpr uint32_t B_STAGE = BN * BK * 2;
   static constexpr uint32_t STAGE = A_STAGE + B_STAGE;
-  static constexpr uint32_t EPI_BYTES = kConsumerWarps * 2 * kStoreStageBytes;  // two store boxes per consumer warp
-  static constexpr uint32_t BAR_BYTES = 256;
+  static constexpr int XBOXES = x_boxes(BN, EPI);
+  static constexpr uint32_t EPI_BYTES = kConsumerWarps * XBOXES * kStoreStageBytes;
+  static constexpr uint32_t BAR_BYTES = EPI == EPI_BIAS_RESID_F32 ? 512 : 256;
   static constexpr uint32_t ALIGN_SLACK = 1024;  // SWIZZLE_128B tiles need a 1024-byte aligned base
   static constexpr int kMaxStages = (227 * 1024 - BAR_BYTES - EPI_BYTES - ALIGN_SLACK) / STAGE;
   static constexpr int STAGES = kMaxStages > 8 ? 8 : kMaxStages;
@@ -92,9 +102,11 @@ __device__ __forceinline__ float2 ln_row_terms(const GemmDev& p, int grow) {
 //   16-bit outputs: a [16 x 64] block is staged in shared memory in the SWIZZLE_128B pattern (conflict-free: the 8
 //   rows of a store instruction hit 8 different 16-byte chunks) and leaves with one TMA bulk store; two staging
 //   blocks per warp alternate, so the math of a block overlaps the store of the previous one.
+//   The fp32 residual (EPI_BIAS_RESID_F32) reads x through the same two blocks, see there.
 template <int BN, int EPI, bool F16>
 __device__ __forceinline__ void epilogue_warp(const GemmDev& p, const CUtensorMap* tmC, float (&d)[BN / 2], uint32_t stage_smem,
-                                              uint32_t& stage_sel, int row_base, int col_base, int n_blk, int lane, float2 ln0, float2 ln1) {
+                                              uint32_t& stage_sel, uint32_t xbar, int row_base, int col_base, int n_blk, int lane,
+                                              float2 ln0, float2 ln1) {
   constexpr bool LN_FOLD = (EPI == EPI_LN_BIAS_BF16 || EPI == EPI_LN_BIAS_GELU_BF16);
   constexpr bool GELU = (EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_LN_BIAS_GELU_BF16);
   constexpr bool HAS_BIAS = (EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_BIAS_RESID_F32 || LN_FOLD);
@@ -144,12 +156,110 @@ __device__ __forceinline__ void epilogue_warp(const GemmDev& p, const CUtensorMa
         tma_store_commit();
       }
     }
+  } else if constexpr (EPI == EPI_BIAS_RESID_F32) {
+    // x += acc + bias in place; with xb_out, also the 16-bit copy of the new rows (A operand of the next,
+    // LayerNorm-folded GEMM) and the (sum, sum of squares) of the fp32 rows, one partial per half of the tile's columns.
+    // x is not read straight into registers: the compiler has to assume that out, xb_out and stats_out alias, so
+    // every load of x would wait for the stores before it (one 8-byte load per lane in flight), and the accumulator
+    // leaves no registers to batch them.  Instead x streams through the warp's NB staging blocks as TMA boxes of
+    // [16 rows x 32 fp32] (tmC: the fp32 rows seen as 16-bit pairs, SWIZZLE_128B, rows past M zero-filled): box c
+    // lands in block c % NB and completes a phase of that block's barrier (xbar + 8 (c % NB)).  Each lane overwrites
+    // the x it read with y, and y leaves with one TMA store of the box (rows past M clipped): full 128-byte lines
+    // instead of 32-byte pieces of 8 rows per store instruction.  Once that store has read the block, the load of box
+    // c + NB goes into it, so NB boxes are always in flight.  (An L2 prefetch of the tile's rows by the producer during
+    // the main loop measured slower: the extra requests delay the A / W feed more than they save here.)
+    // In the swizzled box row r holds its eight 16-byte pieces at (piece ^ r % 8): the reads below (8 rows x 2 pieces
+    // per instruction) are conflict-free.
+    constexpr int kChunkCols = 32;
+    constexpr int kChunks = BN / kChunkCols;
+    constexpr int NB = x_boxes(BN, EPI);
+    static_assert(kChunks % NB == 0, "every tile must start at staging block 0");
+    constexpr int kUses = kChunks / NB;  // barrier phases each block completes per tile
+    const bool ok0 = row0 < p.M, ok1 = row1 < p.M;
+    const bool emit = p.xb_out != nullptr;
+    // element offsets of the lane's first column in its two rows (row1 is only touched when row0 < M as well)
+    const size_t o0 = static_cast<size_t>(ok0 ? row0 : 0) * p.ldo + col_base + 2 * q;
+    const size_t o1 = o0 + 8 * static_cast<size_t>(p.ldo);
+    // parity of the phases the blocks completed in earlier tiles: always even (no state) when kUses is even
+    uint32_t ph0 = 0;
+    if constexpr (kUses % 2 != 0) ph0 = stage_sel++ & 1u;
+    auto fetch = [&](int c) {
+      if (lane == 0) {
+        const uint32_t bar = xbar + 8u * (c % NB);
+        mbar_arrive_expect_tx(bar, kStoreStageBytes);
+        tma_load_2d(stage_smem + (c % NB) * kStoreStageBytes, tmC, bar, 2 * (col_base + c * kChunkCols), row_base);
+      }
+    };
+    // Refilling a block: lane 0 waits until its TMA store has read the block (the lanes' own accesses to it were
+    // ordered before that store by the proxy fence and __syncwarp), then issues the load.
+    if (lane == 0) tma_store_wait_read();  // the previous tile's stores out of every block
+    __syncwarp();
+#pragma unroll
+    for (int c = 0; c < NB; ++c) fetch(c);
+    float st[2][2] = {};  // (sum, sum of squares) of the lane's two rows over the current half of the tile's columns
+#pragma unroll
+    for (int c = 0; c < kChunks; ++c) {
+      const int h = c < kChunks / 2 ? 0 : 1;
+      mbar_wait(xbar + 8u * (c % NB), ph0 ^ ((c / NB) & 1u));
+      const uint32_t buf = stage_smem + (c % NB) * kStoreStageBytes;
+#pragma unroll
+      for (int jj = 0; jj < kChunkCols / 8; ++jj) {
+        const int j = c * (kChunkCols / 8) + jj;
+        const int col = col_base + 8 * j + 2 * q;
+        const uint32_t xoff = (((2 * jj + (q >> 1)) ^ rr) << 4) + (q & 1) * 8;
+        const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+        const float2 v0 = make_float2(d[4 * j + 0] + b.x, d[4 * j + 1] + b.y);
+        const float2 v1 = make_float2(d[4 * j + 2] + b.x, d[4 * j + 3] + b.y);
+        if (ok0) {
+          const float2 x = ld_shared_f32x2(buf + rr * 128 + xoff);
+          const float2 y = make_float2(x.x + v0.x, x.y + v0.y);
+          st_shared_f32x2(buf + rr * 128 + xoff, y);
+          if (emit) {
+            *reinterpret_cast<uint32_t*>(p.xb_out + o0 + 8 * j) = pack_op2<F16>(y.x, y.y);
+            st[0][0] += y.x + y.y;
+            st[0][1] = fmaf(y.x, y.x, fmaf(y.y, y.y, st[0][1]));
+          }
+        }
+        if (ok1) {
+          const float2 x = ld_shared_f32x2(buf + (rr + 8) * 128 + xoff);
+          const float2 y = make_float2(x.x + v1.x, x.y + v1.y);
+          st_shared_f32x2(buf + (rr + 8) * 128 + xoff, y);
+          if (emit) {
+            *reinterpret_cast<uint32_t*>(p.xb_out + o1 + 8 * j) = pack_op2<F16>(y.x, y.y);
+            st[1][0] += y.x + y.y;
+            st[1][1] = fmaf(y.x, y.x, fmaf(y.y, y.y, st[1][1]));
+          }
+        }
+      }
+      fence_proxy_async_smem();  // y in the block -> visible to the TMA store
+      __syncwarp();
+      if (lane == 0) {
+        tma_store_2d(tmC, buf, 2 * (col_base + c * kChunkCols), row_base);
+        tma_store_commit();
+      }
+      if (c + NB < kChunks) {
+        if (lane == 0) tma_store_wait_read();
+        fetch(c + NB);
+      }
+      if (emit && (c + 1) % (kChunks / 2) == 0) {  // a half is complete: its partials leave, freeing the registers
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          float a = st[r][0], b = st[r][1];
+#pragma unroll
+          for (int o = 1; o < 4; o <<= 1) {  // the 4 lanes that share a row
+            a += __shfl_xor_sync(0xffffffffu, a, o);
+            b += __shfl_xor_sync(0xffffffffu, b, o);
+          }
+          if (q == 0 && (r == 0 ? ok0 : ok1))
+            p.stats_out[static_cast<size_t>(row0 + 8 * r) * kStatSlots + 2 * n_blk + h] = make_float2(a, b);
+          st[r][0] = 0.f;
+          st[r][1] = 0.f;
+        }
+      }
+    }
   } else {
     float* out = reinterpret_cast<float*>(p.out);
     const bool ok0 = row0 < p.M, ok1 = row1 < p.M;
-    const bool emit = (EPI == EPI_BIAS_RESID_F32) && p.xb_out != nullptr;
-    // (sum, sum of squares) of the updated residual rows, one partial per half of the tile's columns
-    float st[2][2][2] = {};
     float rs0 = 1.f, rs1 = 1.f;
     size_t o0 = static_cast<size_t>(ok0 ? row0 : 0) * p.ldo, o1 = static_cast<size_t>(ok1 ? row1 : 0) * p.ldo;
     if constexpr (EPI == EPI_SIM_F32) {
@@ -173,30 +283,7 @@ __device__ __forceinline__ void epilogue_warp(const GemmDev& p, const CUtensorMa
         const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
         v0.x += b.x; v0.y += b.y; v1.x += b.x; v1.y += b.y;
       }
-      if constexpr (EPI == EPI_BIAS_RESID_F32) {
-        constexpr int kHalfBlocks = BN / 16;
-        const int h = j < kHalfBlocks ? 0 : 1;
-        if (ok0) {
-          const float2 x = *reinterpret_cast<const float2*>(out + o0 + col);
-          const float2 y = make_float2(x.x + v0.x, x.y + v0.y);
-          *reinterpret_cast<float2*>(out + o0 + col) = y;
-          if (emit) {  // 16-bit copy (A operand of the next, LayerNorm-folded GEMM) + statistics of the fp32 row
-            *reinterpret_cast<uint32_t*>(p.xb_out + o0 + col) = pack_op2<F16>(y.x, y.y);
-            st[h][0][0] += y.x + y.y;
-            st[h][0][1] = fmaf(y.x, y.x, fmaf(y.y, y.y, st[h][0][1]));
-          }
-        }
-        if (ok1) {
-          const float2 x = *reinterpret_cast<const float2*>(out + o1 + col);
-          const float2 y = make_float2(x.x + v1.x, x.y + v1.y);
-          *reinterpret_cast<float2*>(out + o1 + col) = y;
-          if (emit) {
-            *reinterpret_cast<uint32_t*>(p.xb_out + o1 + col) = pack_op2<F16>(y.x, y.y);
-            st[h][1][0] += y.x + y.y;
-            st[h][1][1] = fmaf(y.x, y.x, fmaf(y.y, y.y, st[h][1][1]));
-          }
-        }
-      } else if constexpr (EPI == EPI_SIM_F32) {
+      if constexpr (EPI == EPI_SIM_F32) {
         const float2 cs = __ldg(reinterpret_cast<const float2*>(p.bias + col));  // the column scales
         if (ok0) *reinterpret_cast<float2*>(out + o0 + col) = make_float2(v0.x * rs0 * cs.x, v0.y * rs0 * cs.y);
         if (ok1) *reinterpret_cast<float2*>(out + o1 + col) = make_float2(v1.x * rs1 * cs.x, v1.y * rs1 * cs.y);
@@ -214,24 +301,6 @@ __device__ __forceinline__ void epilogue_warp(const GemmDev& p, const CUtensorMa
         if (ok1) *reinterpret_cast<float2*>(out + o1 + col) = v1;
       }
     }
-    if constexpr (EPI == EPI_BIAS_RESID_F32) {
-      if (emit) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int r = 0; r < 2; ++r) {
-            float a = st[h][r][0], b = st[h][r][1];
-#pragma unroll
-            for (int o = 1; o < 4; o <<= 1) {  // the 4 lanes that share a row
-              a += __shfl_xor_sync(0xffffffffu, a, o);
-              b += __shfl_xor_sync(0xffffffffu, b, o);
-            }
-            const int grow = r == 0 ? row0 : row1;
-            if (q == 0 && grow < p.M)
-              p.stats_out[static_cast<size_t>(grow) * kStatSlots + 2 * n_blk + h] = make_float2(a, b);
-          }
-      }
-    }
   }
 }
 
@@ -239,7 +308,7 @@ template <int CG, int BN, int EPI, bool F16>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ CUtensorMap tmC, const GemmDev p) {
-  using C = Cfg<BN>;
+  using C = Cfg<BN, EPI>;
   constexpr int STAGES = C::STAGES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -247,6 +316,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   const uint32_t bar_base = epi_base + C::EPI_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+  const uint32_t resid_bar = bar_base + 8u * (2 * STAGES);  // EPI_BIAS_RESID_F32: one per staging block
+  static_assert(8 * (2 * STAGES + (EPI == EPI_BIAS_RESID_F32 ? C::XBOXES * kConsumerWarps : 0)) <= C::BAR_BYTES,
+                "barrier area too small");
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -259,6 +331,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);        // the producer's arrive.expect_tx
       mbar_init(empty_bar(s), 2 * CG);  // one arrive per consumer warpgroup of every CTA that reads the slot's W tile
+    }
+    if constexpr (EPI == EPI_BIAS_RESID_F32) {
+      tma_prefetch_desc(&tmC);
+      for (int i = 0; i < C::XBOXES * kConsumerWarps; ++i) mbar_init(resid_bar + 8u * i, 1);  // lane 0's arrive.expect_tx
     }
     fence_mbar_init();
   }
@@ -339,7 +415,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       wgmma_wait<0>();
       wgmma_pin(d);
       release(prev);
-      epilogue_warp<BN, EPI, F16>(p, &tmC, d, epi_base + warp * 2 * kStoreStageBytes, stage_sel, wrow, n_blk * BN, n_blk, lane, ln0, ln1);
+      epilogue_warp<BN, EPI, F16>(p, &tmC, d, epi_base + warp * C::XBOXES * kStoreStageBytes, stage_sel,
+                                  resid_bar + 8u * C::XBOXES * warp, wrow,
+                                  n_blk * BN, n_blk, lane, ln0, ln1);
     }
     if (lane == 0) tma_store_wait_all();
     __syncwarp();
@@ -355,7 +433,7 @@ int env_int(const char* name, int dflt) {
 
 template <int CG, int BN, int EPI, bool F16>
 int launch_inst(const GemmArgs& g, cudaStream_t stream) {
-  using C = Cfg<BN>;
+  using C = Cfg<BN, EPI>;
   auto kern = gemm_kernel<CG, BN, EPI, F16>;
   static unsigned long long configured = 0;
   static int max_groups = 0;  // co-resident clusters (CTAs for CG == 1)
@@ -389,6 +467,10 @@ int launch_inst(const GemmArgs& g, cudaStream_t stream) {
   CUtensorMap tmC = tmA;  // placeholder when unused
   if (kOutBf16)
     if (int rc = make_tmap_bf16_2d(&tmC, g.out, g.M, g.N, (uint64_t)g.ldo * 2, 16, 64)) return rc;
+  // the residual epilogue loads [16 x 32] fp32 boxes of x: the same bytes as [16 x 64] 16-bit elements, so the fp32
+  // rows are described as rows of 2 N 16-bit elements (a plain copy: the element type only sets the unit of the box)
+  if (EPI == EPI_BIAS_RESID_F32)
+    if (int rc = make_tmap_bf16_2d(&tmC, g.out, g.M, 2 * (uint64_t)g.N, (uint64_t)g.ldo * 4, 16, 64)) return rc;
 
   GemmDev p;
   p.M = g.M; p.N = g.N; p.K = g.K;
