@@ -32,7 +32,7 @@ extern "C" {
 
 #define PLIP_API __attribute__((visibility("default")))
 
-#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning */
+#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs (new symbols only) */
 
 /* Model constants (TF:configuration_clip.py:47-64,97-109,160-161). */
 #define PLIP_IMAGE_SIZE 224
@@ -153,6 +153,37 @@ PLIP_API int plip_encode_text_prefix(plip_engine_t* e, const void* ids_dev, int 
                                      const void* attention_mask_dev, int64_t n, int seq_len, int prefix_len,
                                      float* out_dev, int normalize, void* stream);
 
+/* ---- per-token outputs: output_hidden_states / output_attentions ------------------------------ */
+/* Device buffers (float32, caller-owned) filled by ONE pass of a tower: CLIPModel.vision_model(...) /
+ * text_model(..., output_hidden_states=True, output_attentions=True) (TF:modeling_clip.py:477-507, 531-589, 667-691).
+ * Every pointer is optional (NULL = not computed), but at least one must be set.  S is the sequence length (vision:
+ * (height / 32) * (width / 32) + 1; text: seq_len), D the tower width (768 / 512), heads 12 / 8.
+ *   embeds       [n,512]  projected pooled row (what plip_encode_* returns); normalize != 0 L2-normalises it
+ *   pooled       [n,D]    pooler_output: vision post_layernorm(CLS row); text final_layer_norm(pooled row)
+ *   last_hidden  [n,S,D]  vision: residual stream after the last layer (before post_layernorm);
+ *                         text: final_layer_norm of every row
+ *   hidden       [13,n,S,D]  hidden_states: [0] the encoder input (vision: after pre_layrnorm; text: token + position
+ *                         embeddings), [l] the residual stream after layer l
+ *   attn         [12,n,heads,S,S]  attentions: softmax(q k^T / 8 + mask) in fp32; masked keys are exactly 0, and a row
+ *                         without any visible key (text whose position 0 is padded) is all zeros
+ * These calls never replay CUDA graphs and never prune the last layer; the embeds equal plip_encode_* with pruning
+ * off bit for bit.  attn is large: heads * S^2 * 4 bytes per sequence and layer (120 KB at 224 x 224, 50 MB at
+ * 1024 x 1024).  Profile role of the probabilities kernel: "<tower>/attention[probs]". */
+typedef struct plip_tower_outputs {
+  float* embeds;
+  float* pooled;
+  float* last_hidden;
+  float* hidden;
+  float* attn;
+  int32_t normalize;
+} plip_tower_outputs_t;
+/* Vision at any size accepted by plip_encode_images_hw (224 x 224 included), micro-batched the same way. */
+PLIP_API int plip_vision_outputs(plip_engine_t* e, const void* pixels_dev, int pixel_format, int64_t n, int height,
+                                 int width, const plip_tower_outputs_t* outputs, void* stream);
+/* Text: ids / mask as plip_encode_text; all seq_len positions are processed. */
+PLIP_API int plip_text_outputs(plip_engine_t* e, const void* ids_dev, int ids_dtype, const void* attention_mask_dev,
+                               int64_t n, int seq_len, const plip_tower_outputs_t* outputs, void* stream);
+
 /* Similarity head: logits_per_image[n,m] = scale * norm(img)[n,512] . norm(txt)[m,512]^T
  * (TF:923-930; numpy versions at plip.py:73-76, evaluation/zero_shot/zero_shot.py:12,
  * evaluation/retrieval/retrieval.py:14).  normalize_img / normalize_txt select which side is
@@ -249,6 +280,10 @@ PLIP_API int plip_dbg_layernorm(const float* x, int64_t rows, int dim, int64_t i
 /* seq_len <= 128: any causal / key_mask; 128 < seq_len <= 1025 (long-sequence kernel): causal = 0, key_mask = NULL. */
 PLIP_API int plip_dbg_attention(const void* qkv_bf16, int64_t n_seq, int seq_len, int heads, int causal,
                                 const int32_t* key_mask, void* out_bf16, void* stream);
+/* The attention probabilities of plip_dbg_attention's input: probs_dev float32 [n_seq, heads, seq_len, seq_len], any
+ * causal / key_mask, 1 <= seq_len <= 1025. */
+PLIP_API int plip_dbg_attention_probs(const void* qkv_bf16, int64_t n_seq, int seq_len, int heads, int causal,
+                                      const int32_t* key_mask, float* probs_dev, void* stream);
 PLIP_API int plip_dbg_im2col(const void* pixels, int pixel_format, int64_t n, void* out_bf16, void* stream);
 /* The vision position table pos_dev (float32 [50,768]) resized to a grid_h x grid_w patch grid as
  * plip_encode_images_hw does it: out_dev float32 [1 + grid_h * grid_w, 768]; 1 <= grid_h, grid_w <= 32. */

@@ -54,6 +54,13 @@ class ResizeDesc(C.Structure):
     ]
 
 
+class TowerOutputs(C.Structure):
+    """Mirror of ``plip_tower_outputs_t`` (device pointers, 0 = not requested)."""
+
+    _fields_ = [("embeds", C.c_void_p), ("pooled", C.c_void_p), ("last_hidden", C.c_void_p), ("hidden", C.c_void_p),
+                ("attn", C.c_void_p), ("normalize", C.c_int32)]
+
+
 # name -> (restype, argtypes); must list every PLIP_API symbol of include/plip_b200.h
 SIGNATURES = {
     "plip_last_error": (C.c_char_p, []),
@@ -77,6 +84,8 @@ SIGNATURES = {
     "plip_encode_images_hw": (_i, [_vp, _vp, _i, _i64, _i, _i, _fp, _i, _vp]),
     "plip_encode_text": (_i, [_vp, _vp, _i, _vp, _i64, _i, _fp, _i, _vp]),
     "plip_encode_text_prefix": (_i, [_vp, _vp, _i, _vp, _i64, _i, _i, _fp, _i, _vp]),
+    "plip_vision_outputs": (_i, [_vp, _vp, _i, _i64, _i, _i, C.POINTER(TowerOutputs), _vp]),
+    "plip_text_outputs": (_i, [_vp, _vp, _i, _vp, _i64, _i, C.POINTER(TowerOutputs), _vp]),
     "plip_similarity": (_i, [_fp, _i64, _fp, _i64, _f, _i, _i, _fp, _i64, _vp]),
     "plip_similarity_topk": (_i, [_fp, _i64, _fp, _i64, _f, _i, _i, _i, _vp, _fp, _vp]),
     "plip_l2_normalize": (_i, [_fp, _i64, _i, _vp]),
@@ -91,6 +100,7 @@ SIGNATURES = {
     "plip_dbg_rowstats_cast": (_i, [_fp, _i64, _i, _vp, _fp, _vp]),
     "plip_dbg_layernorm": (_i, [_fp, _i64, _i, _i64, _fp, _fp, _fp, _vp, _vp]),
     "plip_dbg_attention": (_i, [_vp, _i64, _i, _i, _i, _vp, _vp, _vp]),
+    "plip_dbg_attention_probs": (_i, [_vp, _i64, _i, _i, _i, _vp, _fp, _vp]),
     "plip_dbg_im2col": (_i, [_vp, _i, _i64, _vp, _vp]),
     "plip_dbg_hidden_states": (_i, [_vp, _i, _vp, _i, _vp, _i64, _i, _fp, _vp]),
     "plip_dbg_pos_interp": (_i, [_fp, _i, _i, _fp, _vp]),

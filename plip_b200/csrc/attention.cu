@@ -432,6 +432,193 @@ int launch_attention_long(const CUtensorMap& tmQKV, const CUtensorMap& tmO, cons
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Attention probabilities (output_attentions): P = softmax(q k^T + mask) in fp32, written as [n_seq, heads, S, S], for
+// any 1 <= S <= kMaxVisSeq with the masks of the kernels above.  It reads the QKV buffer the layer's attention has just
+// read and leaves that kernel alone.  One CTA (one warpgroup) per (sequence, head, block of 64 queries):
+//   TMA      the [64 x 64] Q block once, then 64-key K blocks through a two-stage ring; the 3-D tensor maps
+//            ([n_seq][S][3D], as the long kernel's) zero-fill rows past the sequence's end
+//   pass 1   per key block S = Q K^T (wgmma m64n64k16, ss) -> mask -> running row max m and row sum l (l rescaled by
+//            2^(m_old - m_new)), in fp32 and in a fixed block order
+//   pass 2   S recomputed per key block -> exp2(s log2e - m log2e) / l -> the warp's 16 rows of a padded fp32 staging
+//            tile -> global: each warp store instruction writes 32 consecutive floats of the output (128 B), walking
+//            the block's rows x columns in output order, so with one key block (S <= 64) a warp's rows are one
+//            contiguous run.  Streaming stores: the probabilities are not read again.
+// When S <= 128 both key blocks stay in the ring and pass 2 loads nothing.  A row without a visible key (text with a
+// padded first position) has l = 0 and is written as zeros, like the zero output row of the attention kernel.
+// The output rows are S * 4 bytes and not 16-byte aligned for odd S: no TMA store can write them.
+constexpr int kProbThreads = 128;
+constexpr int kProbStages = 2;
+constexpr int kProbLd = 72;                                    // staging row stride in floats: conflict-free float2 writes
+constexpr uint32_t kProbTileBytes = 64 * 64 * 2;               // one [64 x 64] 16-bit operand block
+constexpr uint32_t kProbStageOff = kProbTileBytes;             // K ring after the Q block
+constexpr uint32_t kProbStagingOff = kProbStageOff + kProbStages * kProbTileBytes;
+constexpr uint32_t kProbBarOff = kProbStagingOff + 64 * kProbLd * 4;
+constexpr uint32_t kProbSmem = kProbBarOff + 8 * (1 + kProbStages) + 1024;
+
+struct ProbParams {
+  int seq_len;
+  int heads;
+  int q_blocks;  // ceil(S / 64)
+  int causal;
+  const int32_t* key_mask;  // [n_seq, S] or nullptr
+  float* probs;             // [n_seq, heads, S, S]
+};
+
+template <bool F16>
+__global__ void __launch_bounds__(kProbThreads)
+attention_probs_kernel(const __grid_constant__ CUtensorMap tmQKV, const ProbParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  float* staging = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw)) + kProbStagingOff);
+  const uint32_t sq = smem_base;
+  auto sk = [&](int s) { return smem_base + kProbStageOff + (uint32_t)s * kProbTileBytes; };
+  const uint32_t q_bar = smem_base + kProbBarOff;
+  auto full_bar = [&](int s) { return q_bar + 8u * (1 + s); };
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int S = p.seq_len, D = p.heads * kHeadDim;
+  const int qb = blockIdx.x % p.q_blocks;
+  const int64_t bh = blockIdx.x / p.q_blocks;
+  const int h = (int)(bh % p.heads);
+  const int64_t seq = bh / p.heads;
+  const int q0 = qb * 64;
+  const int n_kb = (S + 63) / 64;
+  const bool resident = n_kb <= kProbStages;        // every key block fits the ring: pass 2 reuses them
+  const int n_loads = resident ? n_kb : 2 * n_kb;   // load i: key block i % n_kb into stage i % kProbStages
+
+  auto issue_k = [&](int i) {
+    const int s = i % kProbStages;
+    mbar_arrive_expect_tx(full_bar(s), kProbTileBytes);
+    tma_load_3d(sk(s), &tmQKV, full_bar(s), D + h * kHeadDim, (i % n_kb) * 64, (int32_t)seq);
+  };
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmQKV);
+    mbar_init(q_bar, 1);
+    for (int s = 0; s < kProbStages; ++s) mbar_init(full_bar(s), 1);
+    fence_mbar_init();
+    mbar_arrive_expect_tx(q_bar, kProbTileBytes);
+    tma_load_3d(sq, &tmQKV, q_bar, h * kHeadDim, q0, (int32_t)seq);
+    for (int i = 0; i < kProbStages && i < n_loads; ++i) issue_k(i);
+  }
+  __syncthreads();
+
+  const int q4 = lane & 3, rr = lane >> 2;
+  const int r0 = 16 * warp + rr;                    // this thread's block rows r0 and r0 + 8
+  const int qa = q0 + r0, qc = qa + 8;              // their queries
+  const int lim0 = qa < S ? (p.causal ? qa : S - 1) : -1;   // last visible key of each row
+  const int lim1 = qc < S ? (p.causal ? qc : S - 1) : -1;
+  const int32_t* km = p.key_mask ? p.key_mask + seq * S : nullptr;
+  constexpr float kLog2e = 1.4426950408889634f;
+  const uint64_t qdesc = make_smem_desc_sw128(sq, 1024, 16);
+  mbar_wait(q_bar, 0);
+
+  // S = Q K^T for use u (key block u % n_kb), masked entries -> -inf
+  float sc[32];
+  auto scores = [&](int u) {
+    const int li = resident ? u % n_kb : u;
+    const int s = li % kProbStages;
+    mbar_wait(full_bar(s), (uint32_t)((li / kProbStages) & 1));
+    const uint64_t kdesc = make_smem_desc_sw128(sk(s), 1024, 16);
+    wgmma_pin(sc);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kHeadDim / 16; ++k) wgmma_ss_n64<F16>(sc, qdesc + 2 * k, kdesc + 2 * k, k != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_pin(sc);
+    if (!resident) {
+      __syncthreads();  // every warp is done with the stage: refill it
+      if (threadIdx.x == 0 && li + kProbStages < n_loads) issue_k(li + kProbStages);
+    }
+    const int kbase = (u % n_kb) * 64 + 2 * q4;     // + 8 j + e = key of column (j, e)
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int key = kbase + 8 * j + e;
+        const bool ok = key < S && (km == nullptr || km[key] != 0);
+        if (!(ok && key <= lim0)) sc[4 * j + e] = -INFINITY;
+        if (!(ok && key <= lim1)) sc[4 * j + 2 + e] = -INFINITY;
+      }
+  };
+
+  // ---- pass 1: running row max / sum
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+  for (int kb = 0; kb < n_kb; ++kb) {
+    scores(kb);
+    float mx0 = m0, mx1 = m1;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      mx0 = fmaxf(mx0, fmaxf(sc[4 * j + 0], sc[4 * j + 1]));
+      mx1 = fmaxf(mx1, fmaxf(sc[4 * j + 2], sc[4 * j + 3]));
+    }
+#pragma unroll
+    for (int off = 1; off < 4; off <<= 1) {  // the 4 lanes that share a row
+      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, off));
+      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, off));
+    }
+    const float ms0 = mx0 == -INFINITY ? 0.f : mx0 * kLog2e, ms1 = mx1 == -INFINITY ? 0.f : mx1 * kLog2e;
+    l0 *= fast_exp2(fmaf(m0, kLog2e, -ms0));  // m_old = -inf: l is still 0
+    l1 *= fast_exp2(fmaf(m1, kLog2e, -ms1));
+    m0 = mx0;
+    m1 = mx1;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      l0 += fast_exp2(fmaf(sc[4 * j + 0], kLog2e, -ms0)) + fast_exp2(fmaf(sc[4 * j + 1], kLog2e, -ms0));
+      l1 += fast_exp2(fmaf(sc[4 * j + 2], kLog2e, -ms1)) + fast_exp2(fmaf(sc[4 * j + 3], kLog2e, -ms1));
+    }
+  }
+#pragma unroll
+  for (int off = 1; off < 4; off <<= 1) {
+    l0 += __shfl_xor_sync(0xffffffffu, l0, off);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, off);
+  }
+  const float ms0 = m0 == -INFINITY ? 0.f : m0 * kLog2e, ms1 = m1 == -INFINITY ? 0.f : m1 * kLog2e;
+  const float inv0 = l0 > 0.f ? 1.0f / l0 : 0.f;
+  const float inv1 = l1 > 0.f ? 1.0f / l1 : 0.f;
+
+  // ---- pass 2: probabilities -> staging rows of this warp -> global
+  float* wst = staging + 16 * warp * kProbLd;       // the warp's 16 staging rows
+  const int rows = S - (q0 + 16 * warp) < 16 ? S - (q0 + 16 * warp) : 16;  // its rows that are queries (may be <= 0)
+  float* out_base = p.probs + ((seq * p.heads + h) * (int64_t)S + q0 + 16 * warp) * S;
+  for (int kb = 0; kb < n_kb; ++kb) {
+    scores(n_kb + kb);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float2 a = make_float2(fast_exp2(fmaf(sc[4 * j + 0], kLog2e, -ms0)) * inv0,
+                                   fast_exp2(fmaf(sc[4 * j + 1], kLog2e, -ms0)) * inv0);
+      const float2 b = make_float2(fast_exp2(fmaf(sc[4 * j + 2], kLog2e, -ms1)) * inv1,
+                                   fast_exp2(fmaf(sc[4 * j + 3], kLog2e, -ms1)) * inv1);
+      *reinterpret_cast<float2*>(wst + rr * kProbLd + 8 * j + 2 * q4) = a;
+      *reinterpret_cast<float2*>(wst + (rr + 8) * kProbLd + 8 * j + 2 * q4) = b;
+    }
+    __syncwarp();
+    const int k0 = kb * 64;
+    const int nc = S - k0 < 64 ? S - k0 : 64;       // columns of this key block
+    const int total = rows > 0 ? rows * nc : 0;
+    int r = 0, c = lane;                            // element lane of the block's rows x columns, in output order
+    while (c >= nc) { c -= nc; ++r; }
+    for (int i = lane; i < total; i += 32) {
+      __stcs(out_base + (int64_t)r * S + k0 + c, wst[r * kProbLd + c]);
+      c += 32;
+      while (c >= nc) { c -= nc; ++r; }
+    }
+    __syncwarp();  // the staging rows are rewritten by the next block
+  }
+}
+
+template <bool F16>
+int launch_attention_probs_inst(const CUtensorMap& tmQKV, const ProbParams& p, int64_t blocks, cudaStream_t st) {
+  auto kern = attention_probs_kernel<F16>;
+  static unsigned long long configured = 0;
+  if (first_use_on_device(configured))
+    PLIP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kProbSmem));
+  PLIP_CUDA_CHECK(launch_kernel(kern, dim3((unsigned)blocks), dim3(kProbThreads), kProbSmem, st, 1, tmQKV, p));
+  return 0;
+}
+
 }  // namespace
 
 int launch_attention(const __nv_bfloat16* qkv, int64_t n_seq, int seq_len, int heads, bool causal,
@@ -475,6 +662,28 @@ int launch_attention(const __nv_bfloat16* qkv, int64_t n_seq, int seq_len, int h
   PLIP_REQUIRE(p.seq_tiles * heads < 0x7fffffff, "attention: too many tiles");
   if (p.slot == 128) return f16 ? launch_attention_inst<true, 128>(tmL, tmS, p, st) : launch_attention_inst<false, 128>(tmL, tmS, p, st);
   return f16 ? launch_attention_inst<true, 64>(tmL, tmS, p, st) : launch_attention_inst<false, 64>(tmL, tmS, p, st);
+}
+
+int launch_attention_probs(const __nv_bfloat16* qkv, int64_t n_seq, int seq_len, int heads, bool causal,
+                           const int32_t* key_mask, float* probs, int f16, cudaStream_t st) {
+  PLIP_REQUIRE(qkv && probs, "attention_probs: null argument");
+  PLIP_REQUIRE(n_seq > 0 && seq_len > 0 && seq_len <= kMaxVisSeq, "attention_probs: bad shape n_seq=%lld seq_len=%d",
+               (long long)n_seq, seq_len);
+  PLIP_REQUIRE(heads > 0 && heads <= 16, "attention_probs: bad head count %d", heads);
+  ProbParams p;
+  p.seq_len = seq_len;
+  p.heads = heads;
+  p.q_blocks = (seq_len + 63) / 64;
+  p.causal = causal ? 1 : 0;
+  p.key_mask = key_mask;
+  p.probs = probs;
+  const int64_t blocks = n_seq * heads * p.q_blocks;
+  PLIP_REQUIRE(blocks < 0x7fffffff && n_seq < 0x7fffffff, "attention_probs: too many sequences");
+  const int D = heads * kHeadDim;
+  CUtensorMap tm;
+  if (int rc = make_tmap_bf16_3d(&tm, qkv, (uint64_t)n_seq, (uint64_t)seq_len, (uint64_t)3 * D, (uint64_t)3 * D * 2,
+                                 (uint64_t)seq_len * 3 * D * 2, 64, 64)) return rc;
+  return f16 ? launch_attention_probs_inst<true>(tm, p, blocks, st) : launch_attention_probs_inst<false>(tm, p, blocks, st);
 }
 
 }  // namespace plip

@@ -107,10 +107,11 @@ struct LayerW {
 constexpr int kEosId = 49407;  // TF:configuration_clip.py:63 (eos_token_id)
 
 enum ProfKind { PK_QKV = 0, PK_ATTN, PK_OUT, PK_FC1, PK_FC2, PK_PATCH, PK_IM2COL, PK_LN, PK_ROWSTATS, PK_EMBED, PK_PROJ,
-                PK_MISC, PK_ATTN_LONG, PK_COUNT };
+                PK_MISC, PK_ATTN_LONG, PK_ATTN_PROBS, PK_COUNT };
 const char* const kProfNames[PK_COUNT] = {"gemm[ln1+qkv]", "attention", "gemm[out_proj+resid]", "gemm[ln2+fc1+gelu]",
                                           "gemm[fc2+resid]", "gemm[patch_embed]", "im2col", "layernorm",
-                                          "rowstats_cast", "text_embed", "gemm[projection]", "misc", "attention[long]"};
+                                          "rowstats_cast", "text_embed", "gemm[projection]", "misc", "attention[long]",
+                                          "attention[probs]"};
 
 size_t pixel_bytes(int fmt, int height = kImage, int width = kImage) {
   const size_t px = (size_t)3 * height * width;
@@ -331,6 +332,16 @@ int layer_tail(plip_engine* e, const LayerW& w, int rows, int D, int FF, const _
   return gemm(e, PK_FC2, g, st);
 }
 
+// Optional per-layer outputs of run_layers (plip_vision_outputs / plip_text_outputs); null pointers are not written.
+//   hidden: X [n_seq * S, D] is copied to hidden on entry and to hidden + (l + 1) * hidden_stride after layer l
+//   probs:  the attention probabilities of layer l go to probs + l * probs_stride ([n_seq, heads, S, S] fp32)
+struct Taps {
+  float* hidden = nullptr;
+  int64_t hidden_stride = 0;  // floats between layers
+  float* probs = nullptr;
+  int64_t probs_stride = 0;
+};
+
 // Encoder layers with both LayerNorms folded into the consuming GEMMs.  On entry X holds the residual
 // stream; Xn / stats are (re)derived from it here and afterwards maintained by the residual epilogues.
 //
@@ -339,12 +350,17 @@ int layer_tail(plip_engine* e, const LayerW& w, int rows, int D, int FF, const _
 // attention nothing mixes rows any more, so that layer's out_proj, LN2, fc1 and fc2 are run on the n_seq pooled rows
 // alone (gathered into compact buffers) instead of all n_seq*S rows — same arithmetic per row, identical embeddings.
 // pool_idx: device row indices of the pooled rows (null = row i*S).  On return e->pooled_x points at them.
+// taps (null: none) are never combined with prune.
 int run_layers(plip_engine* e, const LayerW* L, int64_t n_seq, int S, int D, int FF, int heads, bool causal,
                const int32_t* kmask, int num_layers, cudaStream_t st, bool prune = false,
-               const int32_t* pool_idx = nullptr) {
+               const int32_t* pool_idx = nullptr, const Taps* taps = nullptr) {
   e->pooled_x = nullptr;
   const int64_t M = n_seq * S;
   PLIP_REQUIRE(M <= 0x7fffffff / 4, "micro-batch too large");
+  PLIP_REQUIRE(!(taps && prune), "internal: per-layer outputs of a pruned pass");
+  const size_t x_bytes = (size_t)M * D * 4;
+  if (taps && taps->hidden)
+    PLIP_CUDA_CHECK(cudaMemcpyAsync(taps->hidden, e->X, x_bytes, cudaMemcpyDeviceToDevice, st));
   if (num_layers <= 0) return 0;
   {
     ProfScope ps(e, st, PK_ROWSTATS, 0, (double)M * D * 6 + (double)M * 8);
@@ -366,8 +382,17 @@ int run_layers(plip_engine* e, const LayerW* L, int64_t n_seq, int S, int D, int
       ProfScope ps(e, st, S > 128 ? PK_ATTN_LONG : PK_ATTN, f_att, b_att);
       if (int rc = launch_attention(e->QKV, n_seq, S, heads, causal, kmask, e->AO, e->f16, st)) return rc;
     }
+    if (taps && taps->probs) {
+      // reads Q and K of QKV (intact until the next layer's QKV GEMM), writes heads * S^2 fp32 per sequence
+      ProfScope ps(e, st, PK_ATTN_PROBS, 0.5 * f_att, (double)M * 2 * D * 2 + (double)n_seq * heads * S * S * 4);
+      if (int rc = launch_attention_probs(e->QKV, n_seq, S, heads, causal, kmask, taps->probs + l * taps->probs_stride,
+                                          e->f16, st)) return rc;
+    }
     if (!(prune && last)) {
       if (int rc = layer_tail(e, w, (int)M, D, FF, e->AO, e->X, last, np, st)) return rc;
+      if (taps && taps->hidden)
+        PLIP_CUDA_CHECK(cudaMemcpyAsync(taps->hidden + (l + 1) * taps->hidden_stride, e->X, x_bytes,
+                                        cudaMemcpyDeviceToDevice, st));
       continue;
     }
     // compact copies of the pooled rows: attention output -> head of the (now free) QKV buffer, residual rows behind it
@@ -385,7 +410,7 @@ int run_layers(plip_engine* e, const LayerW* L, int64_t n_seq, int S, int D, int
 
 // Vision tower up to (and including) `num_layers` encoder layers; X holds the residual stream [mb * geo.S, 768].
 int vision_trunk(plip_engine* e, const void* pixels, int fmt, int64_t mb, const VisGeom& geo, int num_layers,
-                 cudaStream_t st, bool prune = false) {
+                 cudaStream_t st, bool prune = false, const Taps* taps = nullptr) {
   e->prof_tower = 0;
   const double dmb = (double)mb;
   const int patches = geo.gh * geo.gw;
@@ -416,20 +441,24 @@ int vision_trunk(plip_engine* e, const void* pixels, int fmt, int64_t mb, const 
     ProfScope ps(e, st, PK_LN, 0, (double)M * kVisDim * 8);
     if (int rc = launch_layernorm(e->X, nullptr, kVisDim, M, kVisDim, e->v_pre_g, e->v_pre_b, e->X, nullptr, e->f16, st)) return rc;
   }
-  return run_layers(e, e->vis, mb, geo.S, kVisDim, kVisFF, kVisHeads, false, nullptr, num_layers, st, prune, nullptr);
+  return run_layers(e, e->vis, mb, geo.S, kVisDim, kVisFF, kVisHeads, false, nullptr, num_layers, st, prune, nullptr,
+                    taps);
 }
 
 // Tower head: LayerNorm of the pooled rows -> projection [-> L2 normalise].  The pooled rows are the compact
 // e->pooled_x rows when the last layer was pruned, else rows pool_idx[i] of X (null: row i*S).
+// pooled_f32 (optional): the LayerNorm-ed pooled rows in fp32 as well, [mb, D] (pooler_output); out null: no projection.
 int pooled_head(plip_engine* e, const int32_t* pool_idx, int64_t mb, int S, int D, const float* gamma,
-                const float* beta, const __nv_bfloat16* proj, float* out, int normalize, cudaStream_t st) {
+                const float* beta, const __nv_bfloat16* proj, float* out, int normalize, cudaStream_t st,
+                float* pooled_f32 = nullptr) {
   {
-    ProfScope ps(e, st, PK_LN, 0, (double)mb * D * 6);
+    ProfScope ps(e, st, PK_LN, 0, (double)mb * D * (pooled_f32 ? 10 : 6));
     const bool compact = e->pooled_x != nullptr;
     if (int rc = launch_layernorm(compact ? e->pooled_x : e->X, compact ? nullptr : pool_idx,
-                                  compact || pool_idx ? (int64_t)D : (int64_t)S * D, mb, D, gamma, beta, nullptr,
+                                  compact || pool_idx ? (int64_t)D : (int64_t)S * D, mb, D, gamma, beta, pooled_f32,
                                   e->pooled, e->f16, st)) return rc;
   }
+  if (!out) return 0;
   GemmArgs g;
   g.A = e->pooled; g.lda = D; g.W = proj; g.ldw = D;
   g.M = (int)mb; g.N = kProj; g.K = D; g.out = out; g.ldo = kProj; g.epi = EPI_F32;
@@ -452,7 +481,7 @@ int vision_forward(plip_engine* e, const void* pixels, int fmt, int64_t mb, floa
 // Causality makes rows after a caption's first EOS irrelevant to its pooled output (TF:571-584), so callers
 // that know the longest caption of the batch may pass a shorter S: same result, proportionally less work.
 int text_trunk(plip_engine* e, const void* ids, int ids_dtype, const void* mask, int64_t mb, int S, int stride,
-               int num_layers, cudaStream_t st, bool prune = false) {
+               int num_layers, cudaStream_t st, bool prune = false, const Taps* taps = nullptr) {
   e->prof_tower = 1;
   {
     ProfScope ps(e, st, PK_EMBED, 0, (double)mb * S * kTxtDim * 8);
@@ -464,7 +493,7 @@ int text_trunk(plip_engine* e, const void* ids, int ids_dtype, const void* mask,
     if (int rc = launch_mask_to_i32(mask, ids_dtype, mb * S, S, stride, e->kmask, st)) return rc;
     km = e->kmask;
   }
-  return run_layers(e, e->txt, mb, S, kTxtDim, kTxtFF, kTxtHeads, true, km, num_layers, st, prune, e->row_idx);
+  return run_layers(e, e->txt, mb, S, kTxtDim, kTxtFF, kTxtHeads, true, km, num_layers, st, prune, e->row_idx, taps);
 }
 
 int text_forward(plip_engine* e, const void* ids, int ids_dtype, const void* mask, int64_t mb, int S, int stride,
@@ -629,6 +658,55 @@ int check_hw_call(const char* fn, const plip_engine* e, const void* in, const vo
                "(%d x max_micro_batch %d); create the engine with max_micro_batch >= %d",
                fn, height, width, S, (long long)kVisSeq * e->max_mb, kVisSeq, e->max_mb, (S + kVisSeq - 1) / kVisSeq);
   return 0;
+}
+
+// ---- per-layer outputs (plip_vision_outputs / plip_text_outputs) ----------------------------------------------------
+int check_outputs(const char* fn, const plip_tower_outputs_t* o) {
+  PLIP_REQUIRE(o != nullptr, "%s: null outputs", fn);
+  PLIP_REQUIRE(o->embeds || o->pooled || o->last_hidden || o->hidden || o->attn, "%s: no output requested", fn);
+  return 0;
+}
+
+// The taps of micro-batch [i0, i0 + mb) of an n-sequence call: the caller's [13, n, S, D] / [12, n, heads, S, S] buffers
+// at the micro-batch's offsets.
+Taps outputs_taps(const plip_tower_outputs_t* o, int64_t n, int64_t i0, int S, int D, int heads) {
+  Taps t;
+  const int64_t tok = (int64_t)S * D, pp = (int64_t)heads * S * S;
+  if (o->hidden) { t.hidden = o->hidden + i0 * tok; t.hidden_stride = n * tok; }
+  if (o->attn) { t.probs = o->attn + i0 * pp; t.probs_stride = n * pp; }
+  return t;
+}
+
+// One vision pass over images [i0, i0 + mb) of n: the full tower (never pruned), then the requested outputs.
+// last_hidden_state is the residual stream after the last layer, before post_layernorm (TF:modeling_clip.py:680-686).
+int vision_outputs_pass(plip_engine* e, const void* pixels, int fmt, int64_t mb, int64_t i0, int64_t n,
+                        const VisGeom& geo, const plip_tower_outputs_t* o, cudaStream_t st) {
+  const Taps t = outputs_taps(o, n, i0, geo.S, kVisDim, kVisHeads);
+  if (int rc = vision_trunk(e, pixels, fmt, mb, geo, kLayers, st, false, &t)) return rc;
+  if (o->last_hidden)
+    PLIP_CUDA_CHECK(cudaMemcpyAsync(o->last_hidden + i0 * geo.S * kVisDim, e->X, (size_t)mb * geo.S * kVisDim * 4,
+                                    cudaMemcpyDeviceToDevice, st));
+  if (!o->embeds && !o->pooled) return 0;
+  return pooled_head(e, nullptr, mb, geo.S, kVisDim, e->v_post_g, e->v_post_b, e->v_proj,
+                     o->embeds ? o->embeds + i0 * kProj : nullptr, o->normalize, st,
+                     o->pooled ? o->pooled + i0 * kVisDim : nullptr);
+}
+
+// One text pass over captions [i0, i0 + mb) of n at the full seq_len (every position is an output).
+// last_hidden_state = final_layer_norm of every row (TF:562); pooler_output its pooled row (TF:571-584).
+int text_outputs_pass(plip_engine* e, const void* ids, int ids_dtype, const void* mask, int64_t mb, int S, int64_t i0,
+                      int64_t n, const plip_tower_outputs_t* o, cudaStream_t st) {
+  const Taps t = outputs_taps(o, n, i0, S, kTxtDim, kTxtHeads);
+  if (int rc = text_trunk(e, ids, ids_dtype, mask, mb, S, S, kLayers, st, false, &t)) return rc;
+  if (o->last_hidden) {
+    ProfScope ps(e, st, PK_LN, 0, (double)mb * S * kTxtDim * 8);
+    if (int rc = launch_layernorm(e->X, nullptr, kTxtDim, mb * S, kTxtDim, e->t_fin_g, e->t_fin_b,
+                                  o->last_hidden + i0 * S * kTxtDim, nullptr, e->f16, st)) return rc;
+  }
+  if (!o->embeds && !o->pooled) return 0;
+  return pooled_head(e, e->row_idx, mb, S, kTxtDim, e->t_fin_g, e->t_fin_b, e->t_proj,
+                     o->embeds ? o->embeds + i0 * kProj : nullptr, o->normalize, st,
+                     o->pooled ? o->pooled + i0 * kTxtDim : nullptr);
 }
 
 bool graph_eligible(const plip_engine* e, int64_t n) {
@@ -941,6 +1019,47 @@ PLIP_API int plip_encode_text_prefix(plip_engine_t* e, const void* ids_dev, int 
   return 0;
 }
 
+PLIP_API int plip_vision_outputs(plip_engine_t* e, const void* pixels_dev, int pixel_format, int64_t n, int height,
+                                 int width, const plip_tower_outputs_t* outputs, void* stream) {
+  if (int rc = check_outputs("plip_vision_outputs", outputs)) return rc;
+  if (int rc = check_hw_call("plip_vision_outputs", e, pixels_dev, outputs, pixel_format, n, height, width)) return rc;
+  const VisGeom geo = vis_geom(height, width);
+  const int64_t per_pass = images_per_pass(e->max_mb, geo.S);
+  const size_t pb = pixel_bytes(pixel_format, height, width);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_last, 0));  // calls on different streams share one workspace
+  for (int64_t i = 0; i < n; i += per_pass) {
+    const int64_t mb = (n - i < per_pass) ? (n - i) : per_pass;
+    if (int rc = vision_outputs_pass(e, static_cast<const uint8_t*>(pixels_dev) + i * pb, pixel_format, mb, i, n, geo,
+                                     outputs, st)) return rc;
+  }
+  PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
+  return 0;
+}
+
+PLIP_API int plip_text_outputs(plip_engine_t* e, const void* ids_dev, int ids_dtype, const void* attention_mask_dev,
+                               int64_t n, int seq_len, const plip_tower_outputs_t* outputs, void* stream) {
+  PLIP_REQUIRE(ids_dev && outputs, "plip_text_outputs: null argument");
+  PLIP_REQUIRE(n > 0, "plip_text_outputs: n must be positive (got %lld)", (long long)n);
+  PLIP_REQUIRE(seq_len >= 1 && seq_len <= kTxtSeq,
+               "Sequence length must be less than max_position_embeddings (got `sequence length`: %d and "
+               "max_position_embeddings: %d)", seq_len, kTxtSeq);  // message mirrors TF:243-247
+  PLIP_REQUIRE(ids_dtype == PLIP_IDS_I32 || ids_dtype == PLIP_IDS_I64, "plip_text_outputs: unknown ids dtype %d", ids_dtype);
+  if (int rc = check_outputs("plip_text_outputs", outputs)) return rc;
+  PLIP_REQUIRE(e != nullptr, "plip_text_outputs: null engine");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_last, 0));
+  const size_t isz = ids_dtype == PLIP_IDS_I64 ? 8 : 4;
+  for (int64_t i = 0; i < n; i += e->max_mb) {
+    const int64_t mb = (n - i < e->max_mb) ? (n - i) : e->max_mb;
+    const uint8_t* ids = static_cast<const uint8_t*>(ids_dev) + i * seq_len * isz;
+    const uint8_t* mk = attention_mask_dev ? static_cast<const uint8_t*>(attention_mask_dev) + i * seq_len * isz : nullptr;
+    if (int rc = text_outputs_pass(e, ids, ids_dtype, mk, mb, seq_len, i, n, outputs, st)) return rc;
+  }
+  PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
+  return 0;
+}
+
 PLIP_API int plip_similarity(const float* img_dev, int64_t n, const float* txt_dev, int64_t m, float scale,
                              int normalize_img, int normalize_txt, float* logits_dev, int64_t ld_logits,
                              void* stream) {
@@ -1154,6 +1273,12 @@ PLIP_API int plip_dbg_attention(const void* qkv_bf16, int64_t n_seq, int seq_len
                                 const int32_t* key_mask, void* out_bf16, void* stream) {
   return launch_attention(static_cast<const __nv_bfloat16*>(qkv_bf16), n_seq, seq_len, heads, causal != 0, key_mask,
                           static_cast<__nv_bfloat16*>(out_bf16), g_dbg_f16, static_cast<cudaStream_t>(stream));
+}
+
+PLIP_API int plip_dbg_attention_probs(const void* qkv_bf16, int64_t n_seq, int seq_len, int heads, int causal,
+                                      const int32_t* key_mask, float* probs_dev, void* stream) {
+  return launch_attention_probs(static_cast<const __nv_bfloat16*>(qkv_bf16), n_seq, seq_len, heads, causal != 0,
+                                key_mask, probs_dev, g_dbg_f16, static_cast<cudaStream_t>(stream));
 }
 
 PLIP_API int plip_dbg_im2col(const void* pixels, int pixel_format, int64_t n, void* out_bf16, void* stream) {

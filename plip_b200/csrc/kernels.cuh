@@ -40,6 +40,10 @@ int resize_filter_host(int in_size, int out_size, int xx, int32_t* k, int k_cap,
 // f16 = 1: q, k, v, P and the output are IEEE half instead of bfloat16 (the engine's operand format).
 int launch_attention(const __nv_bfloat16* qkv, int64_t n_seq, int seq_len, int heads, bool causal,
                      const int32_t* key_mask, __nv_bfloat16* out, int f16, cudaStream_t st);
+// The softmax probabilities of the same call, fp32 [n_seq, heads, seq_len, seq_len] (output_attentions), for any
+// seq_len <= kMaxVisSeq with any causal / key mask.  A row without a visible key is written as zeros.
+int launch_attention_probs(const __nv_bfloat16* qkv, int64_t n_seq, int seq_len, int heads, bool causal,
+                           const int32_t* key_mask, float* probs, int f16, cudaStream_t st);
 
 // similarity.cu
 int launch_similarity(const float* a, int64_t n, const float* b, int64_t m, float scale, bool norm_a, bool norm_b,

@@ -3,7 +3,7 @@ C ABI (``libplip_b200.so``).  There is no fallback path: a missing library or GP
 from __future__ import annotations
 
 import ctypes as C
-from typing import Mapping, Optional, Tuple, Union
+from typing import Dict, Mapping, Optional, Tuple, Union
 
 import numpy as np
 import torch
@@ -17,6 +17,10 @@ EMBED_DIM = 512
 IMAGE_SIZE = 224
 MAX_TEXT_LEN = 77
 
+
+VISION_DIM, VISION_HEADS = 768, 12
+TEXT_DIM, TEXT_HEADS = 512, 8
+NUM_LAYERS = 12
 
 PATCH = 32
 MAX_GRID = 32  # interpolate_pos_encoding: at most 32 x 32 patches (1024 px per side, 1025 tokens)
@@ -280,6 +284,80 @@ class Engine:
                 check(self._L.plip_resize_crop_u8(src.data_ptr(), int(src.numel()), descs.ctypes.data, n,
                                                   out.data_ptr(), self._stream()), "plip_resize_crop_u8")
         return out
+
+    # ---- per-token outputs (output_hidden_states / output_attentions) ----------------------------------------------
+    def _outputs(self, n: int, S: int, D: int, heads: int, output_hidden_states: bool, output_attentions: bool,
+                 last_hidden_from_hidden: bool):
+        """Allocate the buffers of one outputs call; returns ``(ctypes struct, dict of tensors)``."""
+        from ._lib import TowerOutputs
+        f32 = dict(device=self.device, dtype=torch.float32)
+        out = {"embeds": torch.empty(n, EMBED_DIM, **f32), "pooler_output": torch.empty(n, D, **f32),
+               "hidden": torch.empty(NUM_LAYERS + 1, n, S, D, **f32) if output_hidden_states else None,
+               "attn": torch.empty(NUM_LAYERS, n, heads, S, S, **f32) if output_attentions else None}
+        if last_hidden_from_hidden and out["hidden"] is not None:
+            out["last_hidden_state"] = out["hidden"][NUM_LAYERS]
+        else:
+            out["last_hidden_state"] = torch.empty(n, S, D, **f32)
+        own_last = out["hidden"] is None or not last_hidden_from_hidden
+        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+        st = TowerOutputs(ptr(out["embeds"]), ptr(out["pooler_output"]),
+                          ptr(out["last_hidden_state"]) if own_last else None, ptr(out["hidden"]), ptr(out["attn"]), 0)
+        return st, out
+
+    @staticmethod
+    def _outputs_result(out) -> Dict[str, object]:
+        hid, att = out.pop("hidden"), out.pop("attn")
+        out["hidden_states"] = tuple(hid.unbind(0)) if hid is not None else None
+        out["attentions"] = tuple(att.unbind(0)) if att is not None else None
+        return out
+
+    @torch.no_grad()
+    def vision_outputs(self, pixels: torch.Tensor, output_hidden_states: bool = False, output_attentions: bool = False,
+                       interpolate_pos_encoding: bool = False, normalize: bool = False) -> Dict[str, object]:
+        """One vision tower pass that returns, as fp32 device tensors (``plip_vision_outputs``):
+
+        - ``embeds`` ``[n,512]``: what ``encode_images`` returns (L2-normalised with ``normalize``), bit for bit;
+        - ``pooler_output`` ``[n,768]``: ``post_layernorm`` of the CLS row, not projected;
+        - ``last_hidden_state`` ``[n,S,768]``: the residual stream after the last layer, before ``post_layernorm``;
+        - ``hidden_states``: 13 views ``[n,S,768]`` of one ``[13,n,S,768]`` tensor (``output_hidden_states``):
+          ``[0]`` after ``pre_layrnorm``, ``[l]`` after layer ``l``; ``last_hidden_state`` is then ``hidden_states[12]``;
+        - ``attentions``: 12 views ``[n,12,S,S]`` of one ``[12,n,12,S,S]`` tensor (``output_attentions``).
+
+        ``S = vision_seq_len(H, W)`` (50 at 224 x 224).  The attentions take ``12 * 12 * S^2 * 4`` bytes per image
+        (1.4 MB at 224 x 224, 605 MB at 1024 x 1024)."""
+        fmt = _pixel_format(pixels, interpolate_pos_encoding)
+        h, w = _pixel_hw(pixels, fmt)
+        n, S = int(pixels.shape[0]), vision_seq_len(h, w)
+        st, out = self._outputs(n, S, VISION_DIM, VISION_HEADS, output_hidden_states, output_attentions, True)
+        st.normalize = int(bool(normalize))
+        if n:
+            pixels = self._dev(pixels)
+            with torch.cuda.device(self.device):
+                check(self._L.plip_vision_outputs(self._h, pixels.data_ptr(), fmt, n, h, w, C.byref(st),
+                                                  self._stream()), "plip_vision_outputs")
+        return self._outputs_result(out)
+
+    @torch.no_grad()
+    def text_outputs(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor] = None,
+                     output_hidden_states: bool = False, output_attentions: bool = False,
+                     normalize: bool = False) -> Dict[str, object]:
+        """One text tower pass over all ``seq_len`` positions (``plip_text_outputs``); the keys of ``vision_outputs``:
+        ``embeds`` (``encode_text``'s result, bit for bit), ``pooler_output`` ``[n,512]`` (the pooled row of
+        ``last_hidden_state``), ``last_hidden_state`` ``[n,S,512]`` (``final_layer_norm`` of every row),
+        ``hidden_states`` (13 x ``[n,S,512]``, ``[0]`` = token + position embeddings) and ``attentions``
+        (12 x ``[n,8,S,S]``; masked keys are 0, a row with no visible key is all zeros)."""
+        n, s = _check_ids(input_ids, attention_mask)
+        idt = _ids_dtype(input_ids.dtype)
+        st, out = self._outputs(n, s, TEXT_DIM, TEXT_HEADS, output_hidden_states, output_attentions, False)
+        st.normalize = int(bool(normalize))
+        if n:
+            ids = self._dev(input_ids)
+            mask = self._dev(attention_mask.to(input_ids.dtype)) if attention_mask is not None else None
+            with torch.cuda.device(self.device):
+                check(self._L.plip_text_outputs(self._h, ids.data_ptr(), idt,
+                                                mask.data_ptr() if mask is not None else None, n, s, C.byref(st),
+                                                self._stream()), "plip_text_outputs")
+        return self._outputs_result(out)
 
     # ---- host-buffer API (copies inside the call) ------------------------------------------------
     def encode_images_host(self, pixels: Union[np.ndarray, torch.Tensor], normalize: bool = False,

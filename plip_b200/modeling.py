@@ -12,7 +12,7 @@ the ``[n,512]`` tensor itself — the reference calls ``.detach().cpu().numpy()`
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Mapping, Optional, Union
+from typing import Mapping, Optional, Tuple, Union
 
 import torch
 
@@ -20,20 +20,48 @@ from .engine import Engine
 
 
 @dataclass
+class BaseModelOutputWithPooling:
+    """``transformers.modeling_outputs.BaseModelOutputWithPooling``: what ``vision_model`` / ``text_model`` return.
+    ``keys()`` lists the fields that are set, in HF's order."""
+
+    last_hidden_state: torch.Tensor
+    pooler_output: torch.Tensor
+    hidden_states: Optional[Tuple[torch.Tensor, ...]] = None
+    attentions: Optional[Tuple[torch.Tensor, ...]] = None
+
+    def __getitem__(self, k):
+        return getattr(self, k)
+
+    def keys(self):
+        return tuple(k for k in ("last_hidden_state", "pooler_output", "hidden_states", "attentions")
+                     if getattr(self, k) is not None)
+
+
+@dataclass
 class CLIPOutput:
-    """Fields of ``transformers.models.clip.modeling_clip.CLIPOutput`` (TF:104-135) that the engine produces."""
+    """Fields of ``transformers.models.clip.modeling_clip.CLIPOutput`` (TF:104-135) that the engine produces.
+    ``text_model_output`` / ``vision_model_output`` are set only by a forward with ``output_hidden_states`` or
+    ``output_attentions``, and listed by ``keys()`` only then."""
 
     logits_per_image: torch.Tensor
     logits_per_text: torch.Tensor
     text_embeds: torch.Tensor
     image_embeds: torch.Tensor
     loss: Optional[torch.Tensor] = None
+    text_model_output: Optional[BaseModelOutputWithPooling] = None
+    vision_model_output: Optional[BaseModelOutputWithPooling] = None
 
     def __getitem__(self, k):
         return getattr(self, k)
 
     def keys(self):
-        return ("logits_per_image", "logits_per_text", "text_embeds", "image_embeds")
+        return ("logits_per_image", "logits_per_text", "text_embeds", "image_embeds") + tuple(
+            k for k in ("text_model_output", "vision_model_output") if getattr(self, k) is not None)
+
+
+def _model_output(o) -> BaseModelOutputWithPooling:
+    return BaseModelOutputWithPooling(last_hidden_state=o["last_hidden_state"], pooler_output=o["pooler_output"],
+                                      hidden_states=o["hidden_states"], attentions=o["attentions"])
 
 
 class PlipCLIPModel:
@@ -116,16 +144,46 @@ class PlipCLIPModel:
             raise ValueError("You have to specify input_ids")  # TF:540-541
         return self.engine.encode_text(input_ids, attention_mask)
 
+    def vision_model(self, pixel_values: torch.Tensor = None, output_hidden_states: bool = False,
+                     output_attentions: bool = False, interpolate_pos_encoding: bool = False) -> BaseModelOutputWithPooling:
+        """``CLIPModel.vision_model(...)`` (TF:667-691): ``last_hidden_state`` ``[n,S,768]`` (before post_layernorm),
+        ``pooler_output`` ``[n,768]`` (post_layernorm of the CLS row, not projected), and with the flags the 13
+        ``hidden_states`` and 12 ``attentions`` ``[n,12,S,S]`` (eager-attention values), all from one tower pass."""
+        if pixel_values is None:
+            raise ValueError("You have to specify pixel_values")  # TF:670-671
+        return _model_output(self.engine.vision_outputs(pixel_values, bool(output_hidden_states), bool(output_attentions),
+                                                        interpolate_pos_encoding))
+
+    def text_model(self, input_ids: torch.Tensor = None, attention_mask: Optional[torch.Tensor] = None,
+                   output_hidden_states: bool = False, output_attentions: bool = False) -> BaseModelOutputWithPooling:
+        """``CLIPModel.text_model(...)`` (TF:531-589): ``last_hidden_state`` ``[n,S,512]`` (after final_layer_norm),
+        ``pooler_output`` ``[n,512]`` (its pooled row, not projected), and with the flags the 13 ``hidden_states`` and
+        12 ``attentions`` ``[n,8,S,S]`` (eager-attention values; a row with no visible key is all zeros)."""
+        if input_ids is None:
+            raise ValueError("You have to specify input_ids")  # TF:540-541
+        return _model_output(self.engine.text_outputs(input_ids, attention_mask, bool(output_hidden_states),
+                                                      bool(output_attentions)))
+
     def forward(self, input_ids: torch.Tensor = None, pixel_values: torch.Tensor = None,
                 attention_mask: Optional[torch.Tensor] = None, return_loss: Optional[bool] = None,
-                interpolate_pos_encoding: bool = False, **_ignored) -> CLIPOutput:
-        """TF:867-944 — both towers, L2-normalise, ``exp(logit_scale) * I . T^T``."""
+                interpolate_pos_encoding: bool = False, output_hidden_states: Optional[bool] = None,
+                output_attentions: Optional[bool] = None, **_ignored) -> CLIPOutput:
+        """TF:867-944 — both towers, L2-normalise, ``exp(logit_scale) * I . T^T``.  With ``output_hidden_states`` or
+        ``output_attentions`` each tower runs once through ``vision_model`` / ``text_model``'s path, which also fills
+        ``vision_model_output`` / ``text_model_output``; the embeddings and logits are the same either way."""
         if input_ids is None:
             raise ValueError("You have to specify input_ids")
         if pixel_values is None:
             raise ValueError("You have to specify pixel_values")
         ipe = interpolate_pos_encoding
-        if not pixel_values.is_cuda:
+        vout = tout = None
+        if output_hidden_states or output_attentions:
+            ohs, oa = bool(output_hidden_states), bool(output_attentions)
+            vo = self.engine.vision_outputs(pixel_values, ohs, oa, ipe, normalize=True)
+            to = self.engine.text_outputs(input_ids, attention_mask, ohs, oa, normalize=True)
+            img, txt = vo.pop("embeds"), to.pop("embeds")
+            vout, tout = _model_output(vo), _model_output(to)
+        elif not pixel_values.is_cuda:
             # host inputs (an extension: HF would raise on a device mismatch): the pixel upload runs on the engine's
             # copy stream while the text tower computes, so ~3 ms of PCIe time per 1024 uint8 tiles stay hidden
             # ... and batches larger than one micro-batch are uploaded micro-batch by micro-batch, each one computed as
@@ -147,7 +205,8 @@ class PlipCLIPModel:
             lpt = lpi.t()
             tgt = torch.arange(lpt.shape[0], device=lpt.device)
             loss = (torch.nn.functional.cross_entropy(lpt, tgt) + torch.nn.functional.cross_entropy(lpt.t(), tgt)) / 2
-        return CLIPOutput(logits_per_image=lpi, logits_per_text=lpi.t(), text_embeds=txt, image_embeds=img, loss=loss)
+        return CLIPOutput(logits_per_image=lpi, logits_per_text=lpi.t(), text_embeds=txt, image_embeds=img, loss=loss,
+                          text_model_output=tout, vision_model_output=vout)
 
     __call__ = forward
 
