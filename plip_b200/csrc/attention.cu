@@ -19,6 +19,8 @@
 // One CTA runs this chain serially per tile; with 48 KB of operands several CTAs co-reside per SM and hide each
 // other's load -> MMA -> softmax -> MMA -> store latency.
 // Sequences longer than 128 (vision at more than 256 x 256 pixels) go to attention_long_kernel below.
+#include <cfloat>
+
 #include "kernels.cuh"
 #include "wgmma.cuh"
 
@@ -37,6 +39,109 @@ __device__ __forceinline__ float fast_exp2(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
+constexpr float kLog2e = 1.4426950408889634f;
+
+// ---- Per-block steps shared by the three kernels.  A thread's scores are its part of a wgmma accumulator
+// (wgmma.cuh): a row pair, s[4 j + e] in row 0 and s[4 j + 2 + e] in row 1 (8 rows further), both at column
+// 8 j + 2 q4 + e.  Each step is written once, so the kernels that use it share its masks, fp32 operations and order.
+
+// S = Q K^T for one warpgroup: 64 query rows (qdesc) x NK keys (kdesc), K-major SWIZZLE_128B tiles, dh = 64.
+template <bool F16, int NK>
+__device__ __forceinline__ void qk_scores(float (&s)[NK / 2], uint64_t qdesc, uint64_t kdesc) {
+  wgmma_pin(s);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < kHeadDim / 16; ++k) {
+    if constexpr (NK == 64) wgmma_ss_n64<F16>(s, qdesc + 2 * k, kdesc + 2 * k, k != 0 ? 1u : 0u);
+    else wgmma_ss_n128<F16>(s, qdesc + 2 * k, kdesc + 2 * k, k != 0 ? 1u : 0u);
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_pin(s);
+}
+
+// Row max / row sum of a row pair over the 4 lanes that share its accumulator rows.
+__device__ __forceinline__ void quad_max(float& a, float& b) {
+#pragma unroll
+  for (int o = 1; o < 4; o <<= 1) {
+    a = fmaxf(a, __shfl_xor_sync(0xffffffffu, a, o));
+    b = fmaxf(b, __shfl_xor_sync(0xffffffffu, b, o));
+  }
+}
+__device__ __forceinline__ void quad_sum(float& a, float& b) {
+#pragma unroll
+  for (int o = 1; o < 4; o <<= 1) {
+    a += __shfl_xor_sync(0xffffffffu, a, o);
+    b += __shfl_xor_sync(0xffffffffu, b, o);
+  }
+}
+
+// Last key a query row sees: itself under the causal mask, else the last key; -1 for a row past the sequence's end.
+__device__ __forceinline__ int last_visible_key(int row, int S, int causal) {
+  return row < S ? (causal ? row : S - 1) : -1;
+}
+
+// Key `key` (column (j, e)) is visible to a row when it exists and is not padding (ok) and is not past the row's last
+// visible key; an invisible score becomes -inf, so its exp2 is 0.
+template <int N>
+__device__ __forceinline__ void mask_column(float (&s)[N], int j, int e, bool ok, int key, int lim0, int lim1) {
+  if (!(ok && key <= lim0)) s[4 * j + e] = -INFINITY;
+  if (!(ok && key <= lim1)) s[4 * j + 2 + e] = -INFINITY;
+}
+
+// The empty-row rule: a row without a visible key has max -inf and only -inf scores.  Its shift is clamped to a
+// finite value, so every exp2 is 0 (not NaN from -inf + inf), l = 0 and row_inv(l) = 0: the row comes out as zeros.
+__device__ __forceinline__ float row_shift(float m) { return fmaxf(m * kLog2e, -FLT_MAX); }
+__device__ __forceinline__ float row_inv(float l) { return l > 0.f ? 1.0f / l : 0.f; }
+
+// exp2(s log2e - m log2e) of one score, ms = row_shift(m).
+__device__ __forceinline__ float softmax_exp(float s, float ms) { return fast_exp2(fmaf(s, kLog2e, -ms)); }
+
+// Online softmax over key blocks: m <- max(m, the block's row max), l <- l * alpha with alpha = 2^(m_old - m_new)
+// (m_old = -inf: alpha = 0 and l stays 0).  Returns alpha; the block's exps then use row_shift(m).
+__device__ __forceinline__ float2 fold_row_max(const float (&s)[32], float& m0, float& m1, float& l0, float& l1) {
+  float mx0 = m0, mx1 = m1;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    mx0 = fmaxf(mx0, fmaxf(s[4 * j + 0], s[4 * j + 1]));
+    mx1 = fmaxf(mx1, fmaxf(s[4 * j + 2], s[4 * j + 3]));
+  }
+  quad_max(mx0, mx1);
+  const float alpha0 = softmax_exp(m0, row_shift(mx0)), alpha1 = softmax_exp(m1, row_shift(mx1));
+  m0 = mx0;
+  m1 = mx1;
+  l0 *= alpha0;
+  l1 *= alpha1;
+  return make_float2(alpha0, alpha1);
+}
+
+// The exps of a row pair: l += this thread's share of the row sums, in column order, and P in 16 bit as the A
+// fragments of O = P V (k-step kk covers keys 16 kk .. 16 kk + 15).  One loop over the column pairs: written as three
+// passes over s, it compiles to a different schedule of the long kernel that ran 1-2 % slower on an H100.
+template <bool F16, int N>
+__device__ __forceinline__ void exp_sum_pack(const float (&s)[N], float ms0, float ms1, float& l0, float& l1,
+                                             uint32_t (&pa)[N / 8][4]) {
+#pragma unroll
+  for (int j = 0; j < N / 4; ++j) {
+    const float e00 = softmax_exp(s[4 * j + 0], ms0), e01 = softmax_exp(s[4 * j + 1], ms0);
+    const float e10 = softmax_exp(s[4 * j + 2], ms1), e11 = softmax_exp(s[4 * j + 3], ms1);
+    l0 += e00 + e01;
+    l1 += e10 + e11;
+    pa[j >> 1][2 * (j & 1) + 0] = pack_op2<F16>(e00, e01);
+    pa[j >> 1][2 * (j & 1) + 1] = pack_op2<F16>(e10, e11);
+  }
+}
+
+// O / l -> 16 bit -> this thread's rows row0 and row0 + 8 of a [rows x 64] tile, swizzled like a SWIZZLE_128B TMA box.
+template <bool F16>
+__device__ __forceinline__ void stage_rows(uint32_t row0, const float (&o)[32], float inv0, float inv1, int rr, int q4) {
+  const uint32_t row1 = row0 + 8u * 128u;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    st_shared_b32(row0 + ((j ^ rr) << 4) + q4 * 4, pack_op2<F16>(o[4 * j + 0] * inv0, o[4 * j + 1] * inv0));
+    st_shared_b32(row1 + ((j ^ rr) << 4) + q4 * 4, pack_op2<F16>(o[4 * j + 2] * inv1, o[4 * j + 3] * inv1));
+  }
+}
 
 struct AttParams {
   int64_t n_seq;
@@ -48,12 +153,6 @@ struct AttParams {
   int causal;
   const int32_t* key_mask;  // [n_seq, S] or nullptr
 };
-
-template <bool F16, int NK>
-__device__ __forceinline__ void wgmma_qk(float (&s)[NK / 2], uint64_t qdesc, uint64_t kdesc, uint32_t scale_d) {
-  if constexpr (NK == 64) wgmma_ss_n64<F16>(s, qdesc, kdesc, scale_d);
-  else wgmma_ss_n128<F16>(s, qdesc, kdesc, scale_d);
-}
 
 template <bool F16, int NK>
 __global__ void __launch_bounds__(kAttThreads, NK == 64 ? 3 : 2)
@@ -100,9 +199,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmLoad, const __grid_consta
   const int r_in0 = R0 - g * slot, r_in1 = r_in0 + 8;
   const int kbase = (NK == 64) ? 64 * hf : 0;     // first key of the tile this warpgroup multiplies with
   const int k_in_base = kbase - g * slot + 2 * q4; // + 8 j + e = index inside the sequence of column (j, e)
-  const int lim0 = r_in0 < S ? (p.causal ? r_in0 : S - 1) : -1;   // last visible key of each row
-  const int lim1 = r_in1 < S ? (p.causal ? r_in1 : S - 1) : -1;
-  constexpr float kLog2e = 1.4426950408889634f;
+  const int lim0 = last_visible_key(r_in0, S, p.causal), lim1 = last_visible_key(r_in1, S, p.causal);
 
   uint32_t it = 0;
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
@@ -110,7 +207,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmLoad, const __grid_consta
     const int h = tile - st * p.heads;
     const int64_t seq = (int64_t)st * G + g;
 
-    // keys of the sequence that exist (and are not padding): one bit per accumulator column of this thread
+    // keys of the sequence that exist (and are not padding): one bit per accumulator column of this thread, read
+    // before the wait so that the key-mask loads overlap the TMA loads
     uint32_t kv = 0;
 #pragma unroll
     for (int c = 0; c < NK / 4; ++c) {
@@ -124,53 +222,23 @@ attention_kernel(const __grid_constant__ CUtensorMap tmLoad, const __grid_consta
 
     // ---- S = Q K^T
     float s[NK / 2];
-    {
-      const uint64_t qdesc = make_smem_desc_sw128(sq + hf * (64 * 128), 1024, 16);
-      const uint64_t kdesc = make_smem_desc_sw128(sk + kbase * 128, 1024, 16);
-      wgmma_pin(s);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < kHeadDim / 16; ++k) wgmma_qk<F16, NK>(s, qdesc + 2 * k, kdesc + 2 * k, k != 0 ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_pin(s);
-    }
+    qk_scores<F16, NK>(s, make_smem_desc_sw128(sq + hf * (64 * 128), 1024, 16),
+                       make_smem_desc_sw128(sk + kbase * 128, 1024, 16));
 
-    // ---- masked softmax on the registers (masked entries -> -inf -> exp2 = 0)
+    // ---- masked softmax on the registers; one key block, so the row max folds in column by column as it is masked
     float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
     for (int c = 0; c < NK / 4; ++c) {
       const int j = c >> 1, e = c & 1;
-      const int k_in = k_in_base + 8 * j + e;
-      const bool ok = (kv >> c) & 1u;
-      if (!(ok && k_in <= lim0)) s[4 * j + e] = -INFINITY;
-      if (!(ok && k_in <= lim1)) s[4 * j + 2 + e] = -INFINITY;
+      mask_column(s, j, e, (kv >> c) & 1u, k_in_base + 8 * j + e, lim0, lim1);
       mx0 = fmaxf(mx0, s[4 * j + e]);
       mx1 = fmaxf(mx1, s[4 * j + 2 + e]);
     }
-#pragma unroll
-    for (int o = 1; o < 4; o <<= 1) {  // the 4 lanes that share a row
-      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, o));
-      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, o));
-    }
-    const float ms0 = (mx0 == -INFINITY) ? 0.f : mx0 * kLog2e;
-    const float ms1 = (mx1 == -INFINITY) ? 0.f : mx1 * kLog2e;
+    quad_max(mx0, mx1);
     float sum0 = 0.f, sum1 = 0.f;
-    uint32_t pa[NK / 16][4];  // P as the A fragments of O = P V: k-step kk covers keys 16 kk .. 16 kk + 15
-#pragma unroll
-    for (int j = 0; j < NK / 8; ++j) {
-      const float e00 = fast_exp2(fmaf(s[4 * j + 0], kLog2e, -ms0)), e01 = fast_exp2(fmaf(s[4 * j + 1], kLog2e, -ms0));
-      const float e10 = fast_exp2(fmaf(s[4 * j + 2], kLog2e, -ms1)), e11 = fast_exp2(fmaf(s[4 * j + 3], kLog2e, -ms1));
-      sum0 += e00 + e01;
-      sum1 += e10 + e11;
-      pa[j >> 1][2 * (j & 1) + 0] = pack_op2<F16>(e00, e01);
-      pa[j >> 1][2 * (j & 1) + 1] = pack_op2<F16>(e10, e11);
-    }
-#pragma unroll
-    for (int o = 1; o < 4; o <<= 1) {
-      sum0 += __shfl_xor_sync(0xffffffffu, sum0, o);
-      sum1 += __shfl_xor_sync(0xffffffffu, sum1, o);
-    }
+    uint32_t pa[NK / 16][4];
+    exp_sum_pack<F16>(s, row_shift(mx0), row_shift(mx1), sum0, sum1, pa);
+    quad_sum(sum0, sum1);
 
     // ---- O = P V   (V tile [keys][64 dh]: advancing 16 keys = 16 rows of 128 B)
     float o[32];
@@ -185,18 +253,11 @@ attention_kernel(const __grid_constant__ CUtensorMap tmLoad, const __grid_consta
     wgmma_wait<0>();
     wgmma_pin(o);
 
-    // ---- epilogue: O / rowsum -> 16 bit -> this thread's Q rows (swizzled like a TMA box) -> bulk store per sequence
-    const float inv0 = sum0 > 0.f ? 1.0f / sum0 : 0.f;
-    const float inv1 = sum1 > 0.f ? 1.0f / sum1 : 0.f;
-    const uint32_t row0 = sq + static_cast<uint32_t>(R0) * 128u, row1 = row0 + 8u * 128u;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      st_shared_b32(row0 + ((j ^ rr) << 4) + q4 * 4, pack_op2<F16>(o[4 * j + 0] * inv0, o[4 * j + 1] * inv0));
-      st_shared_b32(row1 + ((j ^ rr) << 4) + q4 * 4, pack_op2<F16>(o[4 * j + 2] * inv1, o[4 * j + 3] * inv1));
-    }
+    // ---- epilogue: O / rowsum -> 16 bit -> this thread's Q rows -> one bulk store per sequence of the tile
+    stage_rows<F16>(sq + static_cast<uint32_t>(R0) * 128u, o, row_inv(sum0), row_inv(sum1), rr, q4);
     fence_proxy_async_smem();
     __syncthreads();  // the output tile is complete, and both warpgroups are done with K and V
-    if (threadIdx.x == 0) {
+    if (threadIdx.x == 0) {  // persistent: the CTA's next tile is loaded once the stores have read the Q buffer
       for (int gg = 0; gg < G; ++gg) {
         const int64_t sq_idx = (int64_t)st * G + gg;
         if (sq_idx < p.n_seq)
@@ -311,7 +372,6 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_co
   // ===================== consumers =====================
   const int q4 = lane & 3, rr = lane >> 2;
   const int R0 = 64 * wg + 16 * (warp & 3) + rr;  // this thread's tile rows R0 and R0 + 8
-  constexpr float kLog2e = 1.4426950408889634f;
   float o[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
@@ -326,18 +386,9 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_co
 
     // ---- S = Q K^T
     float sc[32];
-    {
-      const uint64_t kdesc = make_smem_desc_sw128(sk(s), 1024, 16);
-      wgmma_pin(sc);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < kHeadDim / 16; ++k) wgmma_ss_n64<F16>(sc, qdesc + 2 * k, kdesc + 2 * k, k != 0 ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_pin(sc);
-    }
+    qk_scores<F16, 64>(sc, qdesc, make_smem_desc_sw128(sk(s), 1024, 16));
 
-    // ---- online softmax on the registers
+    // ---- online softmax on the registers; no causal or key mask (vision only): keys >= S exist in the last block only
     const int kbase = kb * kLongKeys + 2 * q4;  // + 8 j + e = key of column (j, e)
     if (kb * kLongKeys + kLongKeys > S) {
 #pragma unroll
@@ -349,39 +400,16 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_co
             sc[4 * j + 2 + e] = -INFINITY;
           }
     }
-    float mx0 = m0, mx1 = m1;
+    // Every block holds at least one real key, and zero-filled query rows still score 0 against real keys, so the
+    // row max is finite and row_shift's empty-row case never occurs here.
+    const float2 alpha = fold_row_max(sc, m0, m1, l0, l1);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      mx0 = fmaxf(mx0, fmaxf(sc[4 * j + 0], sc[4 * j + 1]));
-      mx1 = fmaxf(mx1, fmaxf(sc[4 * j + 2], sc[4 * j + 3]));
+      o[4 * j + 0] *= alpha.x; o[4 * j + 1] *= alpha.x;
+      o[4 * j + 2] *= alpha.y; o[4 * j + 3] *= alpha.y;
     }
-#pragma unroll
-    for (int off = 1; off < 4; off <<= 1) {  // the 4 lanes that share a row
-      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, off));
-      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, off));
-    }
-    // every block holds at least one real key, so mx is finite; m_old = -inf (first block) gives alpha = 0
-    const float ms0 = mx0 * kLog2e, ms1 = mx1 * kLog2e;
-    const float alpha0 = fast_exp2(fmaf(m0, kLog2e, -ms0)), alpha1 = fast_exp2(fmaf(m1, kLog2e, -ms1));
-    m0 = mx0;
-    m1 = mx1;
-    l0 *= alpha0;
-    l1 *= alpha1;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      o[4 * j + 0] *= alpha0; o[4 * j + 1] *= alpha0;
-      o[4 * j + 2] *= alpha1; o[4 * j + 3] *= alpha1;
-    }
-    uint32_t pa[4][4];  // P as the A fragments of O += P V: k-step kk covers keys 16 kk .. 16 kk + 15 of the block
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float e00 = fast_exp2(fmaf(sc[4 * j + 0], kLog2e, -ms0)), e01 = fast_exp2(fmaf(sc[4 * j + 1], kLog2e, -ms0));
-      const float e10 = fast_exp2(fmaf(sc[4 * j + 2], kLog2e, -ms1)), e11 = fast_exp2(fmaf(sc[4 * j + 3], kLog2e, -ms1));
-      l0 += e00 + e01;
-      l1 += e10 + e11;
-      pa[j >> 1][2 * (j & 1) + 0] = pack_op2<F16>(e00, e01);
-      pa[j >> 1][2 * (j & 1) + 1] = pack_op2<F16>(e10, e11);
-    }
+    uint32_t pa[4][4];
+    exp_sum_pack<F16>(sc, row_shift(m0), row_shift(m1), l0, l1, pa);
 
     // ---- O += P V   (V block [keys][64 dh]: advancing 16 keys = 16 rows of 128 B)
     wgmma_pin(o);
@@ -397,20 +425,9 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_co
     if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar(s));  // this warpgroup is done with K / V of the stage
   }
 
-  // ---- epilogue: O / l -> 16 bit -> this warpgroup's Q rows (swizzled like a TMA box) -> one TMA store
-#pragma unroll
-  for (int off = 1; off < 4; off <<= 1) {
-    l0 += __shfl_xor_sync(0xffffffffu, l0, off);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, off);
-  }
-  const float inv0 = l0 > 0.f ? 1.0f / l0 : 0.f;
-  const float inv1 = l1 > 0.f ? 1.0f / l1 : 0.f;
-  const uint32_t row0 = sq + static_cast<uint32_t>(R0) * 128u, row1 = row0 + 8u * 128u;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    st_shared_b32(row0 + ((j ^ rr) << 4) + q4 * 4, pack_op2<F16>(o[4 * j + 0] * inv0, o[4 * j + 1] * inv0));
-    st_shared_b32(row1 + ((j ^ rr) << 4) + q4 * 4, pack_op2<F16>(o[4 * j + 2] * inv1, o[4 * j + 3] * inv1));
-  }
+  // ---- epilogue: O / l -> 16 bit -> this warpgroup's Q rows -> one TMA store
+  quad_sum(l0, l1);
+  stage_rows<F16>(sq + static_cast<uint32_t>(R0) * 128u, o, row_inv(l0), row_inv(l1), rr, q4);
   fence_proxy_async_smem();
   if (wg == 0) named_barrier_sync<1, 128>();  // the warpgroup's 64 output rows are staged
   else named_barrier_sync<2, 128>();
@@ -419,17 +436,6 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_co
     tma_store_commit();
     tma_store_wait_all();
   }
-}
-
-template <bool F16>
-int launch_attention_long(const CUtensorMap& tmQKV, const CUtensorMap& tmO, const LongAttParams& p, int64_t blocks,
-                          cudaStream_t st) {
-  auto kern = attention_long_kernel<F16>;
-  static unsigned long long configured = 0;
-  if (first_use_on_device(configured))
-    PLIP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLongSmem));
-  PLIP_CUDA_CHECK(launch_kernel(kern, dim3((unsigned)blocks), dim3(kLongThreads), kLongSmem, st, 1, tmQKV, tmO, p));
-  return 0;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -507,10 +513,8 @@ attention_probs_kernel(const __grid_constant__ CUtensorMap tmQKV, const ProbPara
   const int q4 = lane & 3, rr = lane >> 2;
   const int r0 = 16 * warp + rr;                    // this thread's block rows r0 and r0 + 8
   const int qa = q0 + r0, qc = qa + 8;              // their queries
-  const int lim0 = qa < S ? (p.causal ? qa : S - 1) : -1;   // last visible key of each row
-  const int lim1 = qc < S ? (p.causal ? qc : S - 1) : -1;
+  const int lim0 = last_visible_key(qa, S, p.causal), lim1 = last_visible_key(qc, S, p.causal);
   const int32_t* km = p.key_mask ? p.key_mask + seq * S : nullptr;
-  constexpr float kLog2e = 1.4426950408889634f;
   const uint64_t qdesc = make_smem_desc_sw128(sq, 1024, 16);
   mbar_wait(q_bar, 0);
 
@@ -520,14 +524,7 @@ attention_probs_kernel(const __grid_constant__ CUtensorMap tmQKV, const ProbPara
     const int li = resident ? u % n_kb : u;
     const int s = li % kProbStages;
     mbar_wait(full_bar(s), (uint32_t)((li / kProbStages) & 1));
-    const uint64_t kdesc = make_smem_desc_sw128(sk(s), 1024, 16);
-    wgmma_pin(sc);
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < kHeadDim / 16; ++k) wgmma_ss_n64<F16>(sc, qdesc + 2 * k, kdesc + 2 * k, k != 0 ? 1u : 0u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_pin(sc);
+    qk_scores<F16, 64>(sc, qdesc, make_smem_desc_sw128(sk(s), 1024, 16));
     if (!resident) {
       __syncthreads();  // every warp is done with the stage: refill it
       if (threadIdx.x == 0 && li + kProbStages < n_loads) issue_k(li + kProbStages);
@@ -536,11 +533,9 @@ attention_probs_kernel(const __grid_constant__ CUtensorMap tmQKV, const ProbPara
 #pragma unroll
     for (int j = 0; j < 8; ++j)
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
+      for (int e = 0; e < 2; ++e) {  // one warpgroup per CTA: the key mask is read per column, after the wait
         const int key = kbase + 8 * j + e;
-        const bool ok = key < S && (km == nullptr || km[key] != 0);
-        if (!(ok && key <= lim0)) sc[4 * j + e] = -INFINITY;
-        if (!(ok && key <= lim1)) sc[4 * j + 2 + e] = -INFINITY;
+        mask_column(sc, j, e, key < S && (km == nullptr || km[key] != 0), key, lim0, lim1);
       }
   };
 
@@ -548,36 +543,17 @@ attention_probs_kernel(const __grid_constant__ CUtensorMap tmQKV, const ProbPara
   float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
   for (int kb = 0; kb < n_kb; ++kb) {
     scores(kb);
-    float mx0 = m0, mx1 = m1;
+    fold_row_max(sc, m0, m1, l0, l1);
+    const float ms0 = row_shift(m0), ms1 = row_shift(m1);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      mx0 = fmaxf(mx0, fmaxf(sc[4 * j + 0], sc[4 * j + 1]));
-      mx1 = fmaxf(mx1, fmaxf(sc[4 * j + 2], sc[4 * j + 3]));
-    }
-#pragma unroll
-    for (int off = 1; off < 4; off <<= 1) {  // the 4 lanes that share a row
-      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, off));
-      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, off));
-    }
-    const float ms0 = mx0 == -INFINITY ? 0.f : mx0 * kLog2e, ms1 = mx1 == -INFINITY ? 0.f : mx1 * kLog2e;
-    l0 *= fast_exp2(fmaf(m0, kLog2e, -ms0));  // m_old = -inf: l is still 0
-    l1 *= fast_exp2(fmaf(m1, kLog2e, -ms1));
-    m0 = mx0;
-    m1 = mx1;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      l0 += fast_exp2(fmaf(sc[4 * j + 0], kLog2e, -ms0)) + fast_exp2(fmaf(sc[4 * j + 1], kLog2e, -ms0));
-      l1 += fast_exp2(fmaf(sc[4 * j + 2], kLog2e, -ms1)) + fast_exp2(fmaf(sc[4 * j + 3], kLog2e, -ms1));
+      l0 += softmax_exp(sc[4 * j + 0], ms0) + softmax_exp(sc[4 * j + 1], ms0);
+      l1 += softmax_exp(sc[4 * j + 2], ms1) + softmax_exp(sc[4 * j + 3], ms1);
     }
   }
-#pragma unroll
-  for (int off = 1; off < 4; off <<= 1) {
-    l0 += __shfl_xor_sync(0xffffffffu, l0, off);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, off);
-  }
-  const float ms0 = m0 == -INFINITY ? 0.f : m0 * kLog2e, ms1 = m1 == -INFINITY ? 0.f : m1 * kLog2e;
-  const float inv0 = l0 > 0.f ? 1.0f / l0 : 0.f;
-  const float inv1 = l1 > 0.f ? 1.0f / l1 : 0.f;
+  quad_sum(l0, l1);
+  const float ms0 = row_shift(m0), ms1 = row_shift(m1);
+  const float inv0 = row_inv(l0), inv1 = row_inv(l1);
 
   // ---- pass 2: probabilities -> staging rows of this warp -> global
   float* wst = staging + 16 * warp * kProbLd;       // the warp's 16 staging rows
@@ -587,12 +563,10 @@ attention_probs_kernel(const __grid_constant__ CUtensorMap tmQKV, const ProbPara
     scores(n_kb + kb);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      const float2 a = make_float2(fast_exp2(fmaf(sc[4 * j + 0], kLog2e, -ms0)) * inv0,
-                                   fast_exp2(fmaf(sc[4 * j + 1], kLog2e, -ms0)) * inv0);
-      const float2 b = make_float2(fast_exp2(fmaf(sc[4 * j + 2], kLog2e, -ms1)) * inv1,
-                                   fast_exp2(fmaf(sc[4 * j + 3], kLog2e, -ms1)) * inv1);
-      *reinterpret_cast<float2*>(wst + rr * kProbLd + 8 * j + 2 * q4) = a;
-      *reinterpret_cast<float2*>(wst + (rr + 8) * kProbLd + 8 * j + 2 * q4) = b;
+      *reinterpret_cast<float2*>(wst + rr * kProbLd + 8 * j + 2 * q4) =
+          make_float2(softmax_exp(sc[4 * j + 0], ms0) * inv0, softmax_exp(sc[4 * j + 1], ms0) * inv0);
+      *reinterpret_cast<float2*>(wst + (rr + 8) * kProbLd + 8 * j + 2 * q4) =
+          make_float2(softmax_exp(sc[4 * j + 2], ms1) * inv1, softmax_exp(sc[4 * j + 3], ms1) * inv1);
     }
     __syncwarp();
     const int k0 = kb * 64;
@@ -609,27 +583,41 @@ attention_probs_kernel(const __grid_constant__ CUtensorMap tmQKV, const ProbPara
   }
 }
 
-template <bool F16>
-int launch_attention_probs_inst(const CUtensorMap& tmQKV, const ProbParams& p, int64_t blocks, cudaStream_t st) {
-  auto kern = attention_probs_kernel<F16>;
+// Launches `blocks` CTAs of the long or the probabilities kernel; its shared-memory limit is raised once per device.
+template <auto Kern, int Threads, uint32_t Smem, typename... Args>
+int launch_blocks(int64_t blocks, cudaStream_t st, const Args&... args) {
   static unsigned long long configured = 0;
   if (first_use_on_device(configured))
-    PLIP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kProbSmem));
-  PLIP_CUDA_CHECK(launch_kernel(kern, dim3((unsigned)blocks), dim3(kProbThreads), kProbSmem, st, 1, tmQKV, p));
+    PLIP_CUDA_CHECK(cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Smem));
+  PLIP_CUDA_CHECK(launch_kernel(Kern, dim3((unsigned)blocks), dim3(Threads), Smem, st, 1, args...));
   return 0;
+}
+
+// The argument checks of launch_attention and launch_attention_probs; `fn` prefixes the messages.
+int check_attention_args(const char* fn, const void* qkv, const void* out, int64_t n_seq, int seq_len, int heads) {
+  PLIP_REQUIRE(qkv && out, "%s: null argument", fn);
+  PLIP_REQUIRE(n_seq > 0 && seq_len > 0 && seq_len <= kMaxVisSeq, "%s: bad shape n_seq=%lld seq_len=%d", fn,
+               (long long)n_seq, seq_len);
+  PLIP_REQUIRE(heads > 0 && heads <= 16, "%s: bad head count %d", fn, heads);
+  return 0;
+}
+
+// [n_seq][S][cols] view of a 16-bit activation with a {64, 64, 1} box: rows past a sequence's end are zero-filled on
+// load and clipped on store.
+int make_seq_tmap(CUtensorMap* tm, const void* base, int64_t n_seq, int seq_len, int cols) {
+  return make_tmap_bf16_3d(tm, base, (uint64_t)n_seq, (uint64_t)seq_len, (uint64_t)cols, (uint64_t)cols * 2,
+                           (uint64_t)seq_len * cols * 2, 64, 64);
 }
 
 }  // namespace
 
 int launch_attention(const __nv_bfloat16* qkv, int64_t n_seq, int seq_len, int heads, bool causal,
                      const int32_t* key_mask, __nv_bfloat16* out, int f16, cudaStream_t st) {
-  PLIP_REQUIRE(n_seq > 0 && seq_len > 0 && seq_len <= kMaxVisSeq, "attention: bad shape n_seq=%lld seq_len=%d",
-               (long long)n_seq, seq_len);
-  PLIP_REQUIRE(heads > 0 && heads <= 16, "attention: bad head count %d", heads);
+  if (int rc = check_attention_args("attention", qkv, out, n_seq, seq_len, heads)) return rc;
+  const int D = heads * kHeadDim;
   if (seq_len > 128) {
     PLIP_REQUIRE(!causal && key_mask == nullptr,
                  "attention: seq_len %d > 128 is supported without causal or key mask only", seq_len);
-    const int D = heads * kHeadDim;
     LongAttParams p;
     p.seq_len = seq_len;
     p.heads = heads;
@@ -637,14 +625,11 @@ int launch_attention(const __nv_bfloat16* qkv, int64_t n_seq, int seq_len, int h
     const int64_t blocks = n_seq * heads * p.q_blocks;
     PLIP_REQUIRE(blocks < 0x7fffffff && n_seq < 0x7fffffff, "attention: too many sequences");
     CUtensorMap tmQKV, tmO;
-    if (int rc = make_tmap_bf16_3d(&tmQKV, qkv, (uint64_t)n_seq, (uint64_t)seq_len, (uint64_t)3 * D,
-                                   (uint64_t)3 * D * 2, (uint64_t)seq_len * 3 * D * 2, 64, 64)) return rc;
-    if (int rc = make_tmap_bf16_3d(&tmO, out, (uint64_t)n_seq, (uint64_t)seq_len, (uint64_t)D, (uint64_t)D * 2,
-                                   (uint64_t)seq_len * D * 2, 64, 64)) return rc;
-    return f16 ? launch_attention_long<true>(tmQKV, tmO, p, blocks, st)
-               : launch_attention_long<false>(tmQKV, tmO, p, blocks, st);
+    if (int rc = make_seq_tmap(&tmQKV, qkv, n_seq, seq_len, 3 * D)) return rc;
+    if (int rc = make_seq_tmap(&tmO, out, n_seq, seq_len, D)) return rc;
+    return f16 ? launch_blocks<attention_long_kernel<true>, kLongThreads, kLongSmem>(blocks, st, tmQKV, tmO, p)
+               : launch_blocks<attention_long_kernel<false>, kLongThreads, kLongSmem>(blocks, st, tmQKV, tmO, p);
   }
-  const int D = heads * kHeadDim;
   const int64_t rows = n_seq * seq_len;
   PLIP_REQUIRE(rows + 128 < 0x7fffffff, "attention: too many token rows");
   AttParams p;
@@ -666,10 +651,7 @@ int launch_attention(const __nv_bfloat16* qkv, int64_t n_seq, int seq_len, int h
 
 int launch_attention_probs(const __nv_bfloat16* qkv, int64_t n_seq, int seq_len, int heads, bool causal,
                            const int32_t* key_mask, float* probs, int f16, cudaStream_t st) {
-  PLIP_REQUIRE(qkv && probs, "attention_probs: null argument");
-  PLIP_REQUIRE(n_seq > 0 && seq_len > 0 && seq_len <= kMaxVisSeq, "attention_probs: bad shape n_seq=%lld seq_len=%d",
-               (long long)n_seq, seq_len);
-  PLIP_REQUIRE(heads > 0 && heads <= 16, "attention_probs: bad head count %d", heads);
+  if (int rc = check_attention_args("attention_probs", qkv, probs, n_seq, seq_len, heads)) return rc;
   ProbParams p;
   p.seq_len = seq_len;
   p.heads = heads;
@@ -681,9 +663,9 @@ int launch_attention_probs(const __nv_bfloat16* qkv, int64_t n_seq, int seq_len,
   PLIP_REQUIRE(blocks < 0x7fffffff && n_seq < 0x7fffffff, "attention_probs: too many sequences");
   const int D = heads * kHeadDim;
   CUtensorMap tm;
-  if (int rc = make_tmap_bf16_3d(&tm, qkv, (uint64_t)n_seq, (uint64_t)seq_len, (uint64_t)3 * D, (uint64_t)3 * D * 2,
-                                 (uint64_t)seq_len * 3 * D * 2, 64, 64)) return rc;
-  return f16 ? launch_attention_probs_inst<true>(tm, p, blocks, st) : launch_attention_probs_inst<false>(tm, p, blocks, st);
+  if (int rc = make_seq_tmap(&tm, qkv, n_seq, seq_len, 3 * D)) return rc;
+  return f16 ? launch_blocks<attention_probs_kernel<true>, kProbThreads, kProbSmem>(blocks, st, tm, p)
+             : launch_blocks<attention_probs_kernel<false>, kProbThreads, kProbSmem>(blocks, st, tm, p);
 }
 
 }  // namespace plip
