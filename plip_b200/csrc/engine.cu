@@ -185,7 +185,6 @@ struct plip_engine {
   __nv_bfloat16* pooled = nullptr;  // [mb, 768]
   int32_t* row_idx = nullptr;       // [mb] EOS rows
   int32_t* kmask = nullptr;         // [mb*77] key padding mask
-  const float* pooled_x = nullptr;  // set by run_layers when the last layer was pruned: compact fp32 [n_seq, D] pooled rows
   // last use of the shared workspace through the device-pointer API (any caller stream): the host-buffer
   // path, which runs on the engine's own streams, waits for it before touching the workspace
   cudaEvent_t ev_last = nullptr;
@@ -332,15 +331,38 @@ int layer_tail(plip_engine* e, const LayerW& w, int rows, int D, int FF, const _
   return gemm(e, PK_FC2, g, st);
 }
 
-// Optional per-layer outputs of run_layers (plip_vision_outputs / plip_text_outputs); null pointers are not written.
+// What one pass writes (null: not requested): micro-batch [i0, i0 + mb) of an n-item call's plip_tower_outputs_t, i.e.
+// the caller's buffers at the micro-batch's offsets.  The per-layer ones are written by run_layers:
 //   hidden: X [n_seq * S, D] is copied to hidden on entry and to hidden + (l + 1) * hidden_stride after layer l
-//   probs:  the attention probabilities of layer l go to probs + l * probs_stride ([n_seq, heads, S, S] fp32)
-struct Taps {
+//   attn:   the attention probabilities of layer l go to attn + l * attn_stride ([n_seq, heads, S, S] fp32)
+struct PassOut {
+  float *embeds = nullptr, *pooled = nullptr, *last_hidden = nullptr;
   float* hidden = nullptr;
   int64_t hidden_stride = 0;  // floats between layers
-  float* probs = nullptr;
-  int64_t probs_stride = 0;
+  float* attn = nullptr;
+  int64_t attn_stride = 0;
+  int normalize = 0;
 };
+
+PassOut pass_out(const plip_tower_outputs_t& o, int64_t n, int64_t i0, int S, int D, int heads) {
+  PassOut p;
+  const int64_t tok = (int64_t)S * D, pp = (int64_t)heads * S * S;
+  if (o.embeds) p.embeds = o.embeds + i0 * kProj;
+  if (o.pooled) p.pooled = o.pooled + i0 * D;
+  if (o.last_hidden) p.last_hidden = o.last_hidden + i0 * tok;
+  if (o.hidden) { p.hidden = o.hidden + i0 * tok; p.hidden_stride = n * tok; }
+  if (o.attn) { p.attn = o.attn + i0 * pp; p.attn_stride = n * pp; }
+  p.normalize = o.normalize;
+  return p;
+}
+
+// The embedding calls (plip_encode_*): [mb, 512] at out.
+PassOut embeds_only(float* out, int normalize) {
+  PassOut p;
+  p.embeds = out;
+  p.normalize = normalize;
+  return p;
+}
 
 // Encoder layers with both LayerNorms folded into the consuming GEMMs.  On entry X holds the residual
 // stream; Xn / stats are (re)derived from it here and afterwards maintained by the residual epilogues.
@@ -349,18 +371,16 @@ struct Taps {
 // each sequence leaves the tower (CLS, TF:modeling_clip.py:685; first-EOS row, :571-584), and after the last layer's
 // attention nothing mixes rows any more, so that layer's out_proj, LN2, fc1 and fc2 are run on the n_seq pooled rows
 // alone (gathered into compact buffers) instead of all n_seq*S rows — same arithmetic per row, identical embeddings.
-// pool_idx: device row indices of the pooled rows (null = row i*S).  On return e->pooled_x points at them.
-// taps (null: none) are never combined with prune.
+// pool_idx: device row indices of the pooled rows (null = row i*S).  A pruned pass sets *pooled_x to the compact fp32
+// [n_seq, D] pooled rows and writes no per-layer outputs.
 int run_layers(plip_engine* e, const LayerW* L, int64_t n_seq, int S, int D, int FF, int heads, bool causal,
                const int32_t* kmask, int num_layers, cudaStream_t st, bool prune = false,
-               const int32_t* pool_idx = nullptr, const Taps* taps = nullptr) {
-  e->pooled_x = nullptr;
+               const int32_t* pool_idx = nullptr, const PassOut& out = PassOut(), const float** pooled_x = nullptr) {
   const int64_t M = n_seq * S;
   PLIP_REQUIRE(M <= 0x7fffffff / 4, "micro-batch too large");
-  PLIP_REQUIRE(!(taps && prune), "internal: per-layer outputs of a pruned pass");
+  PLIP_REQUIRE(!prune || (pooled_x && !out.hidden && !out.attn), "internal: per-layer outputs of a pruned pass");
   const size_t x_bytes = (size_t)M * D * 4;
-  if (taps && taps->hidden)
-    PLIP_CUDA_CHECK(cudaMemcpyAsync(taps->hidden, e->X, x_bytes, cudaMemcpyDeviceToDevice, st));
+  if (out.hidden) PLIP_CUDA_CHECK(cudaMemcpyAsync(out.hidden, e->X, x_bytes, cudaMemcpyDeviceToDevice, st));
   if (num_layers <= 0) return 0;
   {
     ProfScope ps(e, st, PK_ROWSTATS, 0, (double)M * D * 6 + (double)M * 8);
@@ -382,16 +402,16 @@ int run_layers(plip_engine* e, const LayerW* L, int64_t n_seq, int S, int D, int
       ProfScope ps(e, st, S > 128 ? PK_ATTN_LONG : PK_ATTN, f_att, b_att);
       if (int rc = launch_attention(e->QKV, n_seq, S, heads, causal, kmask, e->AO, e->f16, st)) return rc;
     }
-    if (taps && taps->probs) {
+    if (out.attn) {
       // reads Q and K of QKV (intact until the next layer's QKV GEMM), writes heads * S^2 fp32 per sequence
       ProfScope ps(e, st, PK_ATTN_PROBS, 0.5 * f_att, (double)M * 2 * D * 2 + (double)n_seq * heads * S * S * 4);
-      if (int rc = launch_attention_probs(e->QKV, n_seq, S, heads, causal, kmask, taps->probs + l * taps->probs_stride,
+      if (int rc = launch_attention_probs(e->QKV, n_seq, S, heads, causal, kmask, out.attn + l * out.attn_stride,
                                           e->f16, st)) return rc;
     }
     if (!(prune && last)) {
       if (int rc = layer_tail(e, w, (int)M, D, FF, e->AO, e->X, last, np, st)) return rc;
-      if (taps && taps->hidden)
-        PLIP_CUDA_CHECK(cudaMemcpyAsync(taps->hidden + (l + 1) * taps->hidden_stride, e->X, x_bytes,
+      if (out.hidden)
+        PLIP_CUDA_CHECK(cudaMemcpyAsync(out.hidden + (l + 1) * out.hidden_stride, e->X, x_bytes,
                                         cudaMemcpyDeviceToDevice, st));
       continue;
     }
@@ -403,14 +423,15 @@ int run_layers(plip_engine* e, const LayerW* L, int64_t n_seq, int S, int D, int
       if (int rc = launch_gather_rows(e->AO, e->X, pool_idx, S, n_seq, D, ao_p, x_p, st)) return rc;
     }
     if (int rc = layer_tail(e, w, (int)n_seq, D, FF, ao_p, x_p, true, np, st)) return rc;
-    e->pooled_x = x_p;
+    *pooled_x = x_p;
   }
   return 0;
 }
 
 // Vision tower up to (and including) `num_layers` encoder layers; X holds the residual stream [mb * geo.S, 768].
 int vision_trunk(plip_engine* e, const void* pixels, int fmt, int64_t mb, const VisGeom& geo, int num_layers,
-                 cudaStream_t st, bool prune = false, const Taps* taps = nullptr) {
+                 cudaStream_t st, bool prune = false, const PassOut& out = PassOut(),
+                 const float** pooled_x = nullptr) {
   e->prof_tower = 0;
   const double dmb = (double)mb;
   const int patches = geo.gh * geo.gw;
@@ -442,19 +463,19 @@ int vision_trunk(plip_engine* e, const void* pixels, int fmt, int64_t mb, const 
     if (int rc = launch_layernorm(e->X, nullptr, kVisDim, M, kVisDim, e->v_pre_g, e->v_pre_b, e->X, nullptr, e->f16, st)) return rc;
   }
   return run_layers(e, e->vis, mb, geo.S, kVisDim, kVisFF, kVisHeads, false, nullptr, num_layers, st, prune, nullptr,
-                    taps);
+                    out, pooled_x);
 }
 
 // Tower head: LayerNorm of the pooled rows -> projection [-> L2 normalise].  The pooled rows are the compact
-// e->pooled_x rows when the last layer was pruned, else rows pool_idx[i] of X (null: row i*S).
+// pooled_x rows when the last layer was pruned, else rows pool_idx[i] of X (null: row i*S).
 // pooled_f32 (optional): the LayerNorm-ed pooled rows in fp32 as well, [mb, D] (pooler_output); out null: no projection.
-int pooled_head(plip_engine* e, const int32_t* pool_idx, int64_t mb, int S, int D, const float* gamma,
-                const float* beta, const __nv_bfloat16* proj, float* out, int normalize, cudaStream_t st,
-                float* pooled_f32 = nullptr) {
+int pooled_head(plip_engine* e, const float* pooled_x, const int32_t* pool_idx, int64_t mb, int S, int D,
+                const float* gamma, const float* beta, const __nv_bfloat16* proj, float* out, int normalize,
+                cudaStream_t st, float* pooled_f32) {
   {
     ProfScope ps(e, st, PK_LN, 0, (double)mb * D * (pooled_f32 ? 10 : 6));
-    const bool compact = e->pooled_x != nullptr;
-    if (int rc = launch_layernorm(compact ? e->pooled_x : e->X, compact ? nullptr : pool_idx,
+    const bool compact = pooled_x != nullptr;
+    if (int rc = launch_layernorm(compact ? pooled_x : e->X, compact ? nullptr : pool_idx,
                                   compact || pool_idx ? (int64_t)D : (int64_t)S * D, mb, D, gamma, beta, pooled_f32,
                                   e->pooled, e->f16, st)) return rc;
   }
@@ -470,18 +491,27 @@ int pooled_head(plip_engine* e, const int32_t* pool_idx, int64_t mb, int S, int 
   return 0;
 }
 
-int vision_forward(plip_engine* e, const void* pixels, int fmt, int64_t mb, float* out, int normalize,
-                   cudaStream_t st, const VisGeom& geo = VisGeom()) {
-  if (int rc = vision_trunk(e, pixels, fmt, mb, geo, kLayers, st, e->prune_last != 0)) return rc;
+// One vision pass over mb images: the whole tower, then what `out` asks for.  prune: see run_layers (the embedding
+// calls only).  last_hidden_state is the residual stream after the last layer, before post_layernorm (TF:680-686).
+int vision_pass(plip_engine* e, const void* pixels, int fmt, int64_t mb, const VisGeom& geo, const PassOut& out,
+                bool prune, cudaStream_t st) {
+  const float* pooled_x = nullptr;
+  if (int rc = vision_trunk(e, pixels, fmt, mb, geo, kLayers, st, prune, out, &pooled_x)) return rc;
+  if (out.last_hidden)
+    PLIP_CUDA_CHECK(cudaMemcpyAsync(out.last_hidden, e->X, (size_t)mb * geo.S * kVisDim * 4, cudaMemcpyDeviceToDevice,
+                                    st));
+  if (!out.embeds && !out.pooled) return 0;
   // pooled = post_layernorm(last_hidden_state[:, 0, :])                  TF:modeling_clip.py:685-686
-  return pooled_head(e, nullptr, mb, geo.S, kVisDim, e->v_post_g, e->v_post_b, e->v_proj, out, normalize, st);
+  return pooled_head(e, pooled_x, nullptr, mb, geo.S, kVisDim, e->v_post_g, e->v_post_b, e->v_proj, out.embeds,
+                     out.normalize, st, out.pooled);
 }
 
 // S = number of leading token positions actually processed (<= stride, the row length of ids / mask).
 // Causality makes rows after a caption's first EOS irrelevant to its pooled output (TF:571-584), so callers
 // that know the longest caption of the batch may pass a shorter S: same result, proportionally less work.
 int text_trunk(plip_engine* e, const void* ids, int ids_dtype, const void* mask, int64_t mb, int S, int stride,
-               int num_layers, cudaStream_t st, bool prune = false, const Taps* taps = nullptr) {
+               int num_layers, cudaStream_t st, bool prune = false, const PassOut& out = PassOut(),
+               const float** pooled_x = nullptr) {
   e->prof_tower = 1;
   {
     ProfScope ps(e, st, PK_EMBED, 0, (double)mb * S * kTxtDim * 8);
@@ -493,14 +523,25 @@ int text_trunk(plip_engine* e, const void* ids, int ids_dtype, const void* mask,
     if (int rc = launch_mask_to_i32(mask, ids_dtype, mb * S, S, stride, e->kmask, st)) return rc;
     km = e->kmask;
   }
-  return run_layers(e, e->txt, mb, S, kTxtDim, kTxtFF, kTxtHeads, true, km, num_layers, st, prune, e->row_idx, taps);
+  return run_layers(e, e->txt, mb, S, kTxtDim, kTxtFF, kTxtHeads, true, km, num_layers, st, prune, e->row_idx, out,
+                    pooled_x);
 }
 
-int text_forward(plip_engine* e, const void* ids, int ids_dtype, const void* mask, int64_t mb, int S, int stride,
-                 float* out, int normalize, cudaStream_t st) {
-  if (int rc = text_trunk(e, ids, ids_dtype, mask, mb, S, stride, kLayers, st, e->prune_last != 0)) return rc;
+// One text pass over mb captions (the first S of `stride` positions), then what `out` asks for.
+// last_hidden_state = final_layer_norm of every row (TF:562).
+int text_pass(plip_engine* e, const void* ids, int ids_dtype, const void* mask, int64_t mb, int S, int stride,
+              const PassOut& out, bool prune, cudaStream_t st) {
+  const float* pooled_x = nullptr;
+  if (int rc = text_trunk(e, ids, ids_dtype, mask, mb, S, stride, kLayers, st, prune, out, &pooled_x)) return rc;
+  if (out.last_hidden) {
+    ProfScope ps(e, st, PK_LN, 0, (double)mb * S * kTxtDim * 8);
+    if (int rc = launch_layernorm(e->X, nullptr, kTxtDim, mb * S, kTxtDim, e->t_fin_g, e->t_fin_b, out.last_hidden,
+                                  nullptr, e->f16, st)) return rc;
+  }
+  if (!out.embeds && !out.pooled) return 0;
   // pooled = final_layer_norm(last_hidden_state)[b, first eos]            TF:modeling_clip.py:562-584
-  return pooled_head(e, e->row_idx, mb, S, kTxtDim, e->t_fin_g, e->t_fin_b, e->t_proj, out, normalize, st);
+  return pooled_head(e, pooled_x, e->row_idx, mb, S, kTxtDim, e->t_fin_g, e->t_fin_b, e->t_proj, out.embeds,
+                     out.normalize, st, out.pooled);
 }
 
 int ensure_host_path(plip_engine* e) {
@@ -640,11 +681,11 @@ int capture_graph(plip_engine* e, F&& body, Graph* out) {
   return 0;
 }
 
-// Arguments of a vision call at any image size (interpolate_pos_encoding): 32 <= H, W and a patch grid of at most
-// kMaxGrid x kMaxGrid, and one image's tokens must fit the workspace's kVisSeq * max_micro_batch token rows.  The
-// shape is checked before the handle, so a bad size is reported as such whatever else is wrong.
-int check_hw_call(const char* fn, const plip_engine* e, const void* in, const void* out, int fmt, int64_t n,
-                  int height, int width) {
+// Arguments of a call on n images (interpolate_pos_encoding: any size): 32 <= H, W and a patch grid of at most
+// kMaxGrid x kMaxGrid, and one image's tokens must fit the workspace's kVisSeq * max_micro_batch token rows.  Pointers
+// and shapes are checked before the handle, so a bad argument is reported as such whatever else is wrong.
+int check_pixels(const char* fn, const plip_engine* e, const void* in, const void* out, int fmt, int64_t n,
+                 int height, int width) {
   PLIP_REQUIRE(in && out, "%s: null argument", fn);
   PLIP_REQUIRE(n > 0, "%s: n must be positive (got %lld)", fn, (long long)n);
   PLIP_REQUIRE(fmt >= 0 && fmt <= 2, "%s: unknown pixel format %d", fn, fmt);
@@ -660,53 +701,36 @@ int check_hw_call(const char* fn, const plip_engine* e, const void* in, const vo
   return 0;
 }
 
-// ---- per-layer outputs (plip_vision_outputs / plip_text_outputs) ----------------------------------------------------
+// Arguments of a call on n captions of seq_len ids (the TF message for a bad seq_len), of which the first prefix_len
+// are processed; the same order as check_pixels.
+int check_ids(const char* fn, const plip_engine* e, const void* ids, const void* out, int ids_dtype, int64_t n,
+              int seq_len, int prefix_len) {
+  PLIP_REQUIRE(ids && out, "%s: null argument", fn);
+  PLIP_REQUIRE(n > 0, "%s: n must be positive (got %lld)", fn, (long long)n);
+  PLIP_REQUIRE(seq_len >= 1 && seq_len <= kTxtSeq,
+               "Sequence length must be less than max_position_embeddings (got `sequence length`: %d and "
+               "max_position_embeddings: %d)", seq_len, kTxtSeq);  // message mirrors TF:243-247
+  PLIP_REQUIRE(prefix_len >= 1 && prefix_len <= seq_len, "%s: prefix_len %d out of [1,%d]", fn, prefix_len, seq_len);
+  PLIP_REQUIRE(ids_dtype == PLIP_IDS_I32 || ids_dtype == PLIP_IDS_I64, "%s: unknown ids dtype %d", fn, ids_dtype);
+  PLIP_REQUIRE(e != nullptr, "%s: null engine", fn);
+  return 0;
+}
+
 int check_outputs(const char* fn, const plip_tower_outputs_t* o) {
   PLIP_REQUIRE(o != nullptr, "%s: null outputs", fn);
   PLIP_REQUIRE(o->embeds || o->pooled || o->last_hidden || o->hidden || o->attn, "%s: no output requested", fn);
   return 0;
 }
 
-// The taps of micro-batch [i0, i0 + mb) of an n-sequence call: the caller's [13, n, S, D] / [12, n, heads, S, S] buffers
-// at the micro-batch's offsets.
-Taps outputs_taps(const plip_tower_outputs_t* o, int64_t n, int64_t i0, int S, int D, int heads) {
-  Taps t;
-  const int64_t tok = (int64_t)S * D, pp = (int64_t)heads * S * S;
-  if (o->hidden) { t.hidden = o->hidden + i0 * tok; t.hidden_stride = n * tok; }
-  if (o->attn) { t.probs = o->attn + i0 * pp; t.probs_stride = n * pp; }
-  return t;
-}
-
-// One vision pass over images [i0, i0 + mb) of n: the full tower (never pruned), then the requested outputs.
-// last_hidden_state is the residual stream after the last layer, before post_layernorm (TF:modeling_clip.py:680-686).
-int vision_outputs_pass(plip_engine* e, const void* pixels, int fmt, int64_t mb, int64_t i0, int64_t n,
-                        const VisGeom& geo, const plip_tower_outputs_t* o, cudaStream_t st) {
-  const Taps t = outputs_taps(o, n, i0, geo.S, kVisDim, kVisHeads);
-  if (int rc = vision_trunk(e, pixels, fmt, mb, geo, kLayers, st, false, &t)) return rc;
-  if (o->last_hidden)
-    PLIP_CUDA_CHECK(cudaMemcpyAsync(o->last_hidden + i0 * geo.S * kVisDim, e->X, (size_t)mb * geo.S * kVisDim * 4,
-                                    cudaMemcpyDeviceToDevice, st));
-  if (!o->embeds && !o->pooled) return 0;
-  return pooled_head(e, nullptr, mb, geo.S, kVisDim, e->v_post_g, e->v_post_b, e->v_proj,
-                     o->embeds ? o->embeds + i0 * kProj : nullptr, o->normalize, st,
-                     o->pooled ? o->pooled + i0 * kVisDim : nullptr);
-}
-
-// One text pass over captions [i0, i0 + mb) of n at the full seq_len (every position is an output).
-// last_hidden_state = final_layer_norm of every row (TF:562); pooler_output its pooled row (TF:571-584).
-int text_outputs_pass(plip_engine* e, const void* ids, int ids_dtype, const void* mask, int64_t mb, int S, int64_t i0,
-                      int64_t n, const plip_tower_outputs_t* o, cudaStream_t st) {
-  const Taps t = outputs_taps(o, n, i0, S, kTxtDim, kTxtHeads);
-  if (int rc = text_trunk(e, ids, ids_dtype, mask, mb, S, S, kLayers, st, false, &t)) return rc;
-  if (o->last_hidden) {
-    ProfScope ps(e, st, PK_LN, 0, (double)mb * S * kTxtDim * 8);
-    if (int rc = launch_layernorm(e->X, nullptr, kTxtDim, mb * S, kTxtDim, e->t_fin_g, e->t_fin_b,
-                                  o->last_hidden + i0 * S * kTxtDim, nullptr, e->f16, st)) return rc;
-  }
-  if (!o->embeds && !o->pooled) return 0;
-  return pooled_head(e, e->row_idx, mb, S, kTxtDim, e->t_fin_g, e->t_fin_b, e->t_proj,
-                     o->embeds ? o->embeds + i0 * kProj : nullptr, o->normalize, st,
-                     o->pooled ? o->pooled + i0 * kTxtDim : nullptr);
+// The protocol of an eager device-pointer call: calls on different streams share one workspace, so the call waits for
+// its last use, runs pass(i, mb) over items [i, i + mb) in passes of at most per_pass, and marks its own last use.
+template <typename F>
+int micro_batches(plip_engine* e, int64_t n, int64_t per_pass, cudaStream_t st, F&& pass) {
+  PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_last, 0));
+  for (int64_t i = 0; i < n; i += per_pass)
+    if (int rc = pass(i, n - i < per_pass ? n - i : per_pass)) return rc;
+  PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
+  return 0;
 }
 
 bool graph_eligible(const plip_engine* e, int64_t n) {
@@ -728,12 +752,14 @@ struct Staged {
   size_t bytes;
 };
 
-// Small-batch path (graph_eligible): the first call of a key runs forward(stream, in0, in1, out) eagerly on the
-// caller's buffers, which also configures every kernel, then records it as a graph on the staging buffers.  Later
-// calls copy the inputs in, replay the graph and copy the [n, 512] result out.
+// Small-batch path (graph_eligible), waiting for and marking the workspace as micro_batches does: the first call of a
+// key runs forward(stream, in0, in1, out) eagerly on the caller's buffers, which also configures every kernel, then
+// records it as a graph on the staging buffers.  Later calls copy the inputs in, replay the graph and copy the [n, 512]
+// result out.
 template <typename F>
 int graph_call(plip_engine* e, const GraphKey& key, std::array<Staged, 2> in, float* out, cudaStream_t st,
                F&& forward) {
+  PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_last, 0));
   auto it = e->graphs.find(key);
   if (it == e->graphs.end()) {
     const size_t stage_bytes[2] = {(size_t)e->graph_max_n * pixel_bytes(PLIP_PIX_F32_NCHW),
@@ -758,6 +784,27 @@ int graph_call(plip_engine* e, const GraphKey& key, std::array<Staged, 2> in, fl
   }
   PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
   return 0;
+}
+
+// plip_dbg_hidden_states[_hw]: one pass of a tower's trunk (tower 0: height x width images, 1: 77-token captions) up
+// to num_layers encoder layers, then its residual stream X [n * S, D] copied to hidden.
+int dbg_hidden_states(const char* fn, plip_engine* e, int tower, const void* in, int fmt, const void* mask, int64_t n,
+                      int height, int width, int num_layers, float* hidden, cudaStream_t st) {
+  PLIP_REQUIRE(tower == 0 || tower == 1, "%s: tower %d out of range (0 vision, 1 text)", fn, tower);
+  PLIP_REQUIRE(num_layers >= 0 && num_layers <= kLayers, "%s: num_layers %d out of range", fn, num_layers);
+  if (int rc = tower == 0 ? check_pixels(fn, e, in, hidden, fmt, n, height, width)
+                          : check_ids(fn, e, in, hidden, fmt, n, kTxtSeq, kTxtSeq)) return rc;
+  const VisGeom geo = vis_geom(height, width);
+  const int S = tower == 0 ? geo.S : kTxtSeq, D = tower == 0 ? kVisDim : kTxtDim;
+  const int64_t per_pass = tower == 0 ? images_per_pass(e->max_mb, S) : e->max_mb;
+  PLIP_REQUIRE(n <= per_pass, "%s: n=%lld sequences of %d tokens exceed one pass (%lld)", fn, (long long)n, S,
+               (long long)per_pass);
+  return micro_batches(e, n, n, st, [&](int64_t, int64_t) {
+    if (int rc = tower == 0 ? vision_trunk(e, in, fmt, n, geo, num_layers, st)
+                            : text_trunk(e, in, fmt, mask, n, kTxtSeq, kTxtSeq, num_layers, st)) return rc;
+    PLIP_CUDA_CHECK(cudaMemcpyAsync(hidden, e->X, (size_t)n * S * D * 4, cudaMemcpyDeviceToDevice, st));
+    return 0;
+  });
 }
 
 }  // namespace
@@ -939,45 +986,27 @@ PLIP_API int plip_last_layer_pruning(const plip_engine_t* e) { return e ? e->pru
 
 PLIP_API int plip_encode_images(plip_engine_t* e, const void* pixels_dev, int pixel_format, int64_t n,
                                 float* out_dev, int normalize, void* stream) {
-  PLIP_REQUIRE(e && pixels_dev && out_dev, "plip_encode_images: null argument");
-  PLIP_REQUIRE(n > 0, "plip_encode_images: n must be positive (got %lld)", (long long)n);
-  PLIP_REQUIRE(pixel_format >= 0 && pixel_format <= 2, "plip_encode_images: unknown pixel format %d", pixel_format);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_last, 0));  // calls on different streams share one workspace
-  const size_t pb = pixel_bytes(pixel_format);
-  if (graph_eligible(e, n)) {
-    const GraphKey key{0, (int)n, pixel_format, normalize ? 1 : 0, 0, 0, 0, 0, e->prune_last};
-    return graph_call(e, key, {{{pixels_dev, (size_t)n * pb}, {nullptr, 0}}}, out_dev, st,
-                      [&](cudaStream_t s, const void* pixels, const void*, float* out) {
-                        return vision_forward(e, pixels, pixel_format, n, out, normalize, s);
-                      });
-  }
-  for (int64_t i = 0; i < n; i += e->max_mb) {
-    const int64_t mb = (n - i < e->max_mb) ? (n - i) : e->max_mb;
-    if (int rc = vision_forward(e, static_cast<const uint8_t*>(pixels_dev) + i * pb, pixel_format, mb,
-                                out_dev + i * kProj, normalize, st)) return rc;
-  }
-  PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
-  return 0;
+  return plip_encode_images_hw(e, pixels_dev, pixel_format, n, kImage, kImage, out_dev, normalize, stream);
 }
 
 PLIP_API int plip_encode_images_hw(plip_engine_t* e, const void* pixels_dev, int pixel_format, int64_t n, int height,
                                    int width, float* out_dev, int normalize, void* stream) {
-  if (int rc = check_hw_call("plip_encode_images_hw", e, pixels_dev, out_dev, pixel_format, n, height, width)) return rc;
-  if (height == kImage && width == kImage)
-    return plip_encode_images(e, pixels_dev, pixel_format, n, out_dev, normalize, stream);
+  if (int rc = check_pixels("plip_encode_images_hw", e, pixels_dev, out_dev, pixel_format, n, height, width)) return rc;
   const VisGeom geo = vis_geom(height, width);
-  const int64_t per_pass = images_per_pass(e->max_mb, geo.S);
   const size_t pb = pixel_bytes(pixel_format, height, width);
+  const bool prune = e->prune_last != 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_last, 0));  // calls on different streams share one workspace
-  for (int64_t i = 0; i < n; i += per_pass) {
-    const int64_t mb = (n - i < per_pass) ? (n - i) : per_pass;
-    if (int rc = vision_forward(e, static_cast<const uint8_t*>(pixels_dev) + i * pb, pixel_format, mb,
-                                out_dev + i * kProj, normalize, st, geo)) return rc;
+  if (height == kImage && width == kImage && graph_eligible(e, n)) {
+    const GraphKey key{0, (int)n, pixel_format, normalize ? 1 : 0, 0, 0, 0, 0, e->prune_last};
+    return graph_call(e, key, {{{pixels_dev, (size_t)n * pb}, {nullptr, 0}}}, out_dev, st,
+                      [&](cudaStream_t s, const void* pixels, const void*, float* out) {
+                        return vision_pass(e, pixels, pixel_format, n, geo, embeds_only(out, normalize), prune, s);
+                      });
   }
-  PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
-  return 0;
+  return micro_batches(e, n, images_per_pass(e->max_mb, geo.S), st, [&](int64_t i, int64_t mb) {
+    return vision_pass(e, static_cast<const uint8_t*>(pixels_dev) + i * pb, pixel_format, mb, geo,
+                       embeds_only(out_dev + i * kProj, normalize), prune, st);
+  });
 }
 
 PLIP_API int plip_encode_text(plip_engine_t* e, const void* ids_dev, int ids_dtype, const void* attention_mask_dev,
@@ -989,75 +1018,50 @@ PLIP_API int plip_encode_text(plip_engine_t* e, const void* ids_dev, int ids_dty
 PLIP_API int plip_encode_text_prefix(plip_engine_t* e, const void* ids_dev, int ids_dtype,
                                      const void* attention_mask_dev, int64_t n, int seq_len, int prefix_len,
                                      float* out_dev, int normalize, void* stream) {
-  PLIP_REQUIRE(e && ids_dev && out_dev, "plip_encode_text: null argument");
-  PLIP_REQUIRE(prefix_len >= 1 && prefix_len <= seq_len, "plip_encode_text_prefix: prefix_len %d out of [1,%d]",
-               prefix_len, seq_len);
-  PLIP_REQUIRE(n > 0, "plip_encode_text: n must be positive (got %lld)", (long long)n);
-  PLIP_REQUIRE(seq_len >= 1 && seq_len <= kTxtSeq,
-               "Sequence length must be less than max_position_embeddings (got `sequence length`: %d and "
-               "max_position_embeddings: %d)", seq_len, kTxtSeq);  // message mirrors TF:243-247
-  PLIP_REQUIRE(ids_dtype == PLIP_IDS_I32 || ids_dtype == PLIP_IDS_I64, "plip_encode_text: unknown ids dtype %d", ids_dtype);
+  if (int rc = check_ids("plip_encode_text", e, ids_dev, out_dev, ids_dtype, n, seq_len, prefix_len)) return rc;
+  const size_t row = (size_t)seq_len * (ids_dtype == PLIP_IDS_I64 ? 8 : 4);
+  const bool prune = e->prune_last != 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_last, 0));
-  const size_t isz = ids_dtype == PLIP_IDS_I64 ? 8 : 4;
   if (graph_eligible(e, n)) {
     const GraphKey key{1, (int)n, ids_dtype, normalize ? 1 : 0, seq_len, prefix_len, attention_mask_dev ? 1 : 0,
                        e->text_pool_argmax, e->prune_last};
-    const size_t ib = (size_t)n * seq_len * isz;
-    return graph_call(e, key, {{{ids_dev, ib}, {attention_mask_dev, ib}}}, out_dev, st,
+    return graph_call(e, key, {{{ids_dev, n * row}, {attention_mask_dev, n * row}}}, out_dev, st,
                       [&](cudaStream_t s, const void* ids, const void* mask, float* out) {
-                        return text_forward(e, ids, ids_dtype, mask, n, prefix_len, seq_len, out, normalize, s);
+                        return text_pass(e, ids, ids_dtype, mask, n, prefix_len, seq_len, embeds_only(out, normalize),
+                                         prune, s);
                       });
   }
-  for (int64_t i = 0; i < n; i += e->max_mb) {
-    const int64_t mb = (n - i < e->max_mb) ? (n - i) : e->max_mb;
-    const uint8_t* ids = static_cast<const uint8_t*>(ids_dev) + i * seq_len * isz;
-    const uint8_t* mk = attention_mask_dev ? static_cast<const uint8_t*>(attention_mask_dev) + i * seq_len * isz : nullptr;
-    if (int rc = text_forward(e, ids, ids_dtype, mk, mb, prefix_len, seq_len, out_dev + i * kProj, normalize, st)) return rc;
-  }
-  PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
-  return 0;
+  return micro_batches(e, n, e->max_mb, st, [&](int64_t i, int64_t mb) {
+    const uint8_t* mask = attention_mask_dev ? static_cast<const uint8_t*>(attention_mask_dev) + i * row : nullptr;
+    return text_pass(e, static_cast<const uint8_t*>(ids_dev) + i * row, ids_dtype, mask, mb, prefix_len, seq_len,
+                     embeds_only(out_dev + i * kProj, normalize), prune, st);
+  });
 }
 
 PLIP_API int plip_vision_outputs(plip_engine_t* e, const void* pixels_dev, int pixel_format, int64_t n, int height,
                                  int width, const plip_tower_outputs_t* outputs, void* stream) {
   if (int rc = check_outputs("plip_vision_outputs", outputs)) return rc;
-  if (int rc = check_hw_call("plip_vision_outputs", e, pixels_dev, outputs, pixel_format, n, height, width)) return rc;
+  if (int rc = check_pixels("plip_vision_outputs", e, pixels_dev, outputs, pixel_format, n, height, width)) return rc;
   const VisGeom geo = vis_geom(height, width);
-  const int64_t per_pass = images_per_pass(e->max_mb, geo.S);
   const size_t pb = pixel_bytes(pixel_format, height, width);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_last, 0));  // calls on different streams share one workspace
-  for (int64_t i = 0; i < n; i += per_pass) {
-    const int64_t mb = (n - i < per_pass) ? (n - i) : per_pass;
-    if (int rc = vision_outputs_pass(e, static_cast<const uint8_t*>(pixels_dev) + i * pb, pixel_format, mb, i, n, geo,
-                                     outputs, st)) return rc;
-  }
-  PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
-  return 0;
+  return micro_batches(e, n, images_per_pass(e->max_mb, geo.S), st, [&](int64_t i, int64_t mb) {
+    return vision_pass(e, static_cast<const uint8_t*>(pixels_dev) + i * pb, pixel_format, mb, geo,
+                       pass_out(*outputs, n, i, geo.S, kVisDim, kVisHeads), false, st);
+  });
 }
 
 PLIP_API int plip_text_outputs(plip_engine_t* e, const void* ids_dev, int ids_dtype, const void* attention_mask_dev,
                                int64_t n, int seq_len, const plip_tower_outputs_t* outputs, void* stream) {
-  PLIP_REQUIRE(ids_dev && outputs, "plip_text_outputs: null argument");
-  PLIP_REQUIRE(n > 0, "plip_text_outputs: n must be positive (got %lld)", (long long)n);
-  PLIP_REQUIRE(seq_len >= 1 && seq_len <= kTxtSeq,
-               "Sequence length must be less than max_position_embeddings (got `sequence length`: %d and "
-               "max_position_embeddings: %d)", seq_len, kTxtSeq);  // message mirrors TF:243-247
-  PLIP_REQUIRE(ids_dtype == PLIP_IDS_I32 || ids_dtype == PLIP_IDS_I64, "plip_text_outputs: unknown ids dtype %d", ids_dtype);
   if (int rc = check_outputs("plip_text_outputs", outputs)) return rc;
-  PLIP_REQUIRE(e != nullptr, "plip_text_outputs: null engine");
+  if (int rc = check_ids("plip_text_outputs", e, ids_dev, outputs, ids_dtype, n, seq_len, seq_len)) return rc;
+  const size_t row = (size_t)seq_len * (ids_dtype == PLIP_IDS_I64 ? 8 : 4);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_last, 0));
-  const size_t isz = ids_dtype == PLIP_IDS_I64 ? 8 : 4;
-  for (int64_t i = 0; i < n; i += e->max_mb) {
-    const int64_t mb = (n - i < e->max_mb) ? (n - i) : e->max_mb;
-    const uint8_t* ids = static_cast<const uint8_t*>(ids_dev) + i * seq_len * isz;
-    const uint8_t* mk = attention_mask_dev ? static_cast<const uint8_t*>(attention_mask_dev) + i * seq_len * isz : nullptr;
-    if (int rc = text_outputs_pass(e, ids, ids_dtype, mk, mb, seq_len, i, n, outputs, st)) return rc;
-  }
-  PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
-  return 0;
+  return micro_batches(e, n, e->max_mb, st, [&](int64_t i, int64_t mb) {
+    const uint8_t* mask = attention_mask_dev ? static_cast<const uint8_t*>(attention_mask_dev) + i * row : nullptr;
+    return text_pass(e, static_cast<const uint8_t*>(ids_dev) + i * row, ids_dtype, mask, mb, seq_len, seq_len,
+                     pass_out(*outputs, n, i, seq_len, kTxtDim, kTxtHeads), false, st);
+  });
 }
 
 PLIP_API int plip_similarity(const float* img_dev, int64_t n, const float* txt_dev, int64_t m, float scale,
@@ -1105,9 +1109,8 @@ PLIP_API int plip_dbg_resize_filter(int in_size, int out_size, int xx, int32_t* 
 // ---- host-buffer path ---------------------------------------------------------------------------
 PLIP_API int plip_encode_images_host(plip_engine_t* e, const void* pixels_host, int pixel_format, int64_t n,
                                      float* out_host, int normalize) {
-  PLIP_REQUIRE(e && pixels_host && out_host, "plip_encode_images_host: null argument");
-  PLIP_REQUIRE(n > 0, "plip_encode_images_host: n must be positive (got %lld)", (long long)n);
-  PLIP_REQUIRE(pixel_format >= 0 && pixel_format <= 2, "plip_encode_images_host: unknown pixel format %d", pixel_format);
+  if (int rc = check_pixels("plip_encode_images_host", e, pixels_host, out_host, pixel_format, n, kImage, kImage))
+    return rc;
   PLIP_CUDA_CHECK(cudaSetDevice(e->device));
   if (int rc = ensure_host_path(e)) return rc;
   PLIP_CUDA_CHECK(cudaStreamWaitEvent(e->s_compute, e->ev_last, 0));  // earlier device-API work owns the workspace
@@ -1144,7 +1147,8 @@ PLIP_API int plip_encode_images_host(plip_engine_t* e, const void* pixels_host, 
     PLIP_CUDA_CHECK(cudaMemcpyAsync(e->d_in[b], src, (size_t)mb * pb, cudaMemcpyHostToDevice, e->s_copy));
     PLIP_CUDA_CHECK(cudaEventRecord(e->ev_copied[b], e->s_copy));
     PLIP_CUDA_CHECK(cudaStreamWaitEvent(e->s_compute, e->ev_copied[b], 0));
-    if (int rc = vision_forward(e, e->d_in[b], pixel_format, mb, e->d_out + i * kProj, normalize, e->s_compute)) return rc;
+    if (int rc = vision_pass(e, e->d_in[b], pixel_format, mb, VisGeom(), embeds_only(e->d_out + i * kProj, normalize),
+                             e->prune_last != 0, e->s_compute)) return rc;
     PLIP_CUDA_CHECK(cudaEventRecord(e->ev_done[b], e->s_compute));
   }
   PLIP_CUDA_CHECK(cudaMemcpyAsync(out_host, e->d_out, (size_t)n * kProj * 4, cudaMemcpyDeviceToHost, e->s_compute));
@@ -1154,10 +1158,7 @@ PLIP_API int plip_encode_images_host(plip_engine_t* e, const void* pixels_host, 
 
 PLIP_API int plip_encode_text_host(plip_engine_t* e, const void* ids_host, int ids_dtype, const void* attention_mask_host,
                                    int64_t n, int seq_len, float* out_host, int normalize) {
-  PLIP_REQUIRE(e && ids_host && out_host, "plip_encode_text_host: null argument");
-  PLIP_REQUIRE(n > 0, "plip_encode_text_host: n must be positive (got %lld)", (long long)n);
-  PLIP_REQUIRE(seq_len >= 1 && seq_len <= kTxtSeq, "plip_encode_text_host: seq_len %d out of [1,77]", seq_len);
-  PLIP_REQUIRE(ids_dtype == PLIP_IDS_I32 || ids_dtype == PLIP_IDS_I64, "plip_encode_text_host: unknown ids dtype %d", ids_dtype);
+  if (int rc = check_ids("plip_encode_text_host", e, ids_host, out_host, ids_dtype, n, seq_len, seq_len)) return rc;
   PLIP_CUDA_CHECK(cudaSetDevice(e->device));
   if (int rc = ensure_host_path(e)) return rc;
   PLIP_CUDA_CHECK(cudaStreamWaitEvent(e->s_compute, e->ev_last, 0));
@@ -1293,38 +1294,14 @@ PLIP_API int plip_dbg_pos_interp(const float* pos_dev, int grid_h, int grid_w, f
 PLIP_API int plip_dbg_hidden_states(plip_engine_t* e, int tower, const void* input_dev, int input_format,
                                     const void* attention_mask_dev, int64_t n, int num_layers, float* hidden_dev,
                                     void* stream) {
-  PLIP_REQUIRE(e && input_dev && hidden_dev, "plip_dbg_hidden_states: null argument");
-  PLIP_REQUIRE(n > 0 && n <= e->max_mb, "plip_dbg_hidden_states: n=%lld must be in [1, max_micro_batch]", (long long)n);
-  PLIP_REQUIRE(num_layers >= 0 && num_layers <= kLayers, "plip_dbg_hidden_states: num_layers %d", num_layers);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  size_t bytes;
-  if (tower == 0) {
-    if (int rc = vision_trunk(e, input_dev, input_format, n, VisGeom(), num_layers, st)) return rc;
-    bytes = (size_t)n * kVisSeq * kVisDim * 4;
-  } else {
-    if (int rc = text_trunk(e, input_dev, input_format, attention_mask_dev, n, kTxtSeq, kTxtSeq, num_layers, st)) return rc;
-    bytes = (size_t)n * kTxtSeq * kTxtDim * 4;
-  }
-  PLIP_CUDA_CHECK(cudaMemcpyAsync(hidden_dev, e->X, bytes, cudaMemcpyDeviceToDevice, st));
-  PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
-  return 0;
+  return dbg_hidden_states("plip_dbg_hidden_states", e, tower, input_dev, input_format, attention_mask_dev, n, kImage,
+                           kImage, num_layers, hidden_dev, static_cast<cudaStream_t>(stream));
 }
 
 PLIP_API int plip_dbg_hidden_states_hw(plip_engine_t* e, const void* pixels_dev, int pixel_format, int64_t n,
                                        int height, int width, int num_layers, float* hidden_dev, void* stream) {
-  if (int rc = check_hw_call("plip_dbg_hidden_states_hw", e, pixels_dev, hidden_dev, pixel_format, n, height, width))
-    return rc;
-  const VisGeom geo = vis_geom(height, width);
-  PLIP_REQUIRE(n <= images_per_pass(e->max_mb, geo.S),
-               "plip_dbg_hidden_states_hw: n=%lld images of %d tokens exceed one pass (%lld images)", (long long)n,
-               geo.S, (long long)images_per_pass(e->max_mb, geo.S));
-  PLIP_REQUIRE(num_layers >= 0 && num_layers <= kLayers, "plip_dbg_hidden_states_hw: num_layers %d", num_layers);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_last, 0));
-  if (int rc = vision_trunk(e, pixels_dev, pixel_format, n, geo, num_layers, st)) return rc;
-  PLIP_CUDA_CHECK(cudaMemcpyAsync(hidden_dev, e->X, (size_t)n * geo.S * kVisDim * 4, cudaMemcpyDeviceToDevice, st));
-  PLIP_CUDA_CHECK(cudaEventRecord(e->ev_last, st));
-  return 0;
+  return dbg_hidden_states("plip_dbg_hidden_states_hw", e, 0, pixels_dev, pixel_format, nullptr, n, height, width,
+                           num_layers, hidden_dev, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -198,14 +198,10 @@ class Engine:
             return torch.empty(0, EMBED_DIM, device=self.device)
         pixels = self._dev(pixels)
         out = torch.empty(n, EMBED_DIM, device=self.device, dtype=torch.float32)
+        h, w = _pixel_hw(pixels, fmt)
         with torch.cuda.device(self.device):
-            if interpolate_pos_encoding:
-                h, w = _pixel_hw(pixels, fmt)
-                check(self._L.plip_encode_images_hw(self._h, pixels.data_ptr(), fmt, n, h, w, out.data_ptr(),
-                                                    int(normalize), self._stream()), "plip_encode_images_hw")
-            else:
-                check(self._L.plip_encode_images(self._h, pixels.data_ptr(), fmt, n, out.data_ptr(), int(normalize),
-                                                 self._stream()), "plip_encode_images")
+            check(self._L.plip_encode_images_hw(self._h, pixels.data_ptr(), fmt, n, h, w, out.data_ptr(),
+                                                int(normalize), self._stream()), "plip_encode_images_hw")
         return out
 
     @torch.no_grad()
@@ -413,23 +409,19 @@ class Engine:
         ``interpolate_pos_encoding``: any accepted image size, ``[n, S, 768]`` with ``S = vision_seq_len(H, W)``."""
         x = self._dev(inputs)
         n = int(x.shape[0])
-        if tower == "vision" and interpolate_pos_encoding:
-            fmt = _pixel_format(x, True)
+        if tower == "vision":
+            fmt = _pixel_format(x, interpolate_pos_encoding)
             h, w = _pixel_hw(x, fmt)
             out = torch.empty((n, vision_seq_len(h, w), 768), device=self.device, dtype=torch.float32)
             with torch.cuda.device(self.device):
                 check(self._L.plip_dbg_hidden_states_hw(self._h, x.data_ptr(), fmt, n, h, w, int(num_layers),
                                                         out.data_ptr(), self._stream()), "plip_dbg_hidden_states_hw")
             return out
-        if tower == "vision":
-            fmt, t, shape = _pixel_format(x), 0, (n, 50, 768)
-        else:
-            fmt, t, shape = _ids_dtype(x.dtype), 1, (n, 77, 512)
-            assert x.shape[1] == 77
+        assert x.shape[1] == 77
         mask = self._dev(attention_mask.to(x.dtype)) if attention_mask is not None else None
-        out = torch.empty(shape, device=self.device, dtype=torch.float32)
+        out = torch.empty((n, 77, 512), device=self.device, dtype=torch.float32)
         with torch.cuda.device(self.device):
-            check(self._L.plip_dbg_hidden_states(self._h, t, x.data_ptr(), fmt,
+            check(self._L.plip_dbg_hidden_states(self._h, 1, x.data_ptr(), _ids_dtype(x.dtype),
                                                  mask.data_ptr() if mask is not None else None, n, int(num_layers),
                                                  out.data_ptr(), self._stream()), "plip_dbg_hidden_states")
         return out

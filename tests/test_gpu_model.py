@@ -240,16 +240,19 @@ def test_calls_on_different_streams_are_serialised(engine):
     ids = synth.token_ids(64, seed=12)[0].cuda()
     ref_i = engine.encode_images(tiles).clone()
     ref_t = engine.encode_text(ids).clone()
+    ref_h = engine.hidden_states("vision", tiles, 12).clone()
     torch.cuda.synchronize()
     s1, s2 = torch.cuda.Stream(), torch.cuda.Stream()
     for _ in range(3):
         with torch.cuda.stream(s1):
             a = engine.encode_images(tiles)
         with torch.cuda.stream(s2):
+            h = engine.hidden_states("vision", tiles, 12)   # right behind the image call on the other stream
             b = engine.encode_text(ids)
         c = engine.encode_images_host(tiles.cpu())          # engine's own streams, right behind the two above
         torch.cuda.synchronize()
         assert torch.equal(a, ref_i) and torch.equal(b, ref_t) and torch.equal(c, ref_i.cpu())
+        assert torch.equal(h, ref_h)
 
 
 def test_plip_class_drop_in(state_dict, golden):

@@ -98,7 +98,7 @@ def layer(x, sd, p, heads, mask, c: Cfg, shift):
 
 
 def towers(sd, px, ids, mask, c: Cfg):
-    # vision (engine.cu vision_forward)
+    # vision (engine.cu vision_pass)
     B = px.shape[0]
     w = sd["vision_model.embeddings.patch_embedding.weight"]
     patches = px.reshape(B, 3, 7, 32, 7, 32).permute(0, 2, 4, 1, 3, 5).reshape(B, 49, 3072)
@@ -111,7 +111,7 @@ def towers(sd, px, ids, mask, c: Cfg):
         x, shift = layer(x, sd, f"vision_model.encoder.layers.{i}", 12, None, c, shift)
     pooled = O.layer_norm(x[:, 0], sd["vision_model.post_layernorm.weight"], sd["vision_model.post_layernorm.bias"])
     img = rnd(pooled, c.act) @ rnd(sd["visual_projection.weight"], c.wgt).t()
-    # text (engine.cu text_forward)
+    # text (engine.cu text_pass)
     x = O.text_embeddings(sd, ids)
     m = O.causal_mask(ids.shape[-1], mask)
     shift = x.mean(-1, keepdim=True)
