@@ -290,6 +290,16 @@ template <int ID, int THREADS>
 __device__ __forceinline__ void named_barrier_sync() {
   asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(THREADS) : "memory");
 }
+// The same with a run-time ID, and its non-waiting half: bar.arrive counts the calling warps towards the THREADS of
+// barrier ID and returns at once; the threads that complete the count with bar.sync wait for it.
+template <int THREADS>
+__device__ __forceinline__ void named_barrier_sync(uint32_t id) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "n"(THREADS) : "memory");
+}
+template <int THREADS>
+__device__ __forceinline__ void named_barrier_arrive(uint32_t id) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "n"(THREADS) : "memory");
+}
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // all committed store groups have finished READING their shared-memory source
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }

@@ -9,14 +9,20 @@
 //   fc1 + QuickGELU, fc2        TF:modeling_clip.py:347-351, TF:activations.py:117-123
 //   visual/text_projection      TF:modeling_clip.py:861,823
 //
-// Structure (one CTA per SM, 288 threads, persistent over 128 x BN output tiles):
-//   warpgroups 0-1  consumers: each owns 64 rows of the tile, issues wgmma m64nBNk16 on the staged operands and
-//                   runs the fused epilogue on its accumulator registers
+// Structure (one CTA per SM, 288 threads, persistent over 64 x BN output tiles):
+//   warpgroups 0-1  consumers, ping-pong: warpgroup w takes the CTA's tiles i with i % 2 == w, each a whole
+//                   64 x BN tile, issues wgmma m64nBNk16 on the staged operands and runs the fused epilogue on its
+//                   accumulator registers.  The main loops run one at a time, in tile order (two named barriers pass
+//                   the turn): a warpgroup hands the turn over once its last k-block is issued, so its epilogue runs
+//                   while the other warpgroup's MMAs keep the tensor cores busy.
 //   warp 8          producer: one thread feeds the shared-memory ring with TMA, A / W k-blocks of 64 bf16 (one
-//                   128B-swizzle atom wide).  A single warp instead of a register-donating warpgroup: with 288
-//                   threads the compile-time register bound already fits the 128-register accumulator (no spills)
-// CG == 2 launches clusters of two CTAs on neighbouring M blocks of the same N block: each CTA loads its own A
-// rows and one half of the W tile, which TMA multicasts into both CTAs, halving the L2 -> smem W traffic.
+//                   128B-swizzle atom wide), in the same tile order.  A single warp instead of a register-donating
+//                   warpgroup: with 288 threads the compile-time register bound fits the 128-register accumulator
+//                   without a spill in any main loop (a 384-thread CTA with setmaxnreg 40 / 232 compiled to the same
+//                   168-register bound with more epilogue spills)
+// CG == 2 launches clusters of two CTAs on neighbouring 64-row blocks of the same N block: each CTA loads its own A
+// rows and one half of the W tile, which TMA multicasts into both CTAs, halving the L2 -> smem W traffic.  Both CTAs
+// walk the same tile sequence, so their warpgroups consume each ring stage in lockstep.
 #include "gemm.cuh"
 #include "wgmma.cuh"
 
@@ -27,7 +33,7 @@ namespace plip {
 
 namespace {
 
-constexpr int BM = 128;  // rows per CTA tile: 64 per consumer warpgroup
+constexpr int BM = 64;   // rows per tile: one consumer warpgroup's wgmma m64
 constexpr int BK = 64;   // k-block: 64 bf16 = 128 B = one swizzle atom
 constexpr int kThreads = 288;
 constexpr int kConsumerWarps = 8;
@@ -36,9 +42,9 @@ constexpr uint32_t kStoreStageBytes = 16 * 128;  // one [16 rows x 64 bf16] TMA 
 
 // Staging blocks (2 KB each) per consumer warp.  The 16-bit epilogues alternate two store boxes.  The fp32 residual
 // epilogue streams x in and y out through them, one box per block in flight: two blocks at BN 256 and 128, three at
-// BN 192 (which still leaves 4 ring stages).  Each count divides the tile's BN / 32 boxes, so every tile starts at
-// block 0.  Four blocks at BN 256 would cost a ring stage (4 -> 3) and measured slower (tools/gemm_epilogue_probe.py:
-// out_proj 378 vs 351 us, fc2 638 vs 581 us on an H100 80GB HBM3 at 700 W).
+// BN 192 (which still leaves 5 ring stages).  Each count divides the tile's BN / 32 boxes, so every tile starts at
+// block 0.  Four blocks at BN 256 would cost a ring stage and measured slower with 128-row tiles
+// (tools/gemm_epilogue_probe.py: out_proj 378 vs 351 us, fc2 638 vs 581 us on an H100 80GB HBM3 at 700 W).
 constexpr int x_boxes(int BN, int EPI) {
   return EPI != EPI_BIAS_RESID_F32 ? 2 : BN == 192 ? 3 : 2;
 }
@@ -330,7 +336,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);        // the producer's arrive.expect_tx
-      mbar_init(empty_bar(s), 2 * CG);  // one arrive per consumer warpgroup of every CTA that reads the slot's W tile
+      mbar_init(empty_bar(s), CG);      // one arrive from the consuming warpgroup of every CTA that reads the slot's W tile
     }
     if constexpr (EPI == EPI_BIAS_RESID_F32) {
       tma_prefetch_desc(&tmC);
@@ -346,6 +352,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   const int num_kb = p.K / BK;
   const int tile0 = blockIdx.x / CG;
   const int tile_step = gridDim.x / CG;
+  const int my_tiles = (num_tiles - tile0 + tile_step - 1) / tile_step;  // >= 1: the grid has at most num_tiles groups
 
   if (wg == 2) {
     // ===================== TMA producer =====================
@@ -373,7 +380,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     }
     __syncwarp();
   } else {
-    // ===================== MMA + epilogue =====================
+    // ===================== MMA + epilogue, two warpgroups taking turns =====================
+    // Named barrier 1 + w completes when warpgroup w may start its next main loop: warpgroup w syncs on it (128
+    // threads) and the other warpgroup arrives on it (128) once its own main loop is issued.  The turn order also
+    // keeps each warpgroup's ring waits within one phase of the barriers it waits on.  Both warpgroups run the same
+    // number of rounds; every arrive is matched by one sync: warpgroup 1 waits for its turn even in a last round
+    // without a tile, and does not pass the turn after its last round (warpgroup 0 has nothing left to start).
     const int wtid = threadIdx.x & 127;
     auto release = [&](int s) {  // the warpgroup's wgmmas on slot s have retired
       if (wtid == 0) mbar_arrive(empty_bar(s));
@@ -384,24 +396,38 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     float d[BN / 2];
     int s = 0;
     uint32_t ph = 0;
+    auto skip_tile = [&]() {  // the other warpgroup's k-blocks in the ring
+      s += num_kb;
+      ph ^= static_cast<uint32_t>(s / STAGES) & 1u;
+      s %= STAGES;
+    };
     uint32_t stage_sel = 0;
-    for (int t = tile0; t < num_tiles; t += tile_step) {
+    const uint32_t my_turn = 1u + wg, other_turn = 2u - wg;
+    const int rounds = (my_tiles + 1) / 2;
+    if (wg == 1) skip_tile();
+    for (int r = 0; r < rounds; ++r) {
+      const int i = 2 * r + wg;
+      const int t = tile0 + i * tile_step;
       const int n_blk = t % num_n_blk;
       const int m0 = ((t / num_n_blk) * CG + cta_rank) * BM;
-      const int wrow = m0 + wg * 64 + (warp & 3) * 16;  // first of this warp's 16 rows
+      const int wrow = m0 + (warp & 3) * 16;  // first of this warp's 16 rows
       float2 ln0 = make_float2(0.f, 1.f), ln1 = make_float2(0.f, 1.f);
       if constexpr (EPI == EPI_LN_BIAS_BF16 || EPI == EPI_LN_BIAS_GELU_BF16) {
         // the row statistics are fetched before the main loop: the loads overlap the MMAs and need no registers next
         // to the full accumulator
-        ln0 = ln_row_terms(p, wrow + (lane >> 2));
-        ln1 = ln_row_terms(p, wrow + (lane >> 2) + 8);
+        if (i < my_tiles) {
+          ln0 = ln_row_terms(p, wrow + (lane >> 2));
+          ln1 = ln_row_terms(p, wrow + (lane >> 2) + 8);
+        }
       }
+      if (wg == 1 || r > 0) named_barrier_sync<256>(my_turn);
+      if (i >= my_tiles) break;  // warpgroup 1 in the last round of an odd tile count
       int prev = -1;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(full_bar(s), ph);
-        const uint32_t sa = smem_base + s * C::STAGE + wg * (64 * 128);
+        const uint32_t sa = smem_base + s * C::STAGE;
         const uint64_t adesc = make_smem_desc_sw128(sa, 1024, 16);
-        const uint64_t bdesc = make_smem_desc_sw128(smem_base + s * C::STAGE + A_STAGE, 1024, 16);
+        const uint64_t bdesc = make_smem_desc_sw128(sa + A_STAGE, 1024, 16);
         wgmma_pin(d);
         wgmma_fence();
 #pragma unroll
@@ -412,9 +438,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         prev = s;
         if (++s == STAGES) { s = 0; ph ^= 1u; }
       }
+      if (wg == 0 || r + 1 < rounds) named_barrier_arrive<256>(other_turn);
       wgmma_wait<0>();
       wgmma_pin(d);
       release(prev);
+      skip_tile();
       epilogue_warp<BN, EPI, F16>(p, &tmC, d, epi_base + warp * C::XBOXES * kStoreStageBytes, stage_sel,
                                   resid_bar + 8u * C::XBOXES * warp, wrow,
                                   n_blk * BN, n_blk, lane, ln0, ln1);
@@ -480,6 +508,8 @@ int launch_inst(const GemmArgs& g, cudaStream_t stream) {
   p.xb_out = g.xb_out; p.stats_out = g.stats_out;
   if (g.n_tiles_used) *g.n_tiles_used = 2 * (g.N / BN);
 
+  // With fewer tiles than resident groups each CTA takes one tile and its second warpgroup idles: two tiles on one SM
+  // would run their main loops one after the other, one tile on each of two SMs runs them side by side.
   const int num_tiles = ((g.M + BM * CG - 1) / (BM * CG)) * (g.N / BN);
   const int groups = max_groups < num_tiles ? max_groups : num_tiles;
   PLIP_CUDA_CHECK(launch_kernel(kern, dim3(groups * CG), dim3(kThreads), C::SMEM_BYTES, stream, CG, tmA, tmB, tmC, p));
