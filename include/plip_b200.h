@@ -32,7 +32,7 @@ extern "C" {
 
 #define PLIP_API __attribute__((visibility("default")))
 
-#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs (new symbols only) */
+#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts (new symbols only) */
 
 /* Model constants (TF:configuration_clip.py:47-64,97-109,160-161). */
 #define PLIP_IMAGE_SIZE 224
@@ -135,6 +135,28 @@ PLIP_API int plip_encode_images(plip_engine_t* e, const void* pixels_dev, int pi
  * 8 x 16 patches) run the long-sequence attention kernel (profile role "vision/attention[long]"). */
 PLIP_API int plip_encode_images_hw(plip_engine_t* e, const void* pixels_dev, int pixel_format, int64_t n, int height,
                                    int width, float* out_dev, int normalize, void* stream);
+
+/* ---- windows of a slide region --------------------------------------------------------------- */
+/* region_dev: one uint8 RGB region [height, width, 3], rows row_pitch_bytes apart (>= 3 * width; a view into a wider
+ * array is fine, no alignment is required).  origins_host: HOST int32 [n, 2] (row, col) of n 224 x 224 windows, each
+ * inside the region (0 <= row <= height - 224, 0 <= col <= width - 224); all are checked before anything is launched and
+ * the error names the first bad window.  The origins are consumed before the call returns (copied from pageable memory,
+ * which may wait for the stream's earlier work, as cudaMemcpyAsync does).  This is the crop loop of the reference's
+ * slide preprocessing (reproducibility/generate_validation_datasets/preprocess/preprocess_DigestPath.py:28-100) without
+ * cutting the crops out: the windows are read in place.
+ *
+ * plip_encode_windows: out_dev float32 [n,512] in window order, exactly what plip_encode_images returns for the same
+ * windows cut out as PLIP_PIX_U8_NHWC tiles in the same order (same micro-batches, same 67 launches per micro-batch,
+ * bit for bit); normalize as there.  The window gather runs under the profile role "vision/im2col".  Never replayed
+ * as a CUDA graph.
+ * plip_window_background_counts (no engine): counts_dev int32 [n], per window the pixels whose three channels are all
+ * >= threshold — the reference's background_ratio(window, threshold) times 224 * 224, exactly. */
+PLIP_API int plip_encode_windows(plip_engine_t* e, const void* region_dev, int height, int width,
+                                 int64_t row_pitch_bytes, const int32_t* origins_host, int64_t n, float* out_dev,
+                                 int normalize, void* stream);
+PLIP_API int plip_window_background_counts(const void* region_dev, int height, int width, int64_t row_pitch_bytes,
+                                           const int32_t* origins_host, int64_t n, int threshold, int32_t* counts_dev,
+                                           void* stream);
 
 /* Text tower + text_projection: replaces CLIPModel.get_text_features (TF:793-825, called at
  * plip.py:68) and model.encode_text (embedders/plip.py:66).

@@ -82,6 +82,8 @@ SIGNATURES = {
     "plip_max_micro_batch": (_i, [_vp]),
     "plip_encode_images": (_i, [_vp, _vp, _i, _i64, _fp, _i, _vp]),
     "plip_encode_images_hw": (_i, [_vp, _vp, _i, _i64, _i, _i, _fp, _i, _vp]),
+    "plip_encode_windows": (_i, [_vp, _vp, _i, _i, _i64, _vp, _i64, _fp, _i, _vp]),
+    "plip_window_background_counts": (_i, [_vp, _i, _i, _i64, _vp, _i64, _i, _vp, _vp]),
     "plip_encode_text": (_i, [_vp, _vp, _i, _vp, _i64, _i, _fp, _i, _vp]),
     "plip_encode_text_prefix": (_i, [_vp, _vp, _i, _vp, _i64, _i, _i, _fp, _i, _vp]),
     "plip_vision_outputs": (_i, [_vp, _vp, _i, _i64, _i, _i, C.POINTER(TowerOutputs), _vp]),

@@ -4,6 +4,8 @@
 // All are pure streaming kernels (roofline: HBM); accesses are 16-byte vectorised and coalesced.
 #include "kernels.cuh"
 
+#include <string.h>
+
 namespace plip {
 
 namespace {
@@ -32,6 +34,20 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8], int f16) {
 struct ImGeom {
   int H, W, gh, gw;
 };
+
+// 8 consecutive RGB pixels of one image row (24 bytes, interleaved) -> the three channel rows of one patch-matrix row
+// at dst (channel c at dst + c * 1024).  Shared by the tile and the window im2col, so both produce the same bits.
+__device__ __forceinline__ void store_u8_patch_row(const uint8_t (&bytes)[24], __nv_bfloat16* dst, int f16) {
+  const float mean[3] = {0.48145466f, 0.4578275f, 0.40821073f};
+  const float istd[3] = {1.0f / 0.26862954f, 1.0f / 0.26130258f, 1.0f / 0.27577711f};
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    float f[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) f[j] = (bytes[j * 3 + c] * (1.0f / 255.0f) - mean[c]) * istd[c];
+    *reinterpret_cast<uint4*>(dst + c * 1024) = pack8(f, f16);
+  }
+}
 
 template <int FMT, bool FIXED>
 __global__ void __launch_bounds__(kEwThreads) im2col_kernel(const void* __restrict__ pixels,
@@ -65,16 +81,7 @@ __global__ void __launch_bounds__(kEwThreads) im2col_kernel(const void* __restri
 #pragma unroll
         for (int j = 0; j < 24; ++j) bytes[j] = __ldg(src + j);
       }
-      const float mean[3] = {0.48145466f, 0.4578275f, 0.40821073f};
-      const float istd[3] = {1.0f / 0.26862954f, 1.0f / 0.26130258f, 1.0f / 0.27577711f};
-      __nv_bfloat16* dst = out + (b * patches + py * gw + px) * (int64_t)kPatchK + ky * 32 + kx;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        float f[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) f[j] = (bytes[j * 3 + c] * (1.0f / 255.0f) - mean[c]) * istd[c];
-        *reinterpret_cast<uint4*>(dst + c * 1024) = pack8(f, f16);
-      }
+      store_u8_patch_row(bytes, out + (b * patches + py * gw + px) * (int64_t)kPatchK + ky * 32 + kx, f16);
     } else {
       const int c = (int)(r % 3);
       const int64_t b = r / 3;
@@ -119,6 +126,90 @@ __global__ void __launch_bounds__(kEwThreads) im2col_kernel(const void* __restri
         *reinterpret_cast<uint4*>(dst) = w;
       }
     }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Windows of a slide region: 224 x 224 crops of one uint8 RGB region [H, W, 3] (row pitch in bytes, may be a view into a
+// wider array) at arbitrary (row, col) origins, read in place instead of being cut out into tiles first.
+//
+// A window row starts at byte row * pitch + 3 * col, which is 8-byte aligned for few origins (the reference's grid
+// steps by 201 pixels), so the 8-byte loads of im2col_kernel do not apply.  load24 reads the 6 or 7 aligned 32-bit
+// words that hold the 24 bytes of an 8-pixel group and realigns them with __byte_perm, one selector for the whole
+// group since the misalignment (address & 3) is the same for every word.  Versus staging each window row through shared
+// memory this needs no barrier and no second pass, and the loads of a warp's 28 active lanes fall in one 672-byte row,
+// so L1 merges them into the same sectors the aligned loads would touch.  Only words holding at least one of the 24
+// bytes are read, never one past the end of the region.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void load24(const uint8_t* src, uint8_t (&bytes)[24]) {
+  const uintptr_t a = reinterpret_cast<uintptr_t>(src);
+  const uint32_t* w = reinterpret_cast<const uint32_t*>(a & ~(uintptr_t)3);
+  const unsigned off = (unsigned)(a & 3);
+  uint32_t v[7];
+#pragma unroll
+  for (int k = 0; k < 6; ++k) v[k] = __ldg(w + k);
+  v[6] = off ? __ldg(w + 6) : 0u;
+  const unsigned sel = 0x3210u + off * 0x1111u;  // bytes off .. off + 3 of the pair (v[k], v[k + 1])
+  uint32_t* out = reinterpret_cast<uint32_t*>(bytes);
+#pragma unroll
+  for (int k = 0; k < 6; ++k) out[k] = __byte_perm(v[k], v[k + 1], sel);
+}
+
+// Window im2col: the matrix im2col_kernel<PLIP_PIX_U8_NHWC, true> builds from the same windows cut out as [n,224,224,3]
+// tiles, bit for bit (same store_u8_patch_row).  origins: device int32 (row, col) pairs, one per window.
+__global__ void __launch_bounds__(kEwThreads) window_im2col_kernel(const uint8_t* __restrict__ region, int64_t pitch,
+                                                                   const int2* __restrict__ origins, int64_t n,
+                                                                   __nv_bfloat16* __restrict__ out, int f16) {
+  constexpr int kX8 = kImage / 8;
+  const int64_t total = n * kImage * kX8;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
+       i += (int64_t)gridDim.x * blockDim.x) {
+    const int x8 = (int)(i % kX8);
+    const int64_t r = i / kX8;
+    const int y = (int)(r % kImage);
+    const int64_t b = r / kImage;
+    const int x = x8 * 8;
+    const int2 o = __ldg(origins + b);
+    alignas(16) uint8_t bytes[24];
+    load24(region + (int64_t)(o.x + y) * pitch + (int64_t)(o.y + x) * 3, bytes);
+    const int py = y >> 5, ky = y & 31, px = x >> 5, kx = x & 31;
+    store_u8_patch_row(bytes, out + (b * kPatches + py * kGrid + px) * (int64_t)kPatchK + ky * 32 + kx, f16);
+  }
+}
+
+// Background pixels of each window: those whose three channels are all >= threshold (the reference's background_ratio,
+// preprocess_DigestPath.py:28-34, times 224 * 224), as exact int32 counts.  One block per window, blocks in window
+// order: for window_grid's row-major origins the blocks resident at once cover neighbouring windows of one band of
+// rows, so the overlap of two windows is read from HBM once and hit in L2 the second time.  The origins of a launch
+// travel as kernel parameters (16 KB), so the call needs no device buffer of its own.
+constexpr int kBgBatch = 2048;
+struct WindowBatch {
+  int2 org[kBgBatch];
+};
+
+__global__ void __launch_bounds__(kEwThreads) window_background_kernel(const uint8_t* __restrict__ region, int64_t pitch,
+                                                                       const __grid_constant__ WindowBatch batch,
+                                                                       int threshold, int32_t* __restrict__ counts) {
+  constexpr int kX8 = kImage / 8;
+  const int2 o = batch.org[blockIdx.x];
+  int cnt = 0;
+  for (int i = threadIdx.x; i < kImage * kX8; i += blockDim.x) {
+    const int y = i / kX8, x = (i % kX8) * 8;
+    alignas(16) uint8_t bytes[24];
+    load24(region + (int64_t)(o.x + y) * pitch + (int64_t)(o.y + x) * 3, bytes);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      cnt += (bytes[3 * j] >= threshold) & (bytes[3 * j + 1] >= threshold) & (bytes[3 * j + 2] >= threshold);
+  }
+  __shared__ int part[kEwThreads / 32];
+  cnt = __reduce_add_sync(0xffffffffu, cnt);
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = cnt;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int s = 0;
+#pragma unroll
+    for (int k = 0; k < kEwThreads / 32; ++k) s += part[k];
+    counts[blockIdx.x] = s;
   }
 }
 
@@ -422,6 +513,30 @@ int launch_im2col(const void* pixels, int fmt, int64_t n, int height, int width,
     default: set_last_error("im2col: unknown pixel format %d", fmt); return -2;
   }
 #undef PLIP_IM2COL
+  PLIP_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+int launch_window_im2col(const WindowSrc& win, int64_t n, __nv_bfloat16* out, int f16, cudaStream_t st) {
+  PLIP_REQUIRE(n > 0 && win.region && win.origins && out, "window_im2col: bad argument");
+  PLIP_REQUIRE((reinterpret_cast<uintptr_t>(win.origins) & 7) == 0, "window_im2col: origins must be 8-byte aligned");
+  const int grid = grid_for(n * kImage * (kImage / 8), kEwThreads);
+  PLIP_CUDA_CHECK(launch_kernel(window_im2col_kernel, dim3(grid), dim3(kEwThreads), 0, st, 1, win.region, win.pitch,
+                                reinterpret_cast<const int2*>(win.origins), n, out, f16));
+  PLIP_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+int launch_window_background(const uint8_t* region, int64_t pitch, const int32_t* origins_host, int64_t n,
+                             int threshold, int32_t* counts, cudaStream_t st) {
+  PLIP_REQUIRE(n > 0 && region && origins_host && counts, "window_background: bad argument");
+  static thread_local WindowBatch b;  // 16 KB: kept off the stack
+  for (int64_t base = 0; base < n; base += kBgBatch) {
+    const int cnt = (int)(n - base < kBgBatch ? n - base : kBgBatch);
+    memcpy(b.org, origins_host + 2 * base, (size_t)cnt * sizeof(int2));
+    PLIP_CUDA_CHECK(launch_kernel(window_background_kernel, dim3(cnt), dim3(kEwThreads), 0, st, 1, region, pitch, b,
+                                  threshold, counts + base));
+  }
   PLIP_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

@@ -131,6 +131,16 @@ VisGeom vis_geom(int height, int width) {
   return g;
 }
 
+// Pixels of a vision pass: mb tiles at `pixels` in `fmt`, or, when win.region is set, mb 224 x 224 windows of a uint8
+// RGB region (plip_encode_windows; win.origins points at the pass's first origin).
+struct VisInput {
+  const void* pixels;
+  int fmt;
+  WindowSrc win;
+};
+
+VisInput tiles(const void* pixels, int fmt) { return VisInput{pixels, fmt, WindowSrc{nullptr, 0, nullptr}}; }
+
 // The workspace holds kVisSeq * max_mb vision token rows (and max_mb pooled rows): images per pass at S tokens each.
 int64_t images_per_pass(int max_mb, int S) {
   const int64_t n = (int64_t)kVisSeq * max_mb / S;
@@ -199,6 +209,8 @@ struct plip_engine {
   size_t d_out_bytes = 0;
   void* d_aux = nullptr;  // ids + mask for the text host path
   size_t d_aux_bytes = 0;
+  int32_t* d_win = nullptr;  // window origins of plip_encode_windows, int32 [n, 2] (lazy)
+  size_t d_win_bytes = 0;
   // small-batch path: the ~67 launches of a tower are replayed as ONE CUDA graph per GraphKey on engine-owned
   // staging buffers (inputs are copied in, the [n,512] result copied out), which removes the host-side launch cost
   // that dominates when a forward is only a few hundred microseconds of GPU work (reference default:
@@ -429,7 +441,7 @@ int run_layers(plip_engine* e, const LayerW* L, int64_t n_seq, int S, int D, int
 }
 
 // Vision tower up to (and including) `num_layers` encoder layers; X holds the residual stream [mb * geo.S, 768].
-int vision_trunk(plip_engine* e, const void* pixels, int fmt, int64_t mb, const VisGeom& geo, int num_layers,
+int vision_trunk(plip_engine* e, const VisInput& in, int64_t mb, const VisGeom& geo, int num_layers,
                  cudaStream_t st, bool prune = false, const PassOut& out = PassOut(),
                  const float** pooled_x = nullptr) {
   e->prof_tower = 0;
@@ -445,8 +457,11 @@ int vision_trunk(plip_engine* e, const void* pixels, int fmt, int64_t mb, const 
     pos = table;
   }
   {
-    ProfScope ps(e, st, PK_IM2COL, 0, dmb * (double)pixel_bytes(fmt, geo.H, geo.W) + dmb * patches * kPatchK * 2);
-    if (int rc = launch_im2col(pixels, fmt, mb, geo.H, geo.W, e->H, e->f16, st)) return rc;
+    // windows: fmt is PLIP_PIX_U8_NHWC and geo 224 x 224, so the bytes are those of the same windows as tiles
+    ProfScope ps(e, st, PK_IM2COL, 0, dmb * (double)pixel_bytes(in.fmt, geo.H, geo.W) + dmb * patches * kPatchK * 2);
+    const int rc = in.win.region ? launch_window_im2col(in.win, mb, e->H, e->f16, st)
+                                 : launch_im2col(in.pixels, in.fmt, mb, geo.H, geo.W, e->H, e->f16, st);
+    if (rc) return rc;
   }
   GemmArgs g;
   g.A = e->H; g.lda = kPatchK; g.W = e->v_patch_w; g.ldw = kPatchK;
@@ -493,10 +508,10 @@ int pooled_head(plip_engine* e, const float* pooled_x, const int32_t* pool_idx, 
 
 // One vision pass over mb images: the whole tower, then what `out` asks for.  prune: see run_layers (the embedding
 // calls only).  last_hidden_state is the residual stream after the last layer, before post_layernorm (TF:680-686).
-int vision_pass(plip_engine* e, const void* pixels, int fmt, int64_t mb, const VisGeom& geo, const PassOut& out,
-                bool prune, cudaStream_t st) {
+int vision_pass(plip_engine* e, const VisInput& in, int64_t mb, const VisGeom& geo, const PassOut& out, bool prune,
+                cudaStream_t st) {
   const float* pooled_x = nullptr;
-  if (int rc = vision_trunk(e, pixels, fmt, mb, geo, kLayers, st, prune, out, &pooled_x)) return rc;
+  if (int rc = vision_trunk(e, in, mb, geo, kLayers, st, prune, out, &pooled_x)) return rc;
   if (out.last_hidden)
     PLIP_CUDA_CHECK(cudaMemcpyAsync(out.last_hidden, e->X, (size_t)mb * geo.S * kVisDim * 4, cudaMemcpyDeviceToDevice,
                                     st));
@@ -722,6 +737,25 @@ int check_outputs(const char* fn, const plip_tower_outputs_t* o) {
   return 0;
 }
 
+// Arguments of a call on n 224 x 224 windows of a height x width uint8 RGB region (rows row_pitch bytes apart): every
+// host origin (row, col) is checked against the region before anything is launched, and a bad one is named.
+int check_windows(const char* fn, const void* region, int height, int width, int64_t row_pitch,
+                  const int32_t* origins, int64_t n, const void* out) {
+  PLIP_REQUIRE(region && origins && out, "%s: null argument", fn);
+  PLIP_REQUIRE(n > 0, "%s: n must be positive (got %lld)", fn, (long long)n);
+  PLIP_REQUIRE(height >= kImage && width >= kImage, "%s: region %dx%d is smaller than one %dx%d window", fn, height,
+               width, kImage, kImage);
+  PLIP_REQUIRE(row_pitch >= 3LL * width, "%s: row pitch %lld bytes < 3 * width = %lld", fn, (long long)row_pitch,
+               3LL * width);
+  for (int64_t i = 0; i < n; ++i) {
+    const int r = origins[2 * i], c = origins[2 * i + 1];
+    PLIP_REQUIRE(r >= 0 && c >= 0 && r <= height - kImage && c <= width - kImage,
+                 "%s: window %lld at (%d, %d) is outside the %dx%d region (rows 0..%d, columns 0..%d)", fn,
+                 (long long)i, r, c, height, width, height - kImage, width - kImage);
+  }
+  return 0;
+}
+
 // The protocol of an eager device-pointer call: calls on different streams share one workspace, so the call waits for
 // its last use, runs pass(i, mb) over items [i, i + mb) in passes of at most per_pass, and marks its own last use.
 template <typename F>
@@ -800,7 +834,7 @@ int dbg_hidden_states(const char* fn, plip_engine* e, int tower, const void* in,
   PLIP_REQUIRE(n <= per_pass, "%s: n=%lld sequences of %d tokens exceed one pass (%lld)", fn, (long long)n, S,
                (long long)per_pass);
   return micro_batches(e, n, n, st, [&](int64_t, int64_t) {
-    if (int rc = tower == 0 ? vision_trunk(e, in, fmt, n, geo, num_layers, st)
+    if (int rc = tower == 0 ? vision_trunk(e, tiles(in, fmt), n, geo, num_layers, st)
                             : text_trunk(e, in, fmt, mask, n, kTxtSeq, kTxtSeq, num_layers, st)) return rc;
     PLIP_CUDA_CHECK(cudaMemcpyAsync(hidden, e->X, (size_t)n * S * D * 4, cudaMemcpyDeviceToDevice, st));
     return 0;
@@ -917,6 +951,7 @@ PLIP_API int plip_destroy(plip_engine_t* e) {
   }
   if (e->d_out) cudaFree(e->d_out);
   if (e->d_aux) cudaFree(e->d_aux);
+  if (e->d_win) cudaFree(e->d_win);
   if (e->ev_last) cudaEventDestroy(e->ev_last);
   for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);
   for (void* p : e->g_in)
@@ -1000,13 +1035,44 @@ PLIP_API int plip_encode_images_hw(plip_engine_t* e, const void* pixels_dev, int
     const GraphKey key{0, (int)n, pixel_format, normalize ? 1 : 0, 0, 0, 0, 0, e->prune_last};
     return graph_call(e, key, {{{pixels_dev, (size_t)n * pb}, {nullptr, 0}}}, out_dev, st,
                       [&](cudaStream_t s, const void* pixels, const void*, float* out) {
-                        return vision_pass(e, pixels, pixel_format, n, geo, embeds_only(out, normalize), prune, s);
+                        return vision_pass(e, tiles(pixels, pixel_format), n, geo, embeds_only(out, normalize), prune,
+                                           s);
                       });
   }
   return micro_batches(e, n, images_per_pass(e->max_mb, geo.S), st, [&](int64_t i, int64_t mb) {
-    return vision_pass(e, static_cast<const uint8_t*>(pixels_dev) + i * pb, pixel_format, mb, geo,
+    return vision_pass(e, tiles(static_cast<const uint8_t*>(pixels_dev) + i * pb, pixel_format), mb, geo,
                        embeds_only(out_dev + i * kProj, normalize), prune, st);
   });
+}
+
+PLIP_API int plip_encode_windows(plip_engine_t* e, const void* region_dev, int height, int width,
+                                 int64_t row_pitch_bytes, const int32_t* origins_host, int64_t n, float* out_dev,
+                                 int normalize, void* stream) {
+  if (int rc = check_windows("plip_encode_windows", region_dev, height, width, row_pitch_bytes, origins_host, n,
+                             out_dev)) return rc;
+  PLIP_REQUIRE(e != nullptr, "plip_encode_windows: null engine");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // the engine's origin buffer may still be read by the previous call (any stream): wait for it before the upload
+  PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_last, 0));
+  if (int rc = grow_dev(reinterpret_cast<void**>(&e->d_win), &e->d_win_bytes, (size_t)n * 2 * sizeof(int32_t)))
+    return rc;
+  PLIP_CUDA_CHECK(cudaMemcpyAsync(e->d_win, origins_host, (size_t)n * 2 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  const bool prune = e->prune_last != 0;
+  const uint8_t* region = static_cast<const uint8_t*>(region_dev);
+  // the micro-batches of plip_encode_images on tiles (no graph replay: its staging buffers hold tiles)
+  return micro_batches(e, n, images_per_pass(e->max_mb, kVisSeq), st, [&](int64_t i, int64_t mb) {
+    const VisInput in{nullptr, PLIP_PIX_U8_NHWC, WindowSrc{region, row_pitch_bytes, e->d_win + 2 * i}};
+    return vision_pass(e, in, mb, VisGeom(), embeds_only(out_dev + i * kProj, normalize), prune, st);
+  });
+}
+
+PLIP_API int plip_window_background_counts(const void* region_dev, int height, int width, int64_t row_pitch_bytes,
+                                           const int32_t* origins_host, int64_t n, int threshold, int32_t* counts_dev,
+                                           void* stream) {
+  if (int rc = check_windows("plip_window_background_counts", region_dev, height, width, row_pitch_bytes,
+                             origins_host, n, counts_dev)) return rc;
+  return launch_window_background(static_cast<const uint8_t*>(region_dev), row_pitch_bytes, origins_host, n, threshold,
+                                  counts_dev, static_cast<cudaStream_t>(stream));
 }
 
 PLIP_API int plip_encode_text(plip_engine_t* e, const void* ids_dev, int ids_dtype, const void* attention_mask_dev,
@@ -1046,7 +1112,7 @@ PLIP_API int plip_vision_outputs(plip_engine_t* e, const void* pixels_dev, int p
   const size_t pb = pixel_bytes(pixel_format, height, width);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   return micro_batches(e, n, images_per_pass(e->max_mb, geo.S), st, [&](int64_t i, int64_t mb) {
-    return vision_pass(e, static_cast<const uint8_t*>(pixels_dev) + i * pb, pixel_format, mb, geo,
+    return vision_pass(e, tiles(static_cast<const uint8_t*>(pixels_dev) + i * pb, pixel_format), mb, geo,
                        pass_out(*outputs, n, i, geo.S, kVisDim, kVisHeads), false, st);
   });
 }
@@ -1147,8 +1213,8 @@ PLIP_API int plip_encode_images_host(plip_engine_t* e, const void* pixels_host, 
     PLIP_CUDA_CHECK(cudaMemcpyAsync(e->d_in[b], src, (size_t)mb * pb, cudaMemcpyHostToDevice, e->s_copy));
     PLIP_CUDA_CHECK(cudaEventRecord(e->ev_copied[b], e->s_copy));
     PLIP_CUDA_CHECK(cudaStreamWaitEvent(e->s_compute, e->ev_copied[b], 0));
-    if (int rc = vision_pass(e, e->d_in[b], pixel_format, mb, VisGeom(), embeds_only(e->d_out + i * kProj, normalize),
-                             e->prune_last != 0, e->s_compute)) return rc;
+    if (int rc = vision_pass(e, tiles(e->d_in[b], pixel_format), mb, VisGeom(),
+                             embeds_only(e->d_out + i * kProj, normalize), e->prune_last != 0, e->s_compute)) return rc;
     PLIP_CUDA_CHECK(cudaEventRecord(e->ev_done[b], e->s_compute));
   }
   PLIP_CUDA_CHECK(cudaMemcpyAsync(out_host, e->d_out, (size_t)n * kProj * 4, cudaMemcpyDeviceToHost, e->s_compute));

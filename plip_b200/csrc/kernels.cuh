@@ -12,6 +12,19 @@ namespace plip {
 // [n * gh * gw, 3072], gh = height / 32, gw = width / 32.
 int launch_im2col(const void* pixels, int fmt, int64_t n, int height, int width, __nv_bfloat16* out, int f16,
                   cudaStream_t st);
+// 224 x 224 windows of one uint8 RGB region [H, W, 3] with a row pitch in bytes.  origins: int32 (row, col) pairs, one
+// per window, each window inside the region (the callers check that on the host).
+struct WindowSrc {
+  const uint8_t* region;
+  int64_t pitch;
+  const int32_t* origins;  // device memory, 8-byte aligned
+};
+// n windows -> the patch matrix [n * 49, 3072], bit-identical to launch_im2col of the same windows as u8 tiles.
+int launch_window_im2col(const WindowSrc& win, int64_t n, __nv_bfloat16* out, int f16, cudaStream_t st);
+// Per window, the pixels whose three channels are all >= threshold -> counts int32 [n].  origins_host: host memory,
+// consumed before the call returns.
+int launch_window_background(const uint8_t* region, int64_t pitch, const int32_t* origins_host, int64_t n,
+                             int threshold, int32_t* counts, cudaStream_t st);
 // The vision position table resized to a gh x gw patch grid: fp32 [1 + gh * gw, 768] (bicubic, as HF).
 int launch_pos_interp(const float* pos, int gh, int gw, float* out, cudaStream_t st);
 int launch_layernorm(const float* x, const int32_t* row_index, int64_t in_row_stride, int64_t rows, int dim,

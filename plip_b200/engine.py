@@ -85,6 +85,66 @@ def _check_ids(input_ids, attention_mask) -> Tuple[int, int]:
     return n, s
 
 
+WINDOW = IMAGE_SIZE  # the side of a region window (plip_encode_windows)
+
+
+def check_region(region: Union[torch.Tensor, np.ndarray]) -> Tuple[int, int, int]:
+    """Validate a uint8 RGB region ``[H, W, 3]`` whose pixels are packed (channel stride 1, pixel stride 3; rows may be
+    any number of bytes apart, e.g. a view into a wider array) and at least one window in size.  Returns
+    ``(H, W, row_pitch_bytes)``; raises ``ValueError`` otherwise."""
+    if region.dtype not in (torch.uint8, np.dtype("uint8")):
+        raise ValueError(f"a region must be uint8 RGB [H, W, 3], got dtype {region.dtype}")
+    shape = tuple(region.shape)
+    if len(shape) != 3 or shape[2] != 3:
+        raise ValueError(f"a region must be uint8 RGB [H, W, 3], got shape {shape}")
+    h, w = int(shape[0]), int(shape[1])
+    if h < WINDOW or w < WINDOW:
+        raise ValueError(f"region {h}x{w} is smaller than one {WINDOW}x{WINDOW} window")
+    strides = region.stride() if torch.is_tensor(region) else tuple(s // region.itemsize for s in region.strides)
+    if strides[2] != 1 or strides[1] != 3 or strides[0] < 3 * w:
+        raise ValueError(f"a region needs packed RGB pixels (strides (>= 3 * W, 3, 1) in bytes), got strides {strides}")
+    return h, w, int(strides[0])
+
+
+def check_origins(origins, height: int, width: int) -> np.ndarray:
+    """``[n, 2]`` (row, col) window origins as a contiguous int32 array, each window inside the ``height x width``
+    region; ``ValueError`` naming the first window that is not."""
+    o = np.asarray(origins.cpu() if torch.is_tensor(origins) else origins)
+    if o.size == 0:
+        return np.zeros((0, 2), np.int32)
+    if o.ndim != 2 or o.shape[1] != 2 or o.dtype.kind not in "iu":
+        raise ValueError(f"origins must be integer [n, 2] (row, col), got {o.dtype} {o.shape}")
+    bad = (o[:, 0] < 0) | (o[:, 1] < 0) | (o[:, 0] > height - WINDOW) | (o[:, 1] > width - WINDOW)
+    if bad.any():
+        i = int(np.flatnonzero(bad)[0])
+        raise ValueError(f"window {i} at ({int(o[i, 0])}, {int(o[i, 1])}) is outside the {height}x{width} region "
+                         f"(rows 0..{height - WINDOW}, columns 0..{width - WINDOW})")
+    return np.ascontiguousarray(o, dtype=np.int32)
+
+
+def _device_region(region) -> Tuple[int, int, int]:
+    if not (torch.is_tensor(region) and region.is_cuda):
+        raise ValueError("the region must be a CUDA tensor here; host regions go through plip_b200.regions.encode_region")
+    return check_region(region)
+
+
+@torch.no_grad()
+def window_background_counts(region: torch.Tensor, origins, threshold: int = 200) -> torch.Tensor:
+    """Per window, the pixels whose three channels are all ``>= threshold``: int32 ``[n]`` on the region's device,
+    exact (``plip_window_background_counts``; needs no engine).  ``count / 50176`` is the reference's
+    ``background_ratio`` of the window."""
+    h, w, pitch = _device_region(region)
+    o = check_origins(origins, h, w)
+    n = int(o.shape[0])
+    out = torch.empty(n, device=region.device, dtype=torch.int32)
+    if n:
+        with torch.cuda.device(region.device):
+            check(lib().plip_window_background_counts(region.data_ptr(), h, w, pitch, o.ctypes.data, n, int(threshold),
+                                                      out.data_ptr(), torch.cuda.current_stream(region.device).cuda_stream),
+                  "plip_window_background_counts")
+    return out
+
+
 @torch.no_grad()
 def similarity_topk(query: torch.Tensor, space: torch.Tensor, k: int, scale: float = 1.0, normalize_query: bool = True,
                     normalize_space: bool = False, device: Union[int, str, torch.device, None] = None):
@@ -203,6 +263,28 @@ class Engine:
             check(self._L.plip_encode_images_hw(self._h, pixels.data_ptr(), fmt, n, h, w, out.data_ptr(),
                                                 int(normalize), self._stream()), "plip_encode_images_hw")
         return out
+
+    @torch.no_grad()
+    def encode_windows(self, region: torch.Tensor, origins, normalize: bool = False) -> torch.Tensor:
+        """224 x 224 windows of one uint8 RGB region ``[H, W, 3]`` on this engine's device (a row-strided view is fine)
+        at ``origins`` (``[n, 2]`` (row, col), host or device) -> ``[n, 512]`` f32 (device), in window order: bit for
+        bit what ``encode_images`` returns for the same windows cut out as uint8 tiles, without cutting them out
+        (``plip_encode_windows``)."""
+        h, w, pitch = _device_region(region)
+        o = check_origins(origins, h, w)
+        n = int(o.shape[0])
+        out = torch.empty(n, EMBED_DIM, device=self.device, dtype=torch.float32)
+        if n:
+            if region.device != self.device:
+                raise ValueError(f"the region is on {region.device}, the engine on {self.device}")
+            with torch.cuda.device(self.device):
+                check(self._L.plip_encode_windows(self._h, region.data_ptr(), h, w, pitch, o.ctypes.data, n,
+                                                  out.data_ptr(), int(normalize), self._stream()), "plip_encode_windows")
+        return out
+
+    def window_background_counts(self, region: torch.Tensor, origins, threshold: int = 200) -> torch.Tensor:
+        """See the module-level :func:`window_background_counts`."""
+        return window_background_counts(region, origins, threshold)
 
     @torch.no_grad()
     def encode_text(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor] = None,

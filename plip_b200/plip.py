@@ -120,6 +120,17 @@ class PLIP:
         pbar.close()
         return out
 
+    def encode_region(self, region, crop_overlap: float = 0.1, non_bg_threshold: float = 0.5):
+        """The crops the reference's slide preprocessing keeps (``random_crop`` with ``downsample = 1``,
+        ``preprocess_DigestPath.py:36-108``), encoded: ``region`` is an RGB uint8 ``[H, W, 3]`` array, CPU / CUDA tensor
+        or PIL image.  Returns ``(embeddings [k,512] float32 un-normalised, origins [k,2] int32 (row, col),
+        tissue_ratio [k] float64)`` as numpy arrays, in the reference's crop order (``regions.encode_region``)."""
+        from .regions import encode_region
+        if isinstance(region, PIL.Image.Image):
+            region = np.asarray(region.convert("RGB"))
+        res = encode_region(self.model.engine, region, crop_overlap=crop_overlap, non_bg_threshold=non_bg_threshold)
+        return res.embeddings.cpu().numpy(), res.origins, res.tissue_ratio
+
     def _tokenize(self, text: List[str]):
         if self.preprocess is None and self.tokenizer is None:
             raise RuntimeError("no tokenizer available for this checkpoint (no vocab.json + merges.txt next to it, "
