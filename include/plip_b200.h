@@ -32,7 +32,7 @@ extern "C" {
 
 #define PLIP_API __attribute__((visibility("default")))
 
-#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts (new symbols only) */
+#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts, plip_window_mask_counts, plip_resize_region_*, plip_resize_filter_bounds (new symbols only) */
 
 /* Model constants (TF:configuration_clip.py:47-64,97-109,160-161). */
 #define PLIP_IMAGE_SIZE 224
@@ -157,6 +157,14 @@ PLIP_API int plip_encode_windows(plip_engine_t* e, const void* region_dev, int h
 PLIP_API int plip_window_background_counts(const void* region_dev, int height, int width, int64_t row_pitch_bytes,
                                            const int32_t* origins_host, int64_t n, int threshold, int32_t* counts_dev,
                                            void* stream);
+/* plip_window_mask_counts (no engine): mask_dev is a uint8 mask [height, width] (channels = 1) or [height, width, 3]
+ * (channels = 3), rows row_pitch_bytes apart (>= channels * width); origins as above.  counts_dev int32 [n]: per
+ * window, the mask elements > threshold, every channel counted — the reference's (msk_np > 10) followed by
+ * np.sum(msk_patch_np > 0).  Its tumour ratios divide by 224 * 224 whatever the channel count, so an RGB mask can give
+ * a ratio above 1; that is kept. */
+PLIP_API int plip_window_mask_counts(const void* mask_dev, int height, int width, int channels,
+                                     int64_t row_pitch_bytes, const int32_t* origins_host, int64_t n, int threshold,
+                                     int32_t* counts_dev, void* stream);
 
 /* Text tower + text_projection: replaces CLIPModel.get_text_features (TF:793-825, called at
  * plip.py:68) and model.encode_text (embedders/plip.py:66).
@@ -242,6 +250,30 @@ typedef struct plip_resize_desc {
 } plip_resize_desc_t;
 PLIP_API int plip_resize_crop_u8(const void* src_dev, uint64_t src_bytes, const plip_resize_desc_t* descs_host,
                                  int64_t n, void* tiles_dev, void* stream);
+
+/* Whole-image resize on the device, bit-identical to PIL.Image.fromarray(src).resize((new_width, new_height)) (BICUBIC,
+ * no reducing_gap) for any ratio from upscaling to shrinks of over 64x (the horizontal filter must fit 64 columns in
+ * 200 KB of shared memory: about 200x).  The source is a height x width RGB uint8 image, the output new_height x
+ * new_width; sizes 1..65536.  The call writes output rows [out_row0, out_row1) and reads only the source rows their
+ * vertical filter windows cover; the filters are always those of the full image, so ranges stitched together equal
+ * the whole image.
+ *   src_dev: source row src_row0 of the image; src_rows rows are readable from there, src_row_pitch bytes apart
+ *            (>= 3 * width, no alignment needed): a band of a larger image, or the whole image (0, height).
+ *   out_dev: output row out_row0, rows out_row_pitch bytes apart (>= 3 * new_width).
+ *   workspace_dev: 16-byte aligned device memory of at least plip_resize_region_workspace(...) bytes (filter tables
+ *            and the uint8 intermediate image of Pillow's horizontal pass); the call allocates nothing.
+ * Every argument is checked before anything is launched, including that the band holds the source rows the output
+ * rows read; an error names the offending value.  Stream-ordered, three launches. */
+PLIP_API int plip_resize_region_workspace(int height, int width, int new_height, int new_width, int out_row0,
+                                          int out_row1, uint64_t* bytes);
+PLIP_API int plip_resize_region_u8(const void* src_dev, int64_t src_row_pitch, int src_row0, int src_rows, int height,
+                                   int width, void* out_dev, int64_t out_row_pitch, int new_height, int new_width,
+                                   int out_row0, int out_row1, void* workspace_dev, uint64_t workspace_bytes,
+                                   void* stream);
+/* Host-only: the filter window of every output index of one resize axis (in_size -> out_size, 1..65536), as the
+ * kernels compute it: bounds_host int32 [out_size][2] = (first source index, count).  Output index i reads source
+ * indices [first, first + count). */
+PLIP_API int plip_resize_filter_bounds(int in_size, int out_size, int32_t* bounds_host);
 
 /* ---- host-buffer convenience (end-to-end path; copies are inside the call) ------------------- */
 /* pixels_host / ids_host / out_host are host pointers (pinned or pageable).  The call stages

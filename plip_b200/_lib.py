@@ -91,7 +91,11 @@ SIGNATURES = {
     "plip_similarity": (_i, [_fp, _i64, _fp, _i64, _f, _i, _i, _fp, _i64, _vp]),
     "plip_similarity_topk": (_i, [_fp, _i64, _fp, _i64, _f, _i, _i, _i, _vp, _fp, _vp]),
     "plip_l2_normalize": (_i, [_fp, _i64, _i, _vp]),
+    "plip_window_mask_counts": (_i, [_vp, _i, _i, _i, _i64, _vp, _i64, _i, _vp, _vp]),
     "plip_resize_crop_u8": (_i, [_vp, _u64, _vp, _i64, _vp, _vp]),
+    "plip_resize_region_workspace": (_i, [_i, _i, _i, _i, _i, _i, C.POINTER(_u64)]),
+    "plip_resize_region_u8": (_i, [_vp, _i64, _i, _i, _i, _i, _vp, _i64, _i, _i, _i, _i, _vp, _u64, _vp]),
+    "plip_resize_filter_bounds": (_i, [_i, _i, _vp]),
     "plip_encode_images_host": (_i, [_vp, _vp, _i, _i64, _fp, _i]),
     "plip_encode_text_host": (_i, [_vp, _vp, _i, _vp, _i64, _i, _fp, _i]),
     "plip_profile_enable": (_i, [_vp, _i]),

@@ -177,6 +177,20 @@ __global__ void __launch_bounds__(kEwThreads) window_im2col_kernel(const uint8_t
   }
 }
 
+// The sum of `cnt` over the block, stored by thread 0 at dst.
+__device__ __forceinline__ void store_block_sum(int cnt, int32_t* dst) {
+  __shared__ int part[kEwThreads / 32];
+  cnt = __reduce_add_sync(0xffffffffu, cnt);
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = cnt;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int s = 0;
+#pragma unroll
+    for (int k = 0; k < kEwThreads / 32; ++k) s += part[k];
+    *dst = s;
+  }
+}
+
 // Background pixels of each window: those whose three channels are all >= threshold (the reference's background_ratio,
 // preprocess_DigestPath.py:28-34, times 224 * 224), as exact int32 counts.  One block per window, blocks in window
 // order: for window_grid's row-major origins the blocks resident at once cover neighbouring windows of one band of
@@ -201,16 +215,41 @@ __global__ void __launch_bounds__(kEwThreads) window_background_kernel(const uin
     for (int j = 0; j < 8; ++j)
       cnt += (bytes[3 * j] >= threshold) & (bytes[3 * j + 1] >= threshold) & (bytes[3 * j + 2] >= threshold);
   }
-  __shared__ int part[kEwThreads / 32];
-  cnt = __reduce_add_sync(0xffffffffu, cnt);
-  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = cnt;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    int s = 0;
-#pragma unroll
-    for (int k = 0; k < kEwThreads / 32; ++k) s += part[k];
-    counts[blockIdx.x] = s;
+  store_block_sum(cnt, counts + blockIdx.x);
+}
+
+// Mask elements > threshold in each window of a uint8 mask [H, W, C] (C = 1 or 3), as exact int32 counts: the
+// reference's (msk_np > 10) then np.sum(msk_patch_np > 0) (preprocess_DigestPath.py:58-62, 83-84), which counts every
+// channel of an RGB mask.  Same launch shape as window_background_kernel; level-sized masks are small, so plain byte
+// loads (coalesced along the window row) suffice.
+template <int C>
+__global__ void __launch_bounds__(kEwThreads) window_mask_kernel(const uint8_t* __restrict__ mask, int64_t pitch,
+                                                                 const __grid_constant__ WindowBatch batch,
+                                                                 int threshold, int32_t* __restrict__ counts) {
+  constexpr int kRow = kImage * C;
+  const int2 o = batch.org[blockIdx.x];
+  const uint8_t* base = mask + (int64_t)o.x * pitch + (int64_t)o.y * C;
+  int cnt = 0;
+  for (int i = threadIdx.x; i < kImage * kRow; i += blockDim.x) {
+    const int y = i / kRow, x = i - y * kRow;
+    cnt += (int)__ldg(base + (int64_t)y * pitch + x) > threshold;
   }
+  store_block_sum(cnt, counts + blockIdx.x);
+}
+
+// One launch of `kernel` per kBgBatch windows, the origins passed by value.
+template <typename K>
+int launch_window_batches(K kernel, const uint8_t* src, int64_t pitch, const int32_t* origins_host, int64_t n,
+                          int threshold, int32_t* counts, cudaStream_t st) {
+  static thread_local WindowBatch b;  // 16 KB: kept off the stack
+  for (int64_t base = 0; base < n; base += kBgBatch) {
+    const int cnt = (int)(n - base < kBgBatch ? n - base : kBgBatch);
+    memcpy(b.org, origins_host + 2 * base, (size_t)cnt * sizeof(int2));
+    PLIP_CUDA_CHECK(launch_kernel(kernel, dim3(cnt), dim3(kEwThreads), 0, st, 1, src, pitch, b, threshold,
+                                  counts + base));
+  }
+  PLIP_CUDA_CHECK(cudaGetLastError());
+  return 0;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -530,15 +569,15 @@ int launch_window_im2col(const WindowSrc& win, int64_t n, __nv_bfloat16* out, in
 int launch_window_background(const uint8_t* region, int64_t pitch, const int32_t* origins_host, int64_t n,
                              int threshold, int32_t* counts, cudaStream_t st) {
   PLIP_REQUIRE(n > 0 && region && origins_host && counts, "window_background: bad argument");
-  static thread_local WindowBatch b;  // 16 KB: kept off the stack
-  for (int64_t base = 0; base < n; base += kBgBatch) {
-    const int cnt = (int)(n - base < kBgBatch ? n - base : kBgBatch);
-    memcpy(b.org, origins_host + 2 * base, (size_t)cnt * sizeof(int2));
-    PLIP_CUDA_CHECK(launch_kernel(window_background_kernel, dim3(cnt), dim3(kEwThreads), 0, st, 1, region, pitch, b,
-                                  threshold, counts + base));
-  }
-  PLIP_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return launch_window_batches(window_background_kernel, region, pitch, origins_host, n, threshold, counts, st);
+}
+
+int launch_window_mask(const uint8_t* mask, int64_t pitch, int channels, const int32_t* origins_host, int64_t n,
+                       int threshold, int32_t* counts, cudaStream_t st) {
+  PLIP_REQUIRE(n > 0 && mask && origins_host && counts, "window_mask: bad argument");
+  PLIP_REQUIRE(channels == 1 || channels == 3, "window_mask: channels must be 1 or 3 (got %d)", channels);
+  return launch_window_batches(channels == 1 ? window_mask_kernel<1> : window_mask_kernel<3>, mask, pitch,
+                               origins_host, n, threshold, counts, st);
 }
 
 int launch_pos_interp(const float* pos, int gh, int gw, float* out, cudaStream_t st) {

@@ -737,16 +737,17 @@ int check_outputs(const char* fn, const plip_tower_outputs_t* o) {
   return 0;
 }
 
-// Arguments of a call on n 224 x 224 windows of a height x width uint8 RGB region (rows row_pitch bytes apart): every
-// host origin (row, col) is checked against the region before anything is launched, and a bad one is named.
+// Arguments of a call on n 224 x 224 windows of a height x width uint8 region of `channels` bytes per pixel (rows
+// row_pitch bytes apart): every host origin (row, col) is checked against the region before anything is launched, and
+// a bad one is named.
 int check_windows(const char* fn, const void* region, int height, int width, int64_t row_pitch,
-                  const int32_t* origins, int64_t n, const void* out) {
+                  const int32_t* origins, int64_t n, const void* out, int channels = 3) {
   PLIP_REQUIRE(region && origins && out, "%s: null argument", fn);
   PLIP_REQUIRE(n > 0, "%s: n must be positive (got %lld)", fn, (long long)n);
   PLIP_REQUIRE(height >= kImage && width >= kImage, "%s: region %dx%d is smaller than one %dx%d window", fn, height,
                width, kImage, kImage);
-  PLIP_REQUIRE(row_pitch >= 3LL * width, "%s: row pitch %lld bytes < 3 * width = %lld", fn, (long long)row_pitch,
-               3LL * width);
+  PLIP_REQUIRE(row_pitch >= (int64_t)channels * width, "%s: row pitch %lld bytes < %d * width = %lld", fn,
+               (long long)row_pitch, channels, (long long)channels * width);
   for (int64_t i = 0; i < n; ++i) {
     const int r = origins[2 * i], c = origins[2 * i + 1];
     PLIP_REQUIRE(r >= 0 && c >= 0 && r <= height - kImage && c <= width - kImage,
@@ -1075,6 +1076,16 @@ PLIP_API int plip_window_background_counts(const void* region_dev, int height, i
                                   counts_dev, static_cast<cudaStream_t>(stream));
 }
 
+PLIP_API int plip_window_mask_counts(const void* mask_dev, int height, int width, int channels,
+                                     int64_t row_pitch_bytes, const int32_t* origins_host, int64_t n, int threshold,
+                                     int32_t* counts_dev, void* stream) {
+  PLIP_REQUIRE(channels == 1 || channels == 3, "plip_window_mask_counts: channels must be 1 or 3 (got %d)", channels);
+  if (int rc = check_windows("plip_window_mask_counts", mask_dev, height, width, row_pitch_bytes, origins_host, n,
+                             counts_dev, channels)) return rc;
+  return launch_window_mask(static_cast<const uint8_t*>(mask_dev), row_pitch_bytes, channels, origins_host, n,
+                            threshold, counts_dev, static_cast<cudaStream_t>(stream));
+}
+
 PLIP_API int plip_encode_text(plip_engine_t* e, const void* ids_dev, int ids_dtype, const void* attention_mask_dev,
                               int64_t n, int seq_len, float* out_dev, int normalize, void* stream) {
   return plip_encode_text_prefix(e, ids_dev, ids_dtype, attention_mask_dev, n, seq_len, seq_len, out_dev, normalize,
@@ -1163,6 +1174,29 @@ PLIP_API int plip_resize_crop_u8(const void* src_dev, uint64_t src_bytes, const 
   PLIP_REQUIRE(n > 0, "plip_resize_crop_u8: n must be positive (got %lld)", (long long)n);
   return launch_resize_crop(static_cast<const uint8_t*>(src_dev), (size_t)src_bytes, descs_host, n,
                             static_cast<uint8_t*>(tiles_dev), static_cast<cudaStream_t>(stream));
+}
+
+PLIP_API int plip_resize_region_workspace(int height, int width, int new_height, int new_width, int out_row0,
+                                          int out_row1, uint64_t* bytes) {
+  PLIP_REQUIRE(bytes, "plip_resize_region_workspace: null argument");
+  return resize_region_workspace(height, width, new_height, new_width, out_row0, out_row1, bytes);
+}
+
+PLIP_API int plip_resize_region_u8(const void* src_dev, int64_t src_row_pitch, int src_row0, int src_rows, int height,
+                                   int width, void* out_dev, int64_t out_row_pitch, int new_height, int new_width,
+                                   int out_row0, int out_row1, void* workspace_dev, uint64_t workspace_bytes,
+                                   void* stream) {
+  PLIP_REQUIRE(src_dev && out_dev && workspace_dev, "plip_resize_region_u8: null argument");
+  return launch_resize_region(static_cast<const uint8_t*>(src_dev), src_row_pitch, src_row0, src_rows, height, width,
+                              static_cast<uint8_t*>(out_dev), out_row_pitch, new_height, new_width, out_row0, out_row1,
+                              static_cast<uint8_t*>(workspace_dev), workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+PLIP_API int plip_resize_filter_bounds(int in_size, int out_size, int32_t* bounds_host) {
+  PLIP_REQUIRE(bounds_host, "plip_resize_filter_bounds: null argument");
+  PLIP_REQUIRE(in_size >= 1 && out_size >= 1 && in_size <= 65536 && out_size <= 65536,
+               "plip_resize_filter_bounds: sizes %d -> %d are outside 1..65536", in_size, out_size);
+  return resize_filter_bounds(in_size, out_size, bounds_host);
 }
 
 PLIP_API int plip_dbg_resize_filter(int in_size, int out_size, int xx, int32_t* k_host, int k_cap, int* xmin,

@@ -25,6 +25,9 @@ int launch_window_im2col(const WindowSrc& win, int64_t n, __nv_bfloat16* out, in
 // consumed before the call returns.
 int launch_window_background(const uint8_t* region, int64_t pitch, const int32_t* origins_host, int64_t n,
                              int threshold, int32_t* counts, cudaStream_t st);
+// Per window of a uint8 mask [H, W, channels] (channels 1 or 3), the elements > threshold -> counts int32 [n].
+int launch_window_mask(const uint8_t* mask, int64_t pitch, int channels, const int32_t* origins_host, int64_t n,
+                       int threshold, int32_t* counts, cudaStream_t st);
 // The vision position table resized to a gh x gw patch grid: fp32 [1 + gh * gw, 768] (bicubic, as HF).
 int launch_pos_interp(const float* pos, int gh, int gw, float* out, cudaStream_t st);
 int launch_layernorm(const float* x, const int32_t* row_index, int64_t in_row_stride, int64_t rows, int dim,
@@ -46,6 +49,16 @@ int launch_resize_crop(const uint8_t* src, size_t src_bytes, const plip_resize_d
                        uint8_t* tiles, cudaStream_t st);
 
 int resize_filter_host(int in_size, int out_size, int xx, int32_t* k, int k_cap, int* xmin, int* count);
+// The same resample over whole images at any shrink: output rows [o0, o1) of the new_h x new_w resize of an h x w RGB
+// uint8 image, from the band of src_rows source rows starting at source row src_row0 (src points at that row).  out
+// points at output row o0.  ws: a 16-byte aligned device workspace of resize_region_workspace bytes.  Every argument
+// is checked before anything is launched.
+int resize_region_workspace(int h, int w, int new_h, int new_w, int o0, int o1, uint64_t* bytes);
+int launch_resize_region(const uint8_t* src, int64_t src_pitch, int src_row0, int src_rows, int h, int w, uint8_t* out,
+                         int64_t out_pitch, int new_h, int new_w, int o0, int o1, uint8_t* ws, uint64_t ws_bytes,
+                         cudaStream_t st);
+// Per output index of one axis, its filter window: bounds[2 * xx] = first source index, bounds[2 * xx + 1] = count.
+int resize_filter_bounds(int in_size, int out_size, int32_t* bounds);
 
 // attention.cu: softmax(q k^T [+causal/padding mask]) v per (sequence, head); q pre-scaled by dh^-0.5.
 // qkv: bf16 [n_seq*seq_len, 3*heads*64]; key_mask: optional int32 [n_seq, seq_len] (0 = masked key).

@@ -371,4 +371,211 @@ int launch_resize_crop(const uint8_t* src, size_t src_bytes, const plip_resize_d
   return 0;
 }
 
+// ---- whole-image resize (plip_resize_region_u8) --------------------------------------------------------------------
+// The same resample at any shrink, whole output rows instead of a 224 x 224 crop: Pillow's own two passes through a
+// uint8 intermediate in global memory, so no filter table or strip has to fit in shared memory at once.
+//   1. resize_filters_kernel: the filter rows of every output column and of the requested output rows, one thread
+//      each (make_axis + filter_row, as above), zero-padded to a multiple of 4 taps.
+//   2. resize_rows_h_kernel: CTAs of 64 output columns x 64 source rows; the columns' filter rows are staged in shared
+//      memory and each thread walks down rows of one column (hpass_pixel) into the intermediate
+//      [s1 - s0 + 3][new_w * 3 rounded up to 4 bytes] (source rows [s0, s1) that the requested output rows touch).
+//   3. resize_rows_v_kernel: one CTA row per output row, one thread per 4 output bytes; the row's filter is read
+//      through the read-only cache (the same address in every lane).
+// Roofline: HBM, source + 2 x intermediate + output bytes.  An output-row range [o0, o1) uses the filters of the full
+// image, so ranges stitched together are the whole image bit for bit.
+namespace {
+
+constexpr int kRgCols = 64;                         // output columns per horizontal-pass CTA
+constexpr int kRgRowLanes = kRsThreads / kRgCols;   // threads per column
+constexpr int kRgRowsPerCta = 64;                   // source rows per horizontal-pass CTA
+constexpr size_t kRgSmemHard = 200 * 1024;
+
+size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
+
+struct RegionPlan {
+  int ksh4, ksv4;
+  int s0, s1;                // source rows the vertical windows of the output rows cover
+  int64_t tmp_pitch;         // intermediate row pitch in bytes (a multiple of 4)
+  size_t kh, bh, kv, bv, tmp, total;  // workspace offsets (16-byte aligned) and size
+};
+
+__global__ void __launch_bounds__(kRsThreads) resize_filters_kernel(int w, int new_w, int h, int new_h, int o0, int nv,
+                                                                    int ksh4, int ksv4, int* __restrict__ kh,
+                                                                    int2* __restrict__ bh, int* __restrict__ kv,
+                                                                    int2* __restrict__ bv) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= new_w + nv) return;
+  const bool horiz = i < new_w;
+  const int j = horiz ? i : i - new_w, k4 = horiz ? ksh4 : ksv4;
+  int* k = (horiz ? kh : kv) + (size_t)j * k4;
+  int lo, cnt;
+  if (horiz)
+    filter_row(make_axis(w, new_w), w, j, k, lo, cnt);
+  else
+    filter_row(make_axis(h, new_h), h, o0 + j, k, lo, cnt);
+  for (int x = cnt; x < k4; ++x) k[x] = 0;
+  (horiz ? bh : bv)[j] = make_int2(lo, cnt);
+}
+
+// src: the first of `rows` source rows to filter (the band's row s0); src_bytes: readable bytes from src on.
+__global__ void __launch_bounds__(kRsThreads) resize_rows_h_kernel(const uint8_t* __restrict__ src, int64_t pitch,
+                                                                   uint64_t src_bytes, int rows, int new_w, int ksh4,
+                                                                   const int* __restrict__ kh,
+                                                                   const int2* __restrict__ bh,
+                                                                   uint8_t* __restrict__ tmp, int64_t tmp_pitch) {
+  extern __shared__ __align__(16) uint8_t rs_smem[];
+  int* ks = reinterpret_cast<int*>(rs_smem);  // [kRgCols][ksh4]
+  const int c0 = blockIdx.x * kRgCols;
+  const int ncols = min(kRgCols, new_w - c0);
+  const int4* g4 = reinterpret_cast<const int4*>(kh + (size_t)c0 * ksh4);
+  for (int i = threadIdx.x; i < ncols * ksh4 / 4; i += kRsThreads) reinterpret_cast<int4*>(ks)[i] = g4[i];
+  __syncthreads();
+  const int c = threadIdx.x % kRgCols, lane = threadIdx.x / kRgCols;
+  if (c >= ncols) return;
+  const int2 b = bh[c0 + c];
+  const int cnt4 = (b.y + 3) & ~3;
+  const int* k = ks + c * ksh4;
+  const uint8_t* end_b = src + src_bytes;
+  const uint32_t* end_w = reinterpret_cast<const uint32_t*>(reinterpret_cast<uintptr_t>(end_b) & ~(uintptr_t)3);
+  const uint8_t* lim = reinterpret_cast<const uint8_t*>(end_w);
+  const int r1 = min(rows, (int)(blockIdx.y + 1) * kRgRowsPerCta);
+  for (int r = blockIdx.y * kRgRowsPerCta + lane; r < r1; r += kRgRowLanes) {
+    const uint8_t* p = src + (int64_t)r * pitch + (int64_t)b.x * 3;
+    int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0;
+    if (p + 3 * cnt4 + 8 <= lim)  // words read: [p & ~3, ... + 3*cnt4 + 4) bytes
+      hpass_pixel<false>(p, k, cnt4, end_w, end_b, a0, a1, a2);
+    else
+      hpass_pixel<true>(p, k, cnt4, end_w, end_b, a0, a1, a2);
+    uint8_t* d = tmp + (int64_t)r * tmp_pitch + (c0 + c) * 3;
+    d[0] = (uint8_t)clip8(a0);
+    d[1] = (uint8_t)clip8(a1);
+    d[2] = (uint8_t)clip8(a2);
+  }
+}
+
+// tmp row 0 is source row s0; out: output row o0 (blockIdx.x = 0); row_bytes = new_w * 3.
+__global__ void __launch_bounds__(kRsThreads) resize_rows_v_kernel(const uint8_t* __restrict__ tmp, int64_t tmp_pitch,
+                                                                   int s0, const int* __restrict__ kv,
+                                                                   const int2* __restrict__ bv, int ksv4,
+                                                                   uint8_t* __restrict__ out, int64_t out_pitch,
+                                                                   int row_bytes) {
+  const int j = blockIdx.x;
+  const int e = blockIdx.y * kRsThreads + threadIdx.x;  // 32-bit word of the row
+  if (4 * e >= row_bytes) return;
+  const int2 b = __ldg(bv + j);
+  const int cnt4 = (b.y + 3) & ~3;
+  const int tw = (int)(tmp_pitch / 4);
+  const uint32_t* sp = reinterpret_cast<const uint32_t*>(tmp + (int64_t)(b.x - s0) * tmp_pitch) + e;
+  const int4* k4 = reinterpret_cast<const int4*>(kv + (size_t)j * ksv4);
+  int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0, a3 = a0;
+  for (int y = 0; y < cnt4; y += 4) {  // taps beyond the window have zero weight (the intermediate has 3 spare rows)
+    const int4 kk = __ldg(k4++);
+    const uint32_t w0 = __ldg(sp), w1 = __ldg(sp + tw), w2 = __ldg(sp + 2 * tw), w3 = __ldg(sp + 3 * tw);
+    sp += 4 * tw;
+    a0 += byte_of(w0, 0) * kk.x + byte_of(w1, 0) * kk.y + byte_of(w2, 0) * kk.z + byte_of(w3, 0) * kk.w;
+    a1 += byte_of(w0, 1) * kk.x + byte_of(w1, 1) * kk.y + byte_of(w2, 1) * kk.z + byte_of(w3, 1) * kk.w;
+    a2 += byte_of(w0, 2) * kk.x + byte_of(w1, 2) * kk.y + byte_of(w2, 2) * kk.z + byte_of(w3, 2) * kk.w;
+    a3 += byte_of(w0, 3) * kk.x + byte_of(w1, 3) * kk.y + byte_of(w2, 3) * kk.z + byte_of(w3, 3) * kk.w;
+  }
+  const uint32_t v = clip8(a0) | (clip8(a1) << 8) | (clip8(a2) << 16) | (clip8(a3) << 24);
+  uint8_t* d = out + (int64_t)j * out_pitch + 4 * e;
+  if ((reinterpret_cast<uintptr_t>(d) & 3) == 0 && 4 * e + 4 <= row_bytes) {
+    *reinterpret_cast<uint32_t*>(d) = v;
+  } else {
+    for (int i = 0; i < 4 && 4 * e + i < row_bytes; ++i) d[i] = (uint8_t)(v >> (8 * i));
+  }
+}
+
+// Window [first, first + count) of output index xx of one axis, from the same filter_row the kernels run.
+void filter_window(int in_size, int out_size, int xx, int& first, int& count) {
+  const AxisFilter f = make_axis(in_size, out_size);
+  int* k = static_cast<int*>(malloc(sizeof(int) * (size_t)f.ksize));
+  filter_row(f, in_size, xx, k, first, count);
+  free(k);
+}
+
+int plan_region(const char* fn, int h, int w, int new_h, int new_w, int o0, int o1, RegionPlan& p) {
+  PLIP_REQUIRE(h >= 1 && w >= 1 && h <= 65536 && w <= 65536, "%s: source size %dx%d is outside 1..65536", fn, h, w);
+  PLIP_REQUIRE(new_h >= 1 && new_w >= 1 && new_h <= 65536 && new_w <= 65536,
+               "%s: output size %dx%d is outside 1..65536", fn, new_h, new_w);
+  PLIP_REQUIRE(o0 >= 0 && o0 < o1 && o1 <= new_h, "%s: output rows [%d, %d) are not a non-empty range of 0..%d", fn,
+               o0, o1, new_h);
+  p.ksh4 = (axis_ksize(w, new_w) + 3) & ~3;
+  p.ksv4 = (axis_ksize(h, new_h) + 3) & ~3;
+  PLIP_REQUIRE((size_t)kRgCols * p.ksh4 * sizeof(int) <= kRgSmemHard,
+               "%s: width %d -> %d shrinks too much (horizontal filter of %d taps; at most %d)", fn, w, new_w,
+               axis_ksize(w, new_w), (int)(kRgSmemHard / (kRgCols * sizeof(int))));
+  int f0, n0, f1, n1;
+  filter_window(h, new_h, o0, f0, n0);
+  filter_window(h, new_h, o1 - 1, f1, n1);
+  p.s0 = f0, p.s1 = f1 + n1;
+  p.tmp_pitch = ((int64_t)new_w * 3 + 3) & ~(int64_t)3;
+  const int nv = o1 - o0;
+  p.kh = 0;
+  p.bh = align16(p.kh + (size_t)new_w * p.ksh4 * sizeof(int));
+  p.kv = align16(p.bh + (size_t)new_w * sizeof(int2));
+  p.bv = align16(p.kv + (size_t)nv * p.ksv4 * sizeof(int));
+  p.tmp = align16(p.bv + (size_t)nv * sizeof(int2));
+  p.total = align16(p.tmp + (size_t)(p.s1 - p.s0 + kStripPadRows) * p.tmp_pitch);
+  return 0;
+}
+
+}  // namespace
+
+int resize_region_workspace(int h, int w, int new_h, int new_w, int o0, int o1, uint64_t* bytes) {
+  RegionPlan p;
+  if (int rc = plan_region("plip_resize_region_workspace", h, w, new_h, new_w, o0, o1, p)) return rc;
+  *bytes = p.total;
+  return 0;
+}
+
+int resize_filter_bounds(int in_size, int out_size, int32_t* bounds) {
+  for (int xx = 0; xx < out_size; ++xx) filter_window(in_size, out_size, xx, bounds[2 * xx], bounds[2 * xx + 1]);
+  return 0;
+}
+
+int launch_resize_region(const uint8_t* src, int64_t src_pitch, int src_row0, int src_rows, int h, int w, uint8_t* out,
+                         int64_t out_pitch, int new_h, int new_w, int o0, int o1, uint8_t* ws, uint64_t ws_bytes,
+                         cudaStream_t st) {
+  const char* fn = "plip_resize_region_u8";
+  RegionPlan p;
+  if (int rc = plan_region(fn, h, w, new_h, new_w, o0, o1, p)) return rc;
+  PLIP_REQUIRE(src_pitch >= 3LL * w, "%s: source row pitch %lld bytes < 3 * width = %lld", fn, (long long)src_pitch,
+               3LL * w);
+  PLIP_REQUIRE(out_pitch >= 3LL * new_w, "%s: output row pitch %lld bytes < 3 * new_width = %lld", fn,
+               (long long)out_pitch, 3LL * new_w);
+  PLIP_REQUIRE(src_row0 >= 0 && src_rows >= 1 && (int64_t)src_row0 + src_rows <= h,
+               "%s: source band of %d rows at row %d is not inside the %d source rows", fn, src_rows, src_row0, h);
+  PLIP_REQUIRE(p.s0 >= src_row0 && p.s1 <= src_row0 + src_rows,
+               "%s: output rows [%d, %d) read source rows [%d, %d), the band holds rows [%d, %d)", fn, o0, o1, p.s0,
+               p.s1, src_row0, src_row0 + src_rows);
+  PLIP_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 15) == 0, "%s: the workspace must be 16-byte aligned", fn);
+  PLIP_REQUIRE(ws_bytes >= p.total, "%s: workspace of %llu bytes, %llu needed (plip_resize_region_workspace)", fn,
+               (unsigned long long)ws_bytes, (unsigned long long)p.total);
+  static unsigned long long configured = 0;
+  if (first_use_on_device(configured))
+    PLIP_CUDA_CHECK(cudaFuncSetAttribute(resize_rows_h_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)kRgSmemHard));
+  int* kh = reinterpret_cast<int*>(ws + p.kh);
+  int2* bh = reinterpret_cast<int2*>(ws + p.bh);
+  int* kv = reinterpret_cast<int*>(ws + p.kv);
+  int2* bv = reinterpret_cast<int2*>(ws + p.bv);
+  uint8_t* tmp = ws + p.tmp;
+  const int nv = o1 - o0, rows = p.s1 - p.s0;
+  PLIP_CUDA_CHECK(launch_kernel(resize_filters_kernel, dim3((new_w + nv + kRsThreads - 1) / kRsThreads),
+                                dim3(kRsThreads), 0, st, 1, w, new_w, h, new_h, o0, nv, p.ksh4, p.ksv4, kh, bh, kv, bv));
+  const uint8_t* band = src + (int64_t)(p.s0 - src_row0) * src_pitch;
+  const uint64_t band_bytes = (uint64_t)(src_row0 + src_rows - 1 - p.s0) * src_pitch + 3ULL * w;
+  PLIP_CUDA_CHECK(launch_kernel(resize_rows_h_kernel,
+                                dim3((new_w + kRgCols - 1) / kRgCols, (rows + kRgRowsPerCta - 1) / kRgRowsPerCta),
+                                dim3(kRsThreads), (size_t)kRgCols * p.ksh4 * sizeof(int), st, 1, band, src_pitch,
+                                band_bytes, rows, new_w, p.ksh4, kh, bh, tmp, p.tmp_pitch));
+  const int row_bytes = new_w * 3;
+  PLIP_CUDA_CHECK(launch_kernel(resize_rows_v_kernel,
+                                dim3(nv, ((row_bytes + 3) / 4 + kRsThreads - 1) / kRsThreads), dim3(kRsThreads), 0, st, 1,
+                                tmp, p.tmp_pitch, p.s0, kv, bv, p.ksv4, out, out_pitch, row_bytes));
+  PLIP_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
 }  // namespace plip

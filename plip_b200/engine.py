@@ -145,6 +145,133 @@ def window_background_counts(region: torch.Tensor, origins, threshold: int = 200
     return out
 
 
+def _packed_u8(t, what: str, channels) -> Tuple[int, int, int, int]:
+    """``(H, W, C, row_pitch_bytes)`` of a uint8 ``[H, W]`` / ``[H, W, C]`` array with packed pixels (rows may be any
+    number of bytes apart), ``C`` in ``channels``; ``ValueError`` otherwise."""
+    if t.dtype not in (torch.uint8, np.dtype("uint8")):
+        raise ValueError(f"{what} must be uint8, got dtype {t.dtype}")
+    shape = tuple(t.shape)
+    c = shape[2] if len(shape) == 3 else 1
+    if len(shape) not in (2, 3) or c not in channels:
+        raise ValueError(f"{what} must be uint8 {' or '.join('[H, W]' if k == 1 else f'[H, W, {k}]' for k in channels)}"
+                         f", got shape {shape}")
+    h, w = int(shape[0]), int(shape[1])
+    if h < 1 or w < 1:
+        raise ValueError(f"{what} is empty ({h}x{w})")
+    strides = tuple(t.stride()) if torch.is_tensor(t) else tuple(s // t.itemsize for s in t.strides)
+    if (len(shape) == 3 and strides[2] != 1) or strides[1] != c or strides[0] < c * w:
+        raise ValueError(f"{what} needs packed pixels (strides (>= {c} * W, {c}{', 1' if len(shape) == 3 else ''}) in "
+                         f"bytes), got strides {strides}")
+    return h, w, c, int(strides[0])
+
+
+MAX_RESIZE = 65536
+_RC_BAD_ARGUMENT = -2  # PLIP_REQUIRE: an argument the library rejected before any launch
+
+
+def _check_args(rc: int, what: str) -> None:
+    """``check``, but an argument the library rejected raises ``ValueError`` (nothing was launched)."""
+    if rc == _RC_BAD_ARGUMENT:
+        from ._lib import last_error
+        raise ValueError(f"{what}: {last_error()}")
+    check(rc, what)
+
+
+def resize_filter_bounds(in_size: int, out_size: int) -> np.ndarray:
+    """The filter window of every output index of one resize axis, as the device resize computes it
+    (``plip_resize_filter_bounds``; host only): int32 ``[out_size, 2]`` = (first source index, count)."""
+    if not (1 <= in_size <= MAX_RESIZE and 1 <= out_size <= MAX_RESIZE):
+        raise ValueError(f"resize sizes {in_size} -> {out_size} are outside 1..{MAX_RESIZE}")
+    b = np.zeros((out_size, 2), np.int32)
+    check(lib().plip_resize_filter_bounds(int(in_size), int(out_size), b.ctypes.data), "plip_resize_filter_bounds")
+    return b
+
+
+class ResizeWorkspace:
+    """Device scratch of ``plip_resize_region_u8``, grown on demand and reused across calls on one stream."""
+
+    def __init__(self, device):
+        self.device, self.buf = torch.device(device), None
+
+    def get(self, nbytes: int) -> torch.Tensor:
+        if self.buf is None or self.buf.numel() < nbytes:
+            self.buf = torch.empty(nbytes, dtype=torch.uint8, device=self.device)  # caching-allocator blocks: 512-aligned
+        return self.buf
+
+
+@torch.no_grad()
+def resize_rows(band: torch.Tensor, src_row0: int, height: int, new_h: int, new_w: int, rows: Tuple[int, int],
+                out: torch.Tensor, workspace: Optional[ResizeWorkspace] = None) -> torch.Tensor:
+    """Output rows ``[o0, o1)`` of the ``new_h x new_w`` Pillow-bicubic resize of a ``height x W`` RGB uint8 image, of
+    which ``band`` (CUDA ``[rows, W, 3]``, rows may be strided) holds the rows from ``src_row0`` on; written into
+    ``out`` (CUDA uint8 ``[o1 - o0, new_w, 3]``, rows may be strided).  The filters are the full image's, so ranges
+    stitched together are the whole resize bit for bit.  ``plip_resize_region_u8``; every argument, including that the
+    band holds the source rows the range reads, is checked before any launch (``ValueError``)."""
+    if not (torch.is_tensor(band) and band.is_cuda):
+        raise ValueError("resize_rows: the source must be a CUDA tensor")
+    bh, w, _, pitch = _packed_u8(band, "the source", (3,))
+    o0, o1 = int(rows[0]), int(rows[1])
+    if not (1 <= height <= MAX_RESIZE and 1 <= w <= MAX_RESIZE and 1 <= new_h <= MAX_RESIZE and 1 <= new_w <= MAX_RESIZE):
+        raise ValueError(f"resize {height}x{w} -> {new_h}x{new_w}: sizes must be in 1..{MAX_RESIZE}")
+    if not 0 <= o0 < o1 <= new_h:
+        raise ValueError(f"output rows [{o0}, {o1}) are not a non-empty range of 0..{new_h}")
+    if not (0 <= src_row0 and src_row0 + bh <= height):
+        raise ValueError(f"a band of {bh} rows at row {src_row0} is not inside the {height} source rows")
+    if not (torch.is_tensor(out) and out.is_cuda and out.device == band.device):
+        raise ValueError(f"the output must be a CUDA tensor on {band.device}")
+    oh, ow, _, opitch = _packed_u8(out, "the output", (3,))
+    if (oh, ow) != (o1 - o0, new_w):
+        raise ValueError(f"the output is {oh}x{ow}, rows [{o0}, {o1}) of width {new_w} need {o1 - o0}x{new_w}")
+    L = lib()
+    need = C.c_uint64(0)
+    _check_args(L.plip_resize_region_workspace(int(height), w, int(new_h), int(new_w), o0, o1, C.byref(need)),
+                "plip_resize_region_workspace")
+    ws = (workspace or ResizeWorkspace(band.device)).get(int(need.value))
+    with torch.cuda.device(band.device):
+        _check_args(L.plip_resize_region_u8(band.data_ptr(), pitch, int(src_row0), bh, int(height), w, out.data_ptr(),
+                                            opitch, int(new_h), int(new_w), o0, o1, ws.data_ptr(), ws.numel(),
+                                            torch.cuda.current_stream(band.device).cuda_stream), "plip_resize_region_u8")
+    return out
+
+
+def resize_region(region: torch.Tensor, new_h: int, new_w: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``PIL.Image.fromarray(region).resize((new_w, new_h))`` on the device, bit for bit (antialiased BICUBIC, no
+    reducing_gap), at any ratio from upscaling to shrinks of over 64x: CUDA uint8 ``[H, W, 3]`` (rows may be strided)
+    -> ``[new_h, new_w, 3]`` (``out``, which may be a row-strided view, or a new tensor).  Needs no engine."""
+    if not (torch.is_tensor(region) and region.is_cuda):
+        raise ValueError("resize_region: the region must be a CUDA tensor")
+    h = _packed_u8(region, "a region", (3,))[0]
+    if out is None:
+        if not (1 <= new_h <= MAX_RESIZE and 1 <= new_w <= MAX_RESIZE):
+            raise ValueError(f"output size {new_h}x{new_w} is outside 1..{MAX_RESIZE}")
+        out = torch.empty((int(new_h), int(new_w), 3), dtype=torch.uint8, device=region.device)
+    return resize_rows(region, 0, h, int(new_h), int(new_w), (0, int(new_h)), out)
+
+
+@torch.no_grad()
+def window_mask_counts(mask: torch.Tensor, origins, threshold: int = 10) -> torch.Tensor:
+    """Per window, the mask elements ``> threshold``: int32 ``[n]`` on the mask's device, exact
+    (``plip_window_mask_counts``; needs no engine).  ``mask``: CUDA uint8 ``[H, W]`` or ``[H, W, 3]`` (a decoded L or
+    RGB mask; rows may be strided).  An RGB mask counts every channel, as the reference's ``np.sum(msk_patch_np > 0)``
+    does, so ``count / 50176`` can exceed 1 there."""
+    if not (torch.is_tensor(mask) and mask.is_cuda):
+        raise ValueError("window_mask_counts: the mask must be a CUDA tensor")
+    h, w, c, pitch = _packed_u8(mask, "a mask", (1, 3))
+    if h < WINDOW or w < WINDOW:
+        raise ValueError(f"mask {h}x{w} is smaller than one {WINDOW}x{WINDOW} window")
+    if not -(2 ** 31) <= int(threshold) < 2 ** 31:
+        raise ValueError(f"threshold {threshold} does not fit int32")
+    o = check_origins(origins, h, w)
+    n = int(o.shape[0])
+    out = torch.empty(n, device=mask.device, dtype=torch.int32)
+    if n:
+        with torch.cuda.device(mask.device):
+            check(lib().plip_window_mask_counts(mask.data_ptr(), h, w, c, pitch, o.ctypes.data, n, int(threshold),
+                                                out.data_ptr(), torch.cuda.current_stream(mask.device).cuda_stream),
+                  "plip_window_mask_counts")
+    return out
+
+
 @torch.no_grad()
 def similarity_topk(query: torch.Tensor, space: torch.Tensor, k: int, scale: float = 1.0, normalize_query: bool = True,
                     normalize_space: bool = False, device: Union[int, str, torch.device, None] = None):

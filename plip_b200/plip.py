@@ -131,6 +131,38 @@ class PLIP:
         res = encode_region(self.model.engine, region, crop_overlap=crop_overlap, non_bg_threshold=non_bg_threshold)
         return res.embeddings.cpu().numpy(), res.origins, res.tissue_ratio
 
+    def encode_region_pyramid(self, region, mask=None, downsample_list=(2, 4, 8, 16, 32), crop_overlap: float = 0.1,
+                              non_bg_threshold: float = 0.5):
+        """The reference's step 1 for one image (``random_crop`` at every ``downsample``,
+        ``preprocess_DigestPath.py:117-140``), encoded: ``region`` as in :meth:`encode_region`; ``mask`` an L / RGB PIL
+        image or a uint8 ``[H, W]`` / ``[H, W, 3]`` array (any size: it is resized per level with NEAREST, as there).
+        Returns ``(embeddings [k,512] float32 un-normalised, stats)``, levels outer in list order; ``stats`` is a dict of
+        numpy columns ``origin_row``, ``origin_col``, ``tissue_ratio``, ``tumor_to_patch_ratio``,
+        ``tumor_to_tissue_ratio``, ``downsample``, ``cropsize``, ``crop_overlap``, ``non_bg_threshold`` in the
+        reference's row order, so ``pandas.DataFrame(stats)`` has its ``df_stat`` columns
+        (``regions.encode_region_pyramid``)."""
+        from .regions import WINDOW, encode_region_pyramid
+        if isinstance(region, PIL.Image.Image):
+            region = np.asarray(region.convert("RGB"))
+        if isinstance(mask, PIL.Image.Image):
+            if mask.mode not in ("L", "RGB"):
+                raise ValueError(f"a mask image must be mode L or RGB, got {mask.mode}")
+            mask = np.asarray(mask)
+        levels = encode_region_pyramid(self.model.engine, region, mask, downsample_list, crop_overlap,
+                                       non_bg_threshold)
+        emb = np.concatenate([lv.embeddings.cpu().numpy() for lv in levels]).reshape(-1, 512)
+        col = lambda f: np.concatenate([f(lv) for lv in levels])  # noqa: E731
+        n = lambda lv: len(lv.origins)  # noqa: E731
+        stats = {"origin_row": col(lambda lv: lv.origins[:, 0]), "origin_col": col(lambda lv: lv.origins[:, 1]),
+                 "tissue_ratio": col(lambda lv: lv.tissue_ratio),
+                 "tumor_to_patch_ratio": col(lambda lv: lv.tumor_to_patch_ratio),
+                 "tumor_to_tissue_ratio": col(lambda lv: lv.tumor_to_tissue_ratio),
+                 "downsample": col(lambda lv: np.full(n(lv), lv.downsample)),
+                 "cropsize": col(lambda lv: np.full(n(lv), WINDOW)),
+                 "crop_overlap": col(lambda lv: np.full(n(lv), float(crop_overlap))),
+                 "non_bg_threshold": col(lambda lv: np.full(n(lv), float(non_bg_threshold)))}
+        return emb, stats
+
     def _tokenize(self, text: List[str]):
         if self.preprocess is None and self.tokenizer is None:
             raise RuntimeError("no tokenizer available for this checkpoint (no vocab.json + merges.txt next to it, "
