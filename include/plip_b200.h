@@ -32,7 +32,7 @@ extern "C" {
 
 #define PLIP_API __attribute__((visibility("default")))
 
-#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts, plip_window_mask_counts, plip_resize_region_*, plip_resize_filter_bounds (new symbols only) */
+#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts, plip_window_mask_counts, plip_resize_region_*, plip_resize_filter_bounds, plip_sgd_*, plip_linear_decision (new symbols only) */
 
 /* Model constants (TF:configuration_clip.py:47-64,97-109,160-161). */
 #define PLIP_IMAGE_SIZE 224
@@ -274,6 +274,53 @@ PLIP_API int plip_resize_region_u8(const void* src_dev, int64_t src_row_pitch, i
  * kernels compute it: bounds_host int32 [out_size][2] = (first source index, count).  Output index i reads source
  * indices [first, first + count). */
 PLIP_API int plip_resize_filter_bounds(int in_size, int out_size, int32_t* bounds_host);
+
+/* ---- linear probe: scikit-learn's SGD logistic regression (no engine) ------------------------- */
+/* The reference's linear probe (reproducibility/evaluation/linear_probing/linear_classifier.py) fits
+ * SGDClassifier(loss="log_loss", penalty="l2", class_weight="balanced", learning_rate="optimal") on float32 [n,512]
+ * embeddings: one-vs-rest binary problems, each a sequential pass of sklearn 1.9's _plain_sgd (32-bit instantiation)
+ * over a shuffled order per epoch.  plip_sgd_fit runs that algorithm, cast for cast, for many binary problems at once
+ * (every class of a fit, every alpha of a sweep): one warp per problem runs all its epochs on the device.  The
+ * results equal sklearn's up to the order of the 512-term double sums and CUDA's exp / log1p against the C library's.
+ *
+ * One binary problem: labels y = (class_host[i] == pos_class), positive / negative sample weight pos_weight /
+ * neg_weight (rounded to float, as sklearn's class_weight local), regularisation alpha (> 0, finite), t starting at 1,
+ * and the epoch order order_e[i] = order_{e-1}[sigma[i]] (order_0 = identity) with sigma row sigma_index of
+ * sigma_host: the permutation sklearn's dataset.shuffle(seed) applies every epoch (plip_sgd_shuffle_permutation). */
+typedef struct plip_sgd_problem {
+  double alpha;
+  double pos_weight;
+  double neg_weight;
+  int32_t pos_class;
+  int32_t sigma_index;
+} plip_sgd_problem_t;
+/* Host-only: sklearn's Fisher-Yates shuffle (utils/_seq_dataset.pyx.tp, our_rand_r xorshift, j = i + r % (n - i))
+ * applied to the identity: sigma_host int32 [n].  1 <= n < 2^31; seed 0 behaves as our_rand_r's default 1. */
+PLIP_API int plip_sgd_shuffle_permutation(int64_t n, uint32_t seed, int32_t* sigma_host);
+/* Device workspace bytes of plip_sgd_fit (problem table, labels, sigma rows and two epoch orders per problem). */
+PLIP_API int plip_sgd_workspace_bytes(int64_t n, int n_sigma, int n_problems, uint64_t* bytes);
+/* x_dev: device float32 [n,512], rows contiguous, 16-byte aligned; 2 <= n < 2^31.  class_host: HOST int32 [n] class ids
+ * in 0..n_classes-1.  problems_host: HOST [n_problems].  sigma_host: HOST int32 [n_sigma, n], every entry in 0..n-1.
+ * Host arrays are consumed before the call returns.  max_iter >= 1 epochs; an epoch whose mean objective exceeds the
+ * best so far minus tol counts towards n_iter_no_change (>= 1) epochs without improvement, which stop the problem
+ * (tol = -INFINITY disables the test).  Outputs (device): coef_dev float32 [n_problems,512], intercept_dev float64
+ * [n_problems], n_iter_dev int32 [n_problems] (epochs run), overflow_dev int32 [n_problems]: 1 if the weights or the
+ * intercept were not finite at the end of epoch n_iter (sklearn raises there; coef / intercept are then undefined).
+ * workspace_dev: 16-byte aligned device memory of at least plip_sgd_workspace_bytes(n, n_sigma, n_problems); the call
+ * allocates nothing.  Every argument is checked before anything is launched; an error names the offending value.
+ * Stream-ordered, one launch. */
+PLIP_API int plip_sgd_fit(const float* x_dev, int64_t n, int dim, const int32_t* class_host, int n_classes,
+                          const plip_sgd_problem_t* problems_host, int n_problems, const int32_t* sigma_host,
+                          int n_sigma, int max_iter, double tol, int n_iter_no_change, float* coef_dev,
+                          double* intercept_dev, int32_t* n_iter_dev, int32_t* overflow_dev, void* workspace_dev,
+                          uint64_t workspace_bytes, void* stream);
+/* decision_function and predict of a fitted linear classifier: scores_dev float32 [n, n_out] = x . coef^T + intercept
+ * (products and sums in double, rounded once), pred_dev int32 [n]: n_out > 1, the first index of the largest score;
+ * n_out == 1, 1 where the score is > 0, else 0.  x_dev float32 [n,512] and coef_dev float32 [n_out,512] 16-byte
+ * aligned, intercept_dev float64 [n_out].  Stream-ordered, one launch. */
+PLIP_API int plip_linear_decision(const float* x_dev, int64_t n, int dim, const float* coef_dev,
+                                  const double* intercept_dev, int n_out, float* scores_dev, int32_t* pred_dev,
+                                  void* stream);
 
 /* ---- host-buffer convenience (end-to-end path; copies are inside the call) ------------------- */
 /* pixels_host / ids_host / out_host are host pointers (pinned or pageable).  The call stages

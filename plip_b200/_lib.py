@@ -54,6 +54,13 @@ class ResizeDesc(C.Structure):
     ]
 
 
+class SgdProblem(C.Structure):
+    """Mirror of ``plip_sgd_problem_t`` (32 bytes)."""
+
+    _fields_ = [("alpha", C.c_double), ("pos_weight", C.c_double), ("neg_weight", C.c_double), ("pos_class", C.c_int32),
+                ("sigma_index", C.c_int32)]
+
+
 class TowerOutputs(C.Structure):
     """Mirror of ``plip_tower_outputs_t`` (device pointers, 0 = not requested)."""
 
@@ -96,6 +103,11 @@ SIGNATURES = {
     "plip_resize_region_workspace": (_i, [_i, _i, _i, _i, _i, _i, C.POINTER(_u64)]),
     "plip_resize_region_u8": (_i, [_vp, _i64, _i, _i, _i, _i, _vp, _i64, _i, _i, _i, _i, _vp, _u64, _vp]),
     "plip_resize_filter_bounds": (_i, [_i, _i, _vp]),
+    "plip_sgd_shuffle_permutation": (_i, [_i64, C.c_uint32, _vp]),
+    "plip_sgd_workspace_bytes": (_i, [_i64, _i, _i, C.POINTER(_u64)]),
+    "plip_sgd_fit": (_i, [_fp, _i64, _i, _vp, _i, _vp, _i, _vp, _i, _i, C.c_double, _i, _fp, _vp, _vp, _vp, _vp, _u64,
+                          _vp]),
+    "plip_linear_decision": (_i, [_fp, _i64, _i, _fp, _vp, _i, _fp, _vp, _vp]),
     "plip_encode_images_host": (_i, [_vp, _vp, _i, _i64, _fp, _i]),
     "plip_encode_text_host": (_i, [_vp, _vp, _i, _vp, _i64, _i, _fp, _i]),
     "plip_profile_enable": (_i, [_vp, _i]),

@@ -8,6 +8,7 @@ from typing import Dict, Mapping, Optional, Tuple, Union
 import numpy as np
 import torch
 
+from ._lib import SgdProblem as _SgdProblem
 from ._lib import check, lib
 from .weights import operand_format, pack_state_dict
 
@@ -293,6 +294,76 @@ def similarity_topk(query: torch.Tensor, space: torch.Tensor, k: int, scale: flo
                                      int(normalize_space), int(k), idx.data_ptr(), val.data_ptr(),
                                      torch.cuda.current_stream(dev).cuda_stream), "plip_similarity_topk")
     return idx, val
+
+
+def sgd_shuffle_permutation(n: int, seed: int) -> np.ndarray:
+    """The permutation scikit-learn's ``dataset.shuffle(seed)`` applies to the sample order every epoch (its
+    Fisher-Yates with ``our_rand_r``): int32 ``[n]``, ``new_order[i] = old_order[sigma[i]]``.  Host only."""
+    if not 1 <= int(n) < 2 ** 31:
+        raise ValueError(f"n = {n} is outside 1..2^31-1")
+    out = np.empty(int(n), np.int32)
+    check(lib().plip_sgd_shuffle_permutation(int(n), int(seed) & 0xFFFFFFFF, out.ctypes.data),
+          "plip_sgd_shuffle_permutation")
+    return out
+
+
+def _device_embeddings(x: torch.Tensor, what: str) -> Tuple[int, int]:
+    if not (torch.is_tensor(x) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and x.is_contiguous()):
+        raise ValueError(f"{what} must be a contiguous CUDA float32 [n, {EMBED_DIM}] tensor")
+    return int(x.shape[0]), int(x.shape[1])
+
+
+@torch.no_grad()
+def sgd_fit(x: torch.Tensor, class_ids, n_classes: int, problems, sigma, max_iter: int = 10000, tol: float = 1e-3,
+            n_iter_no_change: int = 5):
+    """scikit-learn's SGD logistic regression for many binary problems in one launch (``plip_sgd_fit``; needs no
+    engine).  ``x``: CUDA float32 ``[n, 512]``; ``class_ids``: int ``[n]`` in ``0..n_classes-1``; ``problems``: one
+    ``(alpha, pos_class, pos_weight, neg_weight, sigma_index)`` per problem; ``sigma``: int32 ``[n_sigma, n]`` epoch
+    permutations (``sgd_shuffle_permutation``).  Returns device tensors ``(coef f32 [P, 512], intercept f64 [P],
+    n_iter int32 [P], overflow int32 [P])``; bad arguments raise ``ValueError`` before anything is launched."""
+    n, d = _device_embeddings(x, "x")
+    cls = np.ascontiguousarray(np.asarray(class_ids), dtype=np.int32)
+    sig = np.ascontiguousarray(np.asarray(sigma), dtype=np.int32)
+    if cls.shape != (n,) or sig.ndim != 2 or sig.shape[1] != n:
+        raise ValueError(f"class ids {cls.shape} and sigma {sig.shape} do not match n = {n}")
+    table = (_SgdProblem * len(problems))(*[_SgdProblem(float(a), float(wp), float(wn), int(pc), int(si))
+                                            for a, pc, wp, wn, si in problems])
+    p = len(problems)
+    L = lib()
+    need = C.c_uint64(0)
+    _check_args(L.plip_sgd_workspace_bytes(n, int(sig.shape[0]), p, C.byref(need)), "plip_sgd_workspace_bytes")
+    dev = x.device
+    ws = torch.empty(int(need.value), dtype=torch.uint8, device=dev)
+    coef = torch.empty(p, EMBED_DIM, dtype=torch.float32, device=dev)
+    intercept = torch.empty(p, dtype=torch.float64, device=dev)
+    n_iter = torch.empty(p, dtype=torch.int32, device=dev)
+    overflow = torch.empty(p, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _check_args(L.plip_sgd_fit(x.data_ptr(), n, d, cls.ctypes.data, int(n_classes), table, p, sig.ctypes.data,
+                                   int(sig.shape[0]), int(max_iter), C.c_double(tol), int(n_iter_no_change),
+                                   coef.data_ptr(), intercept.data_ptr(), n_iter.data_ptr(), overflow.data_ptr(),
+                                   ws.data_ptr(), ws.numel(), torch.cuda.current_stream(dev).cuda_stream), "plip_sgd_fit")
+    return coef, intercept, n_iter, overflow
+
+
+@torch.no_grad()
+def linear_decision(x: torch.Tensor, coef: torch.Tensor, intercept: torch.Tensor):
+    """``decision_function`` and the predicted index of a linear classifier (``plip_linear_decision``; needs no engine):
+    ``x`` CUDA float32 ``[n, 512]``, ``coef`` float32 ``[C, 512]``, ``intercept`` ``[C]`` on the same device.  Returns
+    ``(scores f32 [n, C], pred int32 [n])``: the first arg-max for ``C > 1``, ``score > 0`` for ``C == 1``."""
+    n, d = _device_embeddings(x, "x")
+    c, dc = _device_embeddings(coef, "coef")
+    b = intercept.to(device=x.device, dtype=torch.float64).contiguous()
+    if coef.device != x.device or dc != d or b.shape != (c,):
+        raise ValueError(f"coef {tuple(coef.shape)} on {coef.device} and intercept {tuple(intercept.shape)} do not "
+                         f"match x on {x.device}")
+    scores = torch.empty(n, c, dtype=torch.float32, device=x.device)
+    pred = torch.empty(n, dtype=torch.int32, device=x.device)
+    with torch.cuda.device(x.device):
+        _check_args(lib().plip_linear_decision(x.data_ptr(), n, d, coef.data_ptr(), b.data_ptr(), c, scores.data_ptr(),
+                                               pred.data_ptr(), torch.cuda.current_stream(x.device).cuda_stream),
+                    "plip_linear_decision")
+    return scores, pred
 
 
 class Engine:

@@ -6,15 +6,21 @@ device) like the reference; the ``dot`` + ``argmax`` / ``argsort()[-50:][::-1]``
 similarity kernels (fp32).  The sklearn metrics of the reference (``metrics.py``) are CPU statistics outside the
 hot path: pass ``eval_metrics=`` to reuse them; the p@10 / p@50 retrieval metric is restated here because it is a
 pure function of the top-k indices.
+
+``LinearProber`` (``evaluation/linear_probing/linear_classifier.py``) fits the reference's
+``SGDClassifier(loss="log_loss", penalty="l2", max_iter=10000, class_weight="balanced")`` with scikit-learn 1.9's
+algorithm restated on the device (``plip_sgd_fit``): same shuffles, same casts, every one-vs-rest problem at once;
+``linear_probe_sweep`` fits a whole alpha sweep in one launch.
 """
 from __future__ import annotations
 
+import warnings
 from typing import Callable, List, Optional, Sequence
 
 import numpy as np
 import torch
 
-from .engine import Engine, similarity_topk
+from .engine import EMBED_DIM, Engine, linear_decision, sgd_fit, sgd_shuffle_permutation, similarity_topk
 
 
 def _t(x) -> torch.Tensor:
@@ -76,3 +82,158 @@ class ImageRetrieval(_Head):
         test_metrics, train_metrics = retrieval_metrics(targets, best), retrieval_metrics(targets, best)
         test_metrics["split"], train_metrics["split"] = "test", "train"
         return train_metrics, test_metrics
+
+
+# ---- linear probe ------------------------------------------------------------------------------------------------
+
+MAX_INT = np.iinfo(np.int32).max
+
+
+class ConvergenceWarning(UserWarning):
+    """A fit stopped at ``max_iter`` epochs (scikit-learn warns with its own ``ConvergenceWarning`` there)."""
+
+
+def _device(engine: Optional[Engine]) -> torch.device:
+    if engine is not None:
+        return engine.device
+    if not torch.cuda.is_available():
+        raise RuntimeError("plip_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
+    return torch.device("cuda", torch.cuda.current_device())
+
+
+def _embeddings(x, device: torch.device) -> torch.Tensor:
+    """float32 ``[n, 512]`` (numpy or torch, host or device) as a contiguous tensor on ``device``.  Other dtypes raise:
+    scikit-learn runs float64 input through its 64-bit instantiation, which is not restated here."""
+    if not torch.is_tensor(x):
+        x = np.asarray(x)
+        if x.dtype != np.float32:
+            raise ValueError(f"the embeddings must be float32 [n, {EMBED_DIM}], got {x.dtype}")
+        x = torch.from_numpy(np.ascontiguousarray(x))
+    if x.dtype != torch.float32 or x.dim() != 2 or x.shape[1] != EMBED_DIM:
+        raise ValueError(f"the embeddings must be float32 [n, {EMBED_DIM}], got {x.dtype} {tuple(x.shape)}")
+    x = x.to(device).contiguous()
+    if x.shape[0] and not bool(torch.isfinite(x).all()):
+        kind = "NaN" if bool(torch.isnan(x).any()) else "infinity or a value too large for dtype('float32')"
+        raise ValueError(f"Input X contains {kind}.")
+    return x
+
+
+def _problem_seeds(n_classes: int, seed: int) -> List[int]:
+    """The ``seed`` scikit-learn hands to ``_plain_sgd`` per binary problem: ``fit_binary`` draws it after
+    ``make_dataset``'s draw, from ``RandomState(seed)`` for two classes, else from one ``RandomState`` per class
+    seeded by ``RandomState(seed).randint(MAX_INT, size=n_classes)`` (``_fit_multiclass``)."""
+    def draw(rs):
+        rs.randint(1, MAX_INT)
+        return int(rs.randint(MAX_INT))
+    if n_classes == 2:
+        return [draw(np.random.RandomState(seed))]
+    return [draw(np.random.RandomState(s)) for s in np.random.RandomState(seed).randint(MAX_INT, size=n_classes)]
+
+
+class SGDLinearClassifier:
+    """A fitted one-vs-rest logistic regression with ``SGDClassifier``'s attributes: ``classes_``, ``coef_`` float32
+    ``[C, 512]`` (``[1, 512]`` for two classes), ``intercept_`` (float32 ``[C]``, float64 ``[1]`` for two classes, as
+    scikit-learn keeps them), ``n_iter_`` and ``alpha``.  ``decision_function`` / ``predict`` run on the device."""
+
+    def __init__(self, classes, coef, intercept, n_iter: int, alpha: float, device: torch.device):
+        self.classes_, self.coef_, self.intercept_, self.n_iter_, self.alpha = classes, coef, intercept, n_iter, alpha
+        self.device = device
+
+    def _decide(self, X):
+        x = _embeddings(X, self.device)
+        coef = torch.from_numpy(self.coef_).to(self.device)
+        return linear_decision(x, coef, torch.from_numpy(self.intercept_.astype(np.float64)))
+
+    def decision_function(self, X) -> np.ndarray:
+        """``X . coef_.T + intercept_``: float32 ``[n, C]``, or ``[n]`` for two classes."""
+        scores = self._decide(X)[0].cpu().numpy()
+        return scores[:, 0] if scores.shape[1] == 1 else scores
+
+    def predict(self, X) -> np.ndarray:
+        """``classes_`` of the first largest score, or ``classes_[1]`` where the score is ``> 0`` for two classes."""
+        return self.classes_[self._decide(X)[1].cpu().numpy()]
+
+
+def fit_sgd_classifiers(X, y, alphas: Sequence[float], seed: int = 7, max_iter: int = 10000, tol: float = 1e-3,
+                        n_iter_no_change: int = 5, engine: Optional[Engine] = None) -> List[SGDLinearClassifier]:
+    """``SGDClassifier(random_state=seed, loss="log_loss", alpha=a, penalty="l2", max_iter=max_iter, tol=tol,
+    class_weight="balanced").fit(X, y)`` for every ``a`` in ``alphas``, all binary problems in one ``plip_sgd_fit``
+    launch.  ``y``: any labels (``classes_ = np.unique(y)``).  A problem whose weights overflow raises scikit-learn's
+    ``ValueError`` (the first alpha and class in order)."""
+    dev = _device(engine)
+    x = _embeddings(X, dev)
+    classes, y_ind = np.unique(np.asarray(y), return_inverse=True)
+    n, n_classes = int(x.shape[0]), len(classes)
+    if y_ind.shape != (n,):
+        raise ValueError(f"{n} samples but {y_ind.size} labels")
+    if n_classes < 2:
+        raise ValueError(f"The number of classes has to be greater than one; got {n_classes} class")
+    counts = np.bincount(y_ind, minlength=n_classes).astype(np.float64)
+    cw = float(n) / (n_classes * counts)                       # compute_class_weight("balanced")
+    seeds = _problem_seeds(n_classes, seed)
+    per_alpha = [(1, cw[1], cw[0], 0)] if n_classes == 2 else [(i, cw[i], 1.0, i) for i in range(n_classes)]
+    problems = [(float(a), pc, wp, wn, si) for a in alphas for pc, wp, wn, si in per_alpha]
+    sigma = np.stack([sgd_shuffle_permutation(n, s) for s in seeds])
+    coef, intercept, n_iter, overflow = (t.cpu().numpy() for t in sgd_fit(x, y_ind, n_classes, problems, sigma,
+                                                                           max_iter, tol, n_iter_no_change))
+    out, k = [], len(per_alpha)
+    for i, a in enumerate(alphas):
+        rows = slice(i * k, (i + 1) * k)
+        bad = np.flatnonzero(overflow[rows])
+        if bad.size:
+            raise ValueError("Floating-point under-/overflow occurred at epoch #%d. Scaling input data with "
+                             "StandardScaler or MinMaxScaler might help." % int(n_iter[rows][bad[0]]))
+        it = int(n_iter[rows].max())
+        if max_iter > 1 and it == max_iter:
+            warnings.warn("Maximum number of iteration reached before convergence. Consider increasing max_iter to "
+                          "improve the fit.", ConvergenceWarning)
+        b = intercept[rows] if n_classes == 2 else intercept[rows].astype(np.float32)
+        out.append(SGDLinearClassifier(classes, coef[rows].copy(), b.copy(), it, float(a), dev))
+    return out
+
+
+def _encode_labels(train_y, test_y):
+    """``LabelEncoder().fit_transform(train_y)`` / ``.transform(test_y)``: indices into the sorted unique labels."""
+    classes = np.unique(np.asarray(train_y))
+    test = np.asarray(test_y)
+    unseen = np.setdiff1d(np.unique(test), classes)
+    if unseen.size:
+        raise ValueError(f"y contains previously unseen labels: {unseen.tolist()}")
+    return np.searchsorted(classes, np.asarray(train_y)), np.searchsorted(classes, test)
+
+
+def _probe_metrics(clf: SGDLinearClassifier, train_x, train_y, test_x, test_y, eval_metrics):
+    test_pred, train_pred = clf.predict(test_x), clf.predict(train_x)
+    if eval_metrics is None:
+        test_metrics = {"accuracy": float(np.mean(test_pred == test_y))}
+        train_metrics = {"accuracy": float(np.mean(train_pred == train_y))}
+    else:
+        test_metrics = eval_metrics(test_y, test_pred, average_method="macro")
+        train_metrics = eval_metrics(train_y, train_pred, average_method="macro")
+    test_metrics["split"], train_metrics["split"] = "test", "train"
+    return test_metrics, train_metrics
+
+
+def linear_probe_sweep(train_x, train_y, test_x, test_y, alphas: Sequence[float], seed: int = 7,
+                       eval_metrics: Optional[Callable] = None, engine: Optional[Engine] = None):
+    """``LinearProber(alpha, seed).train_and_test(...)`` for every alpha of ``alphas`` (the reference's
+    ``reproduce.sh`` loop), fitted in one launch: one ``(classifier, (test_metrics, train_metrics))`` per alpha, each
+    bit-identical to the single-alpha call."""
+    ytr, yte = _encode_labels(train_y, test_y)
+    dev = _device(engine)
+    xtr, xte = _embeddings(train_x, dev), _embeddings(test_x, dev)
+    clfs = fit_sgd_classifiers(xtr, ytr, alphas, seed=seed, max_iter=10000, engine=engine)
+    return [(clf, _probe_metrics(clf, xtr, ytr, xte, yte, eval_metrics)) for clf in clfs]
+
+
+class LinearProber:
+    """The reference's ``LinearProber`` (``linear_classifier.py``): labels are encoded as ``LabelEncoder`` does, the
+    classifier is fitted on the indices (so its ``classes_`` are ``0..C-1``), and the metrics are accuracy, or
+    ``eval_metrics(y, pred, average_method="macro")`` (the reference's ``metrics.eval_metrics``) when given."""
+
+    def __init__(self, alpha: float, seed: int = 7, engine: Optional[Engine] = None):
+        self.alpha, self.seed, self.engine = alpha, seed, engine
+
+    def train_and_test(self, train_x, train_y, test_x, test_y, eval_metrics: Optional[Callable] = None):
+        return linear_probe_sweep(train_x, train_y, test_x, test_y, [self.alpha], self.seed, eval_metrics,
+                                  self.engine)[0]

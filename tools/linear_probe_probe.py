@@ -1,0 +1,94 @@
+"""The linear probe on one GPU, on a Kather-shaped synthetic problem: 100 k training and 7 k test rows of float32
+[., 512] embeddings, 9 classes, and ``reproduce.sh``'s alphas (1e-4, 1e-3, 1e-2, 1e-1).  Reports the wall time of
+``evaluation.linear_probe_sweep`` (all 4 x 9 binary problems in one launch, ending in a device synchronise), the
+epochs per alpha, and ns per sample step along the longest problem's chain (the kernel is bound by that dependent
+chain, not by a roofline).  When scikit-learn imports, also the host time of the same 4 ``SGDClassifier`` fits and
+whether the predictions agree.  Prints the card name and power limit with the numbers.  GPU only.
+
+    python tools/linear_probe_probe.py [out.json] [--no-sklearn]
+"""
+import json
+import os
+import sys
+import time
+import warnings
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+
+from plip_b200.evaluation import fit_sgd_classifiers, linear_probe_sweep  # noqa: E402
+from region_probe import card  # noqa: E402
+
+N_TRAIN, N_TEST, CLASSES = 100_000, 7_000, 9
+ALPHAS = [1e-4, 1e-3, 1e-2, 1e-1]
+
+
+def kather_like(n, seed):
+    """Unit-norm embeddings around 9 class means with class sizes as uneven as Kather's (about 2:1)."""
+    rs = np.random.RandomState(seed)
+    p = np.linspace(1.0, 2.0, CLASSES)
+    y = rs.choice(CLASSES, size=n, p=p / p.sum())
+    means = np.random.RandomState(0).standard_normal((CLASSES, 512))
+    x = means[y] * 0.05 + rs.standard_normal((n, 512)) * 0.3
+    x /= np.linalg.norm(x, axis=1, keepdims=True)
+    return x.astype(np.float32), y
+
+
+def main():
+    if not torch.cuda.is_available():
+        sys.exit("linear_probe_probe: needs a CUDA device")
+    out_path = next((a for a in sys.argv[1:] if not a.startswith("--")), None)
+    xtr, ytr = kather_like(N_TRAIN, 1)
+    xte, yte = kather_like(N_TEST, 2)
+    res = {"card": card(), "n_train": N_TRAIN, "n_test": N_TEST, "classes": CLASSES, "alphas": ALPHAS}
+
+    fit_sgd_classifiers(xtr[:2000], ytr[:2000], ALPHAS)          # module load, first launches
+    dtr, dte = torch.from_numpy(xtr).cuda(), torch.from_numpy(xte).cuda()
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    sweep = linear_probe_sweep(dtr, ytr, dte, yte, ALPHAS)
+    torch.cuda.synchronize()
+    res["sweep_s"] = time.perf_counter() - t0
+    t0 = time.perf_counter()
+    fit_sgd_classifiers(dtr, ytr, ALPHAS)
+    torch.cuda.synchronize()
+    res["fit_s"] = time.perf_counter() - t0
+    epochs = [clf.n_iter_ for clf, _ in sweep]
+    res["epochs_per_alpha"] = epochs
+    res["ns_per_step_longest_chain"] = res["fit_s"] / (max(epochs) * N_TRAIN) * 1e9
+    res["test_accuracy"] = [m[0]["accuracy"] for _, m in sweep]
+
+    if "--no-sklearn" not in sys.argv:
+        try:
+            from sklearn.linear_model import SGDClassifier
+        except ImportError:
+            res["sklearn"] = "not installed"
+        else:
+            sk_s, agree, sk_epochs, dcoef = 0.0, [], [], []
+            for a, (clf, _) in zip(ALPHAS, sweep):
+                sk = SGDClassifier(random_state=7, loss="log_loss", alpha=a, penalty="l2", max_iter=10000,
+                                   class_weight="balanced")
+                with warnings.catch_warnings():
+                    warnings.simplefilter("ignore")
+                    t0 = time.perf_counter()
+                    sk.fit(xtr, ytr)
+                    sk_s += time.perf_counter() - t0
+                sk_epochs.append(int(sk.n_iter_))
+                agree.append(float(np.mean(sk.predict(xte) == clf.predict(dte))))
+                dcoef.append(float(np.abs(sk.coef_ - clf.coef_).max() / np.abs(sk.coef_).max()))
+            res["sklearn_fit_s"] = sk_s
+            res["sklearn_epochs_per_alpha"] = sk_epochs
+            res["prediction_agreement"] = agree
+            res["max_abs_dcoef_over_max_coef"] = dcoef
+    print(json.dumps(res, indent=1))
+    if out_path:
+        with open(out_path, "w") as f:
+            json.dump(res, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
