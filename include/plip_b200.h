@@ -32,7 +32,7 @@ extern "C" {
 
 #define PLIP_API __attribute__((visibility("default")))
 
-#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts, plip_window_mask_counts, plip_resize_region_*, plip_resize_filter_bounds, plip_sgd_*, plip_linear_decision (new symbols only) */
+#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts, plip_window_mask_counts, plip_resize_region_*, plip_resize_filter_bounds, plip_sgd_*, plip_linear_decision, plip_densenet_*, plip_resize_crop_bilinear_u8 (new symbols only) */
 
 /* Model constants (TF:configuration_clip.py:47-64,97-109,160-161). */
 #define PLIP_IMAGE_SIZE 224
@@ -250,6 +250,12 @@ typedef struct plip_resize_desc {
 } plip_resize_desc_t;
 PLIP_API int plip_resize_crop_u8(const void* src_dev, uint64_t src_bytes, const plip_resize_desc_t* descs_host,
                                  int64_t n, void* tiles_dev, void* stream);
+/* Same with Pillow's bilinear filter (triangle, support 1; the same ImagingResample): bit-identical to
+ * PIL.Image.resize((new_width,new_height), BILINEAR).crop(...), i.e. torchvision's Resize(224) (BILINEAR, its default)
+ * + CenterCrop(224) on a PIL image, the MuDiPath transform (reproducibility/embedders/factory.py:41-46) before ToTensor.
+ * Accepts exactly the descriptors plip_resize_crop_u8 accepts. */
+PLIP_API int plip_resize_crop_bilinear_u8(const void* src_dev, uint64_t src_bytes, const plip_resize_desc_t* descs_host,
+                                          int64_t n, void* tiles_dev, void* stream);
 
 /* Whole-image resize on the device, bit-identical to PIL.Image.fromarray(src).resize((new_width, new_height)) (BICUBIC,
  * no reducing_gap) for any ratio from upscaling to shrinks of over 64x (the horizontal filter must fit 64 columns in
@@ -322,6 +328,31 @@ PLIP_API int plip_linear_decision(const float* x_dev, int64_t n, int dim, const 
                                   const double* intercept_dev, int n_out, float* scores_dev, int32_t* pred_dev,
                                   void* stream);
 
+/* ---- MuDiPath DenseNet-121 image embedder (separate handle) ----------------------------------- */
+/* The reference's third embedder (reproducibility/embedders/factory.py:34-47, mudipath.py:125-130,205-215): torchvision's
+ * DenseNet-121 features (growth 32, bottleneck 128, blocks 6/12/24/16) in eval mode, then a global average pool; no
+ * final ReLU, no classifier.  Output: the un-normalised pooled features, float32 [n,1024].
+ * Weights: ONE host blob whose layout the library defines (plip_densenet_tensor_info, same struct as the CLIP blob,
+ * fused always 0): "<torchvision name>.weight" entries are bfloat16 (dtype 1), conv0 [64,160] with K = (ky,kx,c) and
+ * columns 147..159 zero, conv1 [128,C_in], conv2 [32,1152] with K = (ky,kx,c), transition conv [C/2,C];
+ * "<bn name>.scale" / ".shift" are float32 [C]: the eval BatchNorm as y = x * scale + shift
+ * (scale = gamma / sqrt(running_var + 1e-5), shift = beta - running_mean * scale).
+ * Device memory: blob + plip_densenet_workspace_bytes(max_micro_batch) (about 5.3 MB per image). */
+typedef struct plip_densenet plip_densenet_t;
+PLIP_API int plip_densenet_num_tensors(void);
+PLIP_API int plip_densenet_tensor_info(int index, plip_tensor_info_t* info);
+PLIP_API uint64_t plip_densenet_blob_bytes(void);
+PLIP_API uint64_t plip_densenet_workspace_bytes(int max_micro_batch);
+/* 1 <= max_micro_batch <= 4096; device must be an sm_90 GPU. */
+PLIP_API int plip_densenet_create(const void* host_blob, uint64_t blob_bytes, int device, int max_micro_batch,
+                                  plip_densenet_t** out);
+PLIP_API int plip_densenet_destroy(plip_densenet_t* e);
+PLIP_API int plip_densenet_max_micro_batch(const plip_densenet_t* e);
+/* tiles_dev: uint8 RGB [n,224,224,3] (what Resize(224) + CenterCrop(224) produce before ToTensor; ToTensor + the
+ * ImageNet Normalize are fused into the first convolution); out_dev float32 [n,1024].  Micro-batches of at most
+ * max_micro_batch images, 122 launches each, on `stream`; calls on one handle are serialised on the device. */
+PLIP_API int plip_densenet_encode(plip_densenet_t* e, const void* tiles_dev, int64_t n, float* out_dev, void* stream);
+
 /* ---- host-buffer convenience (end-to-end path; copies are inside the call) ------------------- */
 /* pixels_host / ids_host / out_host are host pointers (pinned or pageable).  The call stages
  * micro-batches through pinned buffers on two streams (H2D overlapped with compute), writes the
@@ -368,6 +399,9 @@ PLIP_API int plip_dbg_gemm(const void* A_bf16, int lda, const void* W_bf16, int 
  * kernel runs).  Returns the filter bank width ksize (or -ksize if k_cap is too small). */
 PLIP_API int plip_dbg_resize_filter(int in_size, int out_size, int xx, int32_t* k_host, int k_cap, int* xmin,
                                     int* count);
+/* The same for plip_resize_crop_bilinear_u8's triangle filter. */
+PLIP_API int plip_dbg_resize_filter_bilinear(int in_size, int out_size, int xx, int32_t* k_host, int k_cap, int* xmin,
+                                             int* count);
 /* Host-only: the length-bucket plan plip_encode_text_host uses (lens = first-eos position + 1 per caption).
  * perm_host[i] = original index of the caption at sorted position i (may be NULL); bucket k covers sorted positions
  * [bucket_start[k], bucket_start[k+1]) and is processed with prefix bucket_prefix[k].  Arrays hold cap+1 / cap
@@ -385,6 +419,16 @@ PLIP_API int plip_dbg_attention(const void* qkv_bf16, int64_t n_seq, int seq_len
  * causal / key_mask, 1 <= seq_len <= 1025. */
 PLIP_API int plip_dbg_attention_probs(const void* qkv_bf16, int64_t n_seq, int seq_len, int heads, int causal,
                                       const int32_t* key_mask, float* probs_dev, void* stream);
+/* One DenseNet kernel on caller buffers (bf16 activations NHWC, pixel stride lda / ldo elements, 16-byte aligned):
+ * op 0 stem conv0 + norm0 + ReLU (in: uint8 tiles [n,224,224,3]; out [n*112*112, ldo]); 1 3x3/s2/p1 max pool
+ * (in [n,112,112,64]; out channels [0,64) of [n*56*56, ldo]); 2 conv1: relu(x*a_scale+a_shift) of the first c_in
+ * channels . W^T, then relu(*e_scale+e_shift) (out [n*side^2, ldo], 128 channels); 3 conv2: 3x3/p1 over a dense
+ * [n,side,side,128] (out 32 channels); 4 transition: 2x2 average pool of relu(x*a_scale+a_shift) over
+ * [n,2*side,2*side,lda], then . W^T (out c_in/2 channels); 5 tail: fp32 out [n,1024] = mean over 49 positions of
+ * in [n,49,1024], *e_scale+e_shift. */
+PLIP_API int plip_dbg_densenet_op(int op, const void* in_dev, int lda, int64_t n, int side, int c_in, const void* w_dev,
+                                  const float* a_scale, const float* a_shift, const float* e_scale,
+                                  const float* e_shift, void* out_dev, int ldo, void* stream);
 PLIP_API int plip_dbg_im2col(const void* pixels, int pixel_format, int64_t n, void* out_bf16, void* stream);
 /* The vision position table pos_dev (float32 [50,768]) resized to a grid_h x grid_w patch grid as
  * plip_encode_images_hw does it: out_dev float32 [1 + grid_h * grid_w, 768]; 1 <= grid_h, grid_w <= 32. */

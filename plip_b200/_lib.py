@@ -100,6 +100,7 @@ SIGNATURES = {
     "plip_l2_normalize": (_i, [_fp, _i64, _i, _vp]),
     "plip_window_mask_counts": (_i, [_vp, _i, _i, _i, _i64, _vp, _i64, _i, _vp, _vp]),
     "plip_resize_crop_u8": (_i, [_vp, _u64, _vp, _i64, _vp, _vp]),
+    "plip_resize_crop_bilinear_u8": (_i, [_vp, _u64, _vp, _i64, _vp, _vp]),
     "plip_resize_region_workspace": (_i, [_i, _i, _i, _i, _i, _i, C.POINTER(_u64)]),
     "plip_resize_region_u8": (_i, [_vp, _i64, _i, _i, _i, _i, _vp, _i64, _i, _i, _i, _i, _vp, _u64, _vp]),
     "plip_resize_filter_bounds": (_i, [_i, _i, _vp]),
@@ -108,17 +109,27 @@ SIGNATURES = {
     "plip_sgd_fit": (_i, [_fp, _i64, _i, _vp, _i, _vp, _i, _vp, _i, _i, C.c_double, _i, _fp, _vp, _vp, _vp, _vp, _u64,
                           _vp]),
     "plip_linear_decision": (_i, [_fp, _i64, _i, _fp, _vp, _i, _fp, _vp, _vp]),
+    "plip_densenet_num_tensors": (_i, []),
+    "plip_densenet_tensor_info": (_i, [_i, C.POINTER(TensorInfo)]),
+    "plip_densenet_blob_bytes": (_u64, []),
+    "plip_densenet_workspace_bytes": (_u64, [_i]),
+    "plip_densenet_create": (_i, [_vp, _u64, _i, _i, C.POINTER(_vp)]),
+    "plip_densenet_destroy": (_i, [_vp]),
+    "plip_densenet_max_micro_batch": (_i, [_vp]),
+    "plip_densenet_encode": (_i, [_vp, _vp, _i64, _fp, _vp]),
     "plip_encode_images_host": (_i, [_vp, _vp, _i, _i64, _fp, _i]),
     "plip_encode_text_host": (_i, [_vp, _vp, _i, _vp, _i64, _i, _fp, _i]),
     "plip_profile_enable": (_i, [_vp, _i]),
     "plip_profile_read": (_i, [_vp, C.POINTER(KernelTime), _i, C.POINTER(_i)]),
     "plip_dbg_gemm": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _fp, _vp, _i, _fp, _i, _i, _i, _fp, _fp, _i, _vp, _fp, _vp]),
     "plip_dbg_resize_filter": (_i, [_i, _i, _i, _vp, _i, C.POINTER(_i), C.POINTER(_i)]),
+    "plip_dbg_resize_filter_bilinear": (_i, [_i, _i, _i, _vp, _i, C.POINTER(_i), C.POINTER(_i)]),
     "plip_dbg_text_bucket_plan": (_i, [_vp, _i64, _i, _vp, _vp, _vp, _i]),
     "plip_dbg_rowstats_cast": (_i, [_fp, _i64, _i, _vp, _fp, _vp]),
     "plip_dbg_layernorm": (_i, [_fp, _i64, _i, _i64, _fp, _fp, _fp, _vp, _vp]),
     "plip_dbg_attention": (_i, [_vp, _i64, _i, _i, _i, _vp, _vp, _vp]),
     "plip_dbg_attention_probs": (_i, [_vp, _i64, _i, _i, _i, _vp, _fp, _vp]),
+    "plip_dbg_densenet_op": (_i, [_i, _vp, _i, _i64, _i, _i, _vp, _fp, _fp, _fp, _fp, _vp, _i, _vp]),
     "plip_dbg_im2col": (_i, [_vp, _i, _i64, _vp, _vp]),
     "plip_dbg_hidden_states": (_i, [_vp, _i, _vp, _i, _vp, _i64, _i, _fp, _vp]),
     "plip_dbg_pos_interp": (_i, [_fp, _i, _i, _fp, _vp]),

@@ -1176,6 +1176,14 @@ PLIP_API int plip_resize_crop_u8(const void* src_dev, uint64_t src_bytes, const 
                             static_cast<uint8_t*>(tiles_dev), static_cast<cudaStream_t>(stream));
 }
 
+PLIP_API int plip_resize_crop_bilinear_u8(const void* src_dev, uint64_t src_bytes, const plip_resize_desc_t* descs_host,
+                                          int64_t n, void* tiles_dev, void* stream) {
+  PLIP_REQUIRE(src_dev && descs_host && tiles_dev, "plip_resize_crop_bilinear_u8: null argument");
+  PLIP_REQUIRE(n > 0, "plip_resize_crop_bilinear_u8: n must be positive (got %lld)", (long long)n);
+  return launch_resize_crop(static_cast<const uint8_t*>(src_dev), (size_t)src_bytes, descs_host, n,
+                            static_cast<uint8_t*>(tiles_dev), static_cast<cudaStream_t>(stream), true);
+}
+
 PLIP_API int plip_resize_region_workspace(int height, int width, int new_height, int new_width, int out_row0,
                                           int out_row1, uint64_t* bytes) {
   PLIP_REQUIRE(bytes, "plip_resize_region_workspace: null argument");
@@ -1229,6 +1237,13 @@ PLIP_API int plip_dbg_resize_filter(int in_size, int out_size, int xx, int32_t* 
   PLIP_REQUIRE(k_host && xmin && count && in_size > 0 && out_size > 0 && xx >= 0 && xx < out_size,
                "plip_dbg_resize_filter: bad argument");
   return resize_filter_host(in_size, out_size, xx, k_host, k_cap, xmin, count);
+}
+
+PLIP_API int plip_dbg_resize_filter_bilinear(int in_size, int out_size, int xx, int32_t* k_host, int k_cap, int* xmin,
+                                             int* count) {
+  PLIP_REQUIRE(k_host && xmin && count && in_size > 0 && out_size > 0 && xx >= 0 && xx < out_size,
+               "plip_dbg_resize_filter_bilinear: bad argument");
+  return resize_filter_bilinear_host(in_size, out_size, xx, k_host, k_cap, xmin, count);
 }
 
 // ---- host-buffer path ---------------------------------------------------------------------------

@@ -45,10 +45,12 @@ int launch_gather_rows(const __nv_bfloat16* a16, const float* x32, const int32_t
                        int64_t n, int dim, __nv_bfloat16* a16_out, float* x32_out, cudaStream_t st);
 
 // resize.cu: Pillow-exact bicubic resize + crop of packed RGB uint8 images into [n,224,224,3] tiles.
+// bilinear: Pillow's triangle filter instead of its bicubic one (plip_resize_crop_bilinear_u8).
 int launch_resize_crop(const uint8_t* src, size_t src_bytes, const plip_resize_desc_t* descs_host, int64_t n,
-                       uint8_t* tiles, cudaStream_t st);
+                       uint8_t* tiles, cudaStream_t st, bool bilinear = false);
 
 int resize_filter_host(int in_size, int out_size, int xx, int32_t* k, int k_cap, int* xmin, int* count);
+int resize_filter_bilinear_host(int in_size, int out_size, int xx, int32_t* k, int k_cap, int* xmin, int* count);
 // The same resample over whole images at any shrink: output rows [o0, o1) of the new_h x new_w resize of an h x w RGB
 // uint8 image, from the band of src_rows source rows starting at source row src_row0 (src points at that row).  out
 // points at output row o0.  ws: a 16-byte aligned device workspace of resize_region_workspace bytes.  Every argument

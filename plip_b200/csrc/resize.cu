@@ -67,17 +67,21 @@ struct AxisFilter {
 #define RN_DIV(a, b) ((a) / (b))
 #endif
 
+// BILINEAR selects Pillow's triangle filter (support 1) instead of its bicubic one (support 2): the same
+// ImagingResample, used by torchvision's Resize(BILINEAR) on PIL images.
+template <bool BILINEAR = false>
 __host__ __device__ inline int axis_ksize(int in_size, int out_size) {
   double fs = (double)in_size / (double)out_size;
   if (fs < 1.0) fs = 1.0;
-  return (int)ceil(2.0 * fs) * 2 + 1;
+  return (int)ceil((BILINEAR ? 1.0 : 2.0) * fs) * 2 + 1;
 }
 
+template <bool BILINEAR = false>
 __host__ __device__ __forceinline__ AxisFilter make_axis(int in_size, int out_size) {
   AxisFilter f;
   f.scale = RN_DIV((double)in_size, (double)out_size);
   const double fs = f.scale < 1.0 ? 1.0 : f.scale;
-  f.support = RN_MUL(2.0, fs);
+  f.support = RN_MUL(BILINEAR ? 1.0 : 2.0, fs);
   f.ksize = (int)ceil(f.support) * 2 + 1;
   f.ss = RN_DIV(1.0, fs);
   return f;
@@ -91,7 +95,19 @@ __host__ __device__ __forceinline__ double bicubic_rn(double x) {
   return 0.0;
 }
 
+__host__ __device__ __forceinline__ double triangle_rn(double x) {
+  if (x < 0.0) x = -x;
+  if (x < 1.0) return RN_SUB(1.0, x);
+  return 0.0;
+}
+
+template <bool BILINEAR>
+__host__ __device__ __forceinline__ double filter_rn(double x) {
+  return BILINEAR ? triangle_rn(x) : bicubic_rn(x);
+}
+
 // Filter row of output index `xx`: window [xmin, xmin+count) and fixed-point weights k[0..count).
+template <bool BILINEAR = false>
 __host__ __device__ __forceinline__ void filter_row(const AxisFilter& f, int in_size, int xx, int* k,
                                                     int& xmin_out, int& count_out) {
   const double center = RN_MUL((double)xx + 0.5, f.scale);
@@ -102,10 +118,10 @@ __host__ __device__ __forceinline__ void filter_row(const AxisFilter& f, int in_
   const int count = xmax - xmin;
   double ww = 0.0;
   for (int x = 0; x < count; ++x)
-    ww = RN_ADD(ww, bicubic_rn(RN_MUL(RN_ADD(RN_SUB((double)(x + xmin), center), 0.5), f.ss)));
+    ww = RN_ADD(ww, filter_rn<BILINEAR>(RN_MUL(RN_ADD(RN_SUB((double)(x + xmin), center), 0.5), f.ss)));
   const double one = (double)(1 << kPrecisionBits);
   for (int x = 0; x < count; ++x) {
-    double w = bicubic_rn(RN_MUL(RN_ADD(RN_SUB((double)(x + xmin), center), 0.5), f.ss));
+    double w = filter_rn<BILINEAR>(RN_MUL(RN_ADD(RN_SUB((double)(x + xmin), center), 0.5), f.ss));
     if (ww != 0.0) w = RN_DIV(w, ww);
     k[x] = w < 0.0 ? (int)RN_ADD(-0.5, RN_MUL(w, one)) : (int)RN_ADD(0.5, RN_MUL(w, one));
   }
@@ -171,13 +187,14 @@ __device__ __forceinline__ void hpass_pixel8(const uint8_t* p, const int4 k0, co
   hgroup<GUARD>(wp, prev, mis * 8, k1, end_w, end_b, a0, a1, a2);
 }
 
-__global__ void __launch_bounds__(kRsThreads) resize_crop_kernel(const uint8_t* __restrict__ src, uint64_t src_bytes,
-                                                                 uint8_t* __restrict__ tiles, const ResizeBatch batch,
-                                                                 int64_t first_image) {
+template <bool BILINEAR>
+__device__ __forceinline__ void resize_crop_body(const uint8_t* __restrict__ src, uint64_t src_bytes,
+                                                 uint8_t* __restrict__ tiles, const ResizeBatch& batch,
+                                                 int64_t first_image) {
   extern __shared__ __align__(16) uint8_t rs_smem[];
   const ResizeImg& im = batch.img[blockIdx.y];
   const int row0 = blockIdx.x * kRsRowsPerCta;  // first output row of this CTA
-  const AxisFilter fh = make_axis(im.w, im.new_w), fv = make_axis(im.h, im.new_h);
+  const AxisFilter fh = make_axis<BILINEAR>(im.w, im.new_w), fv = make_axis<BILINEAR>(im.h, im.new_h);
   const int ksh4 = (fh.ksize + 3) & ~3, ksv4 = (fv.ksize + 3) & ~3;  // filter rows zero-padded to 4 taps
 
   int* kh = reinterpret_cast<int*>(rs_smem);                 // [224][ksh4]
@@ -193,9 +210,9 @@ __global__ void __launch_bounds__(kRsThreads) resize_crop_kernel(const uint8_t* 
     int* k = horiz ? kh + j * ksh4 : kv + j * ksv4;
     int lo, cnt;
     if (horiz)
-      filter_row(fh, im.w, im.left + j, k, lo, cnt);
+      filter_row<BILINEAR>(fh, im.w, im.left + j, k, lo, cnt);
     else
-      filter_row(fv, im.h, im.top + row0 + j, k, lo, cnt);
+      filter_row<BILINEAR>(fv, im.h, im.top + row0 + j, k, lo, cnt);
     for (int x = cnt; x < (horiz ? ksh4 : ksv4); ++x) k[x] = 0;
     int* bnd = horiz ? bh + 2 * j : bv + 2 * j;
     bnd[0] = lo;
@@ -273,6 +290,21 @@ __global__ void __launch_bounds__(kRsThreads) resize_crop_kernel(const uint8_t* 
   }
 }
 
+__global__ void __launch_bounds__(kRsThreads) resize_crop_kernel(const uint8_t* __restrict__ src, uint64_t src_bytes,
+                                                                 uint8_t* __restrict__ tiles, const ResizeBatch batch,
+                                                                 int64_t first_image) {
+  resize_crop_body<false>(src, src_bytes, tiles, batch, first_image);
+}
+
+// The same with Pillow's bilinear (triangle) filter: torchvision's Resize(n, BILINEAR) + CenterCrop on PIL images.
+__global__ void __launch_bounds__(kRsThreads) resize_crop_bilinear_kernel(const uint8_t* __restrict__ src,
+                                                                          uint64_t src_bytes,
+                                                                          uint8_t* __restrict__ tiles,
+                                                                          const ResizeBatch batch,
+                                                                          int64_t first_image) {
+  resize_crop_body<true>(src, src_bytes, tiles, batch, first_image);
+}
+
 constexpr size_t kRsSmemHard = 200 * 1024;
 
 size_t table_bytes(int ksh, int ksv) {
@@ -299,18 +331,28 @@ int resize_filter_host(int in_size, int out_size, int xx, int32_t* k, int k_cap,
   return f.ksize;
 }
 
+int resize_filter_bilinear_host(int in_size, int out_size, int xx, int32_t* k, int k_cap, int* xmin, int* count) {
+  const AxisFilter f = make_axis<true>(in_size, out_size);
+  if (k_cap < f.ksize) return -f.ksize;
+  filter_row<true>(f, in_size, xx, k, *xmin, *count);
+  return f.ksize;
+}
+
 // Validates descriptor `idx` and fills the kernel-side plan (strip height, shared memory need).
-static int plan_image(const plip_resize_desc_t& s, long long idx, size_t src_bytes, ResizeImg& o, size_t& need_out) {
+// Tables and strips are sized for the bicubic filter; the bilinear one's windows lie inside the bicubic ones, so the
+// same plan also holds it (with some shared memory to spare).  `fn` names the entry point in errors.
+static int plan_image(const char* fn, const plip_resize_desc_t& s, long long idx, size_t src_bytes, ResizeImg& o,
+                      size_t& need_out) {
   PLIP_REQUIRE(s.width > 0 && s.height > 0 && s.width <= 65536 && s.height <= 65536,
-               "plip_resize_crop_u8: image %lld has invalid size %dx%d", idx, s.width, s.height);
+               "%s: image %lld has invalid size %dx%d", fn, idx, s.width, s.height);
   PLIP_REQUIRE(s.offset >= 0 && (uint64_t)s.offset + (uint64_t)s.width * s.height * 3 <= src_bytes,
-               "plip_resize_crop_u8: image %lld (%dx%d at byte %lld) exceeds the %llu-byte source buffer", idx,
+               "%s: image %lld (%dx%d at byte %lld) exceeds the %llu-byte source buffer", fn, idx,
                s.width, s.height, (long long)s.offset, (unsigned long long)src_bytes);
   PLIP_REQUIRE(s.new_width >= kImage && s.new_height >= kImage && s.new_width <= 65536 && s.new_height <= 65536,
-               "plip_resize_crop_u8: image %lld: resized size %dx%d is smaller than the %dx%d tile", idx,
+               "%s: image %lld: resized size %dx%d is smaller than the %dx%d tile", fn, idx,
                s.new_width, s.new_height, kImage, kImage);
   PLIP_REQUIRE(s.left >= 0 && s.top >= 0 && s.left + kImage <= s.new_width && s.top + kImage <= s.new_height,
-               "plip_resize_crop_u8: image %lld: crop origin (%d,%d) leaves the %dx%d resized image", idx, s.left,
+               "%s: image %lld: crop origin (%d,%d) leaves the %dx%d resized image", fn, idx, s.left,
                s.top, s.new_width, s.new_height);
   const int ksh = axis_ksize(s.width, s.new_width), ksv = axis_ksize(s.height, s.new_height);
   const size_t tb = table_bytes(ksh, ksv);
@@ -331,9 +373,9 @@ static int plan_image(const plip_resize_desc_t& s, long long idx, size_t src_byt
     const double score = kThroughput[resident] / reread;
     if (score > best) best = score, rp = cand, rows = r;
   }
-  PLIP_REQUIRE(rp, "plip_resize_crop_u8: image %lld (%dx%d -> %dx%d) shrinks too much for the on-device "
+  PLIP_REQUIRE(rp, "%s: image %lld (%dx%d -> %dx%d) shrinks too much for the on-device "
                "resize (filter tables need %zu bytes of shared memory); reduce it on the host first",
-               idx, s.width, s.height, s.new_width, s.new_height, tb);
+               fn, idx, s.width, s.height, s.new_width, s.new_height, tb);
   o.src_off = s.offset;
   o.w = s.width, o.h = s.height, o.new_w = s.new_width, o.new_h = s.new_height;
   o.left = s.left, o.top = s.top, o.rows_per_pass = rp, o.strip_rows = rows;
@@ -342,30 +384,31 @@ static int plan_image(const plip_resize_desc_t& s, long long idx, size_t src_byt
 }
 
 int launch_resize_crop(const uint8_t* src, size_t src_bytes, const plip_resize_desc_t* d, int64_t n, uint8_t* tiles,
-                       cudaStream_t st) {
+                       cudaStream_t st, bool bilinear) {
+  const char* fn = bilinear ? "plip_resize_crop_bilinear_u8" : "plip_resize_crop_u8";
   PLIP_REQUIRE(reinterpret_cast<uintptr_t>(src) % 4 == 0 && reinterpret_cast<uintptr_t>(tiles) % 4 == 0,
-               "plip_resize_crop_u8: src_dev and tiles_dev must be 4-byte aligned");
+               "%s: src_dev and tiles_dev must be 4-byte aligned", fn);
   // every descriptor is checked before anything is launched: a bad one leaves the output untouched
   {
     ResizeImg scratch;
     size_t need;
     for (int64_t i = 0; i < n; ++i)
-      if (int rc = plan_image(d[i], (long long)i, src_bytes, scratch, need)) return rc;
+      if (int rc = plan_image(fn, d[i], (long long)i, src_bytes, scratch, need)) return rc;
   }
-  static unsigned long long configured = 0;
-  if (first_use_on_device(configured))
-    PLIP_CUDA_CHECK(cudaFuncSetAttribute(resize_crop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)kRsSmemHard));
+  auto kernel = bilinear ? resize_crop_bilinear_kernel : resize_crop_kernel;
+  static unsigned long long configured[2] = {0, 0};
+  if (first_use_on_device(configured[bilinear]))
+    PLIP_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRsSmemHard));
   for (int64_t base = 0; base < n; base += kRsBatch) {
     const int cnt = (int)((n - base) < kRsBatch ? (n - base) : kRsBatch);
     static thread_local ResizeBatch b;  // 20 KB: kept off the stack
     size_t smem = 0;
     for (int i = 0; i < cnt; ++i) {
       size_t need = 0;
-      if (int rc = plan_image(d[base + i], (long long)(base + i), src_bytes, b.img[i], need)) return rc;
+      if (int rc = plan_image(fn, d[base + i], (long long)(base + i), src_bytes, b.img[i], need)) return rc;
       smem = need > smem ? need : smem;
     }
-    PLIP_CUDA_CHECK(launch_kernel(resize_crop_kernel, dim3(kImage / kRsRowsPerCta, cnt), dim3(kRsThreads), smem, st, 1,
+    PLIP_CUDA_CHECK(launch_kernel(kernel, dim3(kImage / kRsRowsPerCta, cnt), dim3(kRsThreads), smem, st, 1,
                                src, (uint64_t)src_bytes, tiles, b, base));
   }
   return 0;

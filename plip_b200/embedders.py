@@ -20,6 +20,7 @@ import torch
 from .modeling import PlipCLIPModel
 from .tokenizer import find_tokenizer
 from .preprocess import decode_native_then_rgb, SIZE, chunks, decode_rgb, device_resizable, pack_rgb, to_uint8_tiles
+from .preprocess import to_uint8_tiles_bilinear
 
 
 class AbstractEmbedder(ABC):
@@ -106,13 +107,83 @@ class CLIPEmbedder(AbstractEmbedder):
         return torch.cat(outs, dim=0).numpy()
 
 
+class DenseNetEmbedder:
+    """``reproducibility/embedders/mudipath.py:187-215``: the MuDiPath DenseNet-121 baseline.  ``model`` is a
+    :class:`plip_b200.densenet.DenseNetEngine`.  ``embed_images`` returns the **un-normalised** pooled features as
+    float32 numpy ``[N,1024]``.
+
+    Deliberate differences from the reference: the result is always ``[N,1024]`` (the reference's ``.squeeze()``
+    turns a final batch of one image into ``[1024]`` and its ``np.concatenate`` then raises); there is no
+    ``text_embedder``, as in the reference; the ``.npy`` cache is out of scope, as for :class:`CLIPEmbedder`."""
+
+    def __init__(self, model, preprocess, name, backbone):
+        self.model = model
+        self.preprocess = preprocess  # kept for API parity; tiles are prepared by plip_b200.preprocess
+        self.name = name
+        self.backbone = backbone
+
+    def image_embedder(self, list_of_images, device="cuda", num_workers=1, batch_size=32, additional_cache_name=""):
+        return self.embed_images(list_of_images, device=device, num_workers=num_workers, batch_size=batch_size)
+
+    def embed_images(self, list_of_images: Sequence, device="cuda", num_workers=1, batch_size=32) -> np.ndarray:
+        """Paths / PIL images / RGB arrays -> ``[N,1024]`` float32.  Images are converted to RGB first, as the
+        reference's ``CLIPImageDataset`` does, then routed as ``CLIPEmbedder.embed_images`` routes them: a chunk of
+        224 x 224 images goes straight to the engine, a chunk the device resize takes gets ``Resize(224)`` (bilinear) +
+        ``CenterCrop(224)`` on the device (``plip_resize_crop_bilinear_u8``), and a chunk with an image too large
+        for it is resized with PIL on host threads.  Both resize routes give the same tiles, bit for bit."""
+        images = list(list_of_images)
+        eng = self.model
+        outs = [np.empty((0, 1024), dtype=np.float32)]
+        for chunk in chunks(images, max(int(batch_size), eng.max_micro_batch)):
+            arrays = decode_rgb(chunk, int(num_workers))
+            if all(a.shape == (SIZE, SIZE, 3) for a in arrays):
+                outs.append(eng.encode_images_host(np.stack(arrays, axis=0)))
+            elif not all(device_resizable(a.shape[1], a.shape[0]) for a in arrays):   # too large: PIL
+                outs.append(eng.encode_images_host(to_uint8_tiles_bilinear(arrays, int(num_workers))))
+            else:
+                buf, descs = pack_rgb(arrays, crop="round", pinned=True)
+                tiles = eng.resize_crop(buf.to(eng.device, non_blocking=True), descs)
+                outs.append(eng.encode_images(tiles).cpu().numpy())
+        return np.concatenate(outs, axis=0)
+
+
+def mudipath_checkpoint() -> str:
+    """Path of ``densenet121-mh-best-191205-141200.pth``.  ``$PLIP_B200_MTDP``, when set, is the only place looked at
+    (the file, or a directory holding it): a value that resolves to nothing raises instead of falling through to
+    another checkpoint.  Otherwise the directory the reference's ``load_dox_url`` downloads to: ``$TORCH_MODEL_ZOO``,
+    else ``$TORCH_HOME/models`` (``~/.torch/models``).  Nothing is downloaded."""
+    from .densenet import CHECKPOINT_NAME
+    env = os.environ.get("PLIP_B200_MTDP")
+    if env:
+        path = os.path.join(env, CHECKPOINT_NAME) if os.path.isdir(env) else env
+        if not os.path.isfile(path):
+            raise FileNotFoundError(f"$PLIP_B200_MTDP={env!r} names no file (looked at {path}); point it at "
+                                    f"{CHECKPOINT_NAME} or at a directory holding it")
+        return path
+    torch_home = os.path.expanduser(os.environ.get("TORCH_HOME", "~/.torch"))
+    path = os.path.join(os.environ.get("TORCH_MODEL_ZOO", os.path.join(torch_home, "models")), CHECKPOINT_NAME)
+    if os.path.isfile(path):
+        return path
+    raise FileNotFoundError(
+        f"embedder 'mudipath' needs the MuDiPath DenseNet-121 checkpoint {CHECKPOINT_NAME} (the reference downloads "
+        "it from dox.uliege.be; plip_b200 never downloads): point $PLIP_B200_MTDP at the file, or put it into "
+        f"$TORCH_MODEL_ZOO (default $TORCH_HOME/models, ~/.torch/models).  Looked at: {path}")
+
+
 class EmbedderFactory:
-    """``reproducibility/embedders/factory.py:15-32`` for the ``plip`` / ``clip`` branches: ``args.model_name``
-    selects the flavour, ``args.backbone`` is the path of an OpenAI-clip (or HF) state dict saved with ``torch.save``.
-    The ``mudipath`` DenseNet baseline is a different model family and out of scope."""
+    """``reproducibility/embedders/factory.py:15-47``: ``args.model_name`` selects the flavour.  For ``plip`` / ``clip``
+    ``args.backbone`` is the path of an OpenAI-clip (or HF) state dict saved with ``torch.save``; for ``mudipath`` it
+    is only a name kept on the embedder, as in the reference, and the weights come from :func:`mudipath_checkpoint`."""
 
     def factory(self, args):
         name, path = args.model_name, args.backbone
+        if name == "mudipath":  # build_densenet(pretrained="mtdp") + Resize/CenterCrop/Normalize (factory.py:34-47)
+            from .densenet import DenseNetEngine
+            # The reference hands this file straight to clean_state_dict(...).items() and then to a strict
+            # load_state_dict, so it is a mapping of tensors: the tensors-only unpickler (weights_only) is enough and
+            # runs no code from the file.
+            sd = torch.load(mudipath_checkpoint(), map_location="cpu", weights_only=True)
+            return DenseNetEmbedder(DenseNetEngine(sd), None, name, path)
         arch = os.environ.get("PC_CLIP_ARCH", "ViT-B/32")
         if arch != "ViT-B/32":
             raise ValueError(f"plip_b200 implements ViT-B/32 only (PC_CLIP_ARCH={arch!r})")
@@ -127,7 +198,7 @@ class EmbedderFactory:
             model = PlipCLIPModel.from_openai_state_dict(self._openai_pretrained_state_dict(arch))
             model.eval()
             return CLIPEmbedder(model, None, name, path)
-        raise ValueError(f"unsupported embedder {name!r} (plip / clip)")
+        raise ValueError(f"unsupported embedder {name!r} (plip / clip / mudipath)")
 
     @staticmethod
     def _openai_pretrained_state_dict(arch: str):

@@ -169,6 +169,39 @@ def to_uint8_tiles(images: Sequence[ImageLike], workers: int = 0, crop: str = "f
     return out
 
 
+def resize_center_crop_bilinear(img: PIL.Image.Image, size: int = SIZE) -> PIL.Image.Image:
+    """torchvision ``Resize(size)`` (PIL ``BILINEAR``, shortest edge to ``size``, long edge ``int(size * long /
+    short)``) + ``CenterCrop(size)`` (``round`` offsets): the MuDiPath transform (``reproducibility/embedders/
+    factory.py:41-46``) before ``ToTensor``.  A ``size x size`` image is returned as it is, as Pillow's same-size
+    ``resize`` copies it."""
+    w, h = img.size
+    if (w, h) == (size, size):
+        return img
+    nw, nh, left, top = resize_plan(w, h, size, crop="round")
+    if (nw, nh) != (w, h):
+        img = img.resize((nw, nh), resample=PIL.Image.BILINEAR)
+    return img.crop((left, top, left + size, top + size))
+
+
+def to_uint8_tiles_bilinear(images: Sequence[ImageLike], workers: int = 0) -> np.ndarray:
+    """Batch of images -> uint8 ``[n,224,224,3]`` through :func:`resize_center_crop_bilinear`, after the RGB
+    conversion the reference's ``CLIPImageDataset`` applies first (``internal_datasets.py:42``)."""
+    out = np.empty((len(images), SIZE, SIZE, 3), dtype=np.uint8)
+
+    def _one(im: ImageLike) -> np.ndarray:
+        return np.asarray(resize_center_crop_bilinear(load_rgb(im), SIZE))
+
+    if workers > 1 and len(images) > 1:
+        from concurrent.futures import ThreadPoolExecutor
+        with ThreadPoolExecutor(max_workers=workers) as ex:
+            for i, tile in enumerate(ex.map(_one, images)):
+                out[i] = tile
+        return out
+    for i, im in enumerate(images):
+        out[i] = _one(im)
+    return out
+
+
 def chunks(seq: Sequence, n: int) -> Iterable[Sequence]:
     for i in range(0, len(seq), n):
         yield seq[i:i + n]
