@@ -21,18 +21,10 @@ import os
 import pytest
 import torch
 
+from attention_oracle import (ATT_ABS, DT, OBSERVED, REL, SENT, U32, _bits, _note, _round_to,
+                              assert_within, attention_contract_ref)
+
 gpu = pytest.mark.gpu
-
-DT = {0: torch.bfloat16, 1: torch.float16}
-REL = {0: 2.0 ** -8, 1: 2.0 ** -11}      # round-to-nearest into the 16-bit output: half an ulp <= this much of |x|
-U32 = 2.0 ** -23                         # one fp32 ulp, relative
-
-# largest err / tolerance seen per bound in this run; written to $PLIP_EDGE_REPORT (JSON) when that is set
-OBSERVED = {}
-
-
-def _note(key, ratio):
-    OBSERVED[key] = max(OBSERVED.get(key, 0.0), float(ratio))
 
 
 @pytest.fixture(scope="module")
@@ -131,71 +123,6 @@ def gemm_ref(A, W, bias, epi, x0=None, pos=None, ln=None):
     return pre, slack
 
 
-def _round_to(x64, dt):
-    return x64.float().to(dt).double()
-
-
-def _ulp_of(x64, fmt):
-    """Spacing of the 16-bit format in the binade of |x|; fp16 subnormals have a fixed spacing."""
-    _, e = torch.frexp(x64)                                   # x = m 2^e, m in [0.5, 1)
-    e = e.double() - (8 if fmt == 0 else 11)
-    if fmt == 1:
-        e = e.clamp_min(-24.0)
-    return torch.exp2(e)
-
-
-def attention_contract_ref(qkv, n_seq, S, heads, causal, mask, fmt):
-    """What attention_kernel is specified to compute, in float64, per (sequence, head):
-         s = q k^T (no scale: dh^-0.5 lives in the packed q weights), masked keys -> -inf,
-         p = exp(s - rowmax),  rowsum over the UNROUNDED p,  o = (round16(p) @ v) / rowsum.
-    Returns (contract, plain, flip), [n_seq * S, heads * 64] float64 each: `plain` is the ordinary softmax(s) @ v, and
-    `flip` bounds what the output may move when p values that sit on a rounding boundary of the 16-bit format round
-    the other way in the kernel: sum over such keys of ulp(p) |v| / rowsum.  The kernel's p differs from the float64
-    one by the error of its fp32 score and of the row maximum (4 k16 steps, each 2^-23 of at most sum_d |q_d k_d|),
-    by the rounding of the exp2 argument (2^-24 of its magnitude) and by ex2.approx (2 ulp).  A row without a visible key gives NaN here (the kernel returns zeros;
-    the cases below keep key 0 visible)."""
-    D = heads * 64
-    q, k, v = qkv.double().view(n_seq, S, 3, heads, 64).permute(2, 0, 3, 1, 4)
-    s = q @ k.transpose(-1, -2)
-    if causal:
-        s = s + torch.full((S, S), float("-inf"), device=qkv.device, dtype=torch.float64).triu(1)
-    if mask is not None:
-        s = s.masked_fill((mask == 0)[:, None, None, :], float("-inf"))
-    p = torch.exp(s - s.amax(-1, keepdim=True))
-    rowsum = p.sum(-1, keepdim=True)
-    pr = _round_to(p, DT[fmt])
-    ulp = _ulp_of(p, fmt)                                     # of p, not pr: just below a power of two the grid is finer
-    mag = q.abs() @ k.abs().transpose(-1, -2)
-    p_rel = 4 * U32 * (mag + mag.amax(-1, keepdim=True)) + 1.5 * 2.0 ** -24 * (s - s.amax(-1, keepdim=True)).abs() + 1e-6
-    near = (0.5 - (p - pr).abs() / ulp) < p_rel * p / ulp     # distance from the rounding boundary, in ulps
-    near &= p > 0
-    flip = ((ulp * near) @ v.abs()) / rowsum
-    contract = (pr @ v) / rowsum
-    plain = (p / rowsum) @ v
-
-    def rows(t):
-        return t.permute(0, 2, 1, 3).reshape(n_seq * S, D)
-    return rows(contract), rows(plain), rows(flip)
-
-
-def _first_bad(bad, err, tol, out, ref, what, where=None):
-    r, c = bad.nonzero()[0].tolist()
-    msg = (f"{what}: {int(bad.sum())} of {bad.numel()} elements out of bound; first at row {r} col {c}: "
-           f"out {out[r, c].item():.9g} ref {ref[r, c].item():.9g} err {err[r, c].item():.3g} tol {tol[r, c].item():.3g}")
-    if where is not None:
-        msg += " (" + where(r, c) + ")"
-    return msg
-
-
-def assert_within(out, ref, slack, rel, key, what, where=None):
-    out64 = out.double()
-    err = (out64 - ref).abs()
-    tol = rel * ref.abs() + slack
-    bad = ~(err <= tol)                                       # NaN counts as bad
-    assert not bad.any(), _first_bad(bad, err, tol, out64, ref, what, where)
-    _note(key, (err / tol).max().item())
-
-
 def test_references_against_torch_functional():
     """The float64 helpers agree with torch.nn.functional on small inputs (runs without a GPU)."""
     F = torch.nn.functional
@@ -244,16 +171,57 @@ def test_references_against_torch_functional():
             assert (flip >= 0).all() and torch.isfinite(flip).all()
 
 
+def test_long_and_probs_references_against_torch_functional(monkeypatch):
+    """The block-wise references of the long and the probabilities kernel against torch.nn.functional and against
+    the one-block reference (runs without a GPU)."""
+    import attention_oracle as AO
+    F = torch.nn.functional
+    g = torch.Generator().manual_seed(2)
+    for fmt in (0, 1):
+        for n_seq, S, heads in ((2, 7, 2), (1, 64, 2), (2, 65, 1), (2, 129, 2), (1, 200, 1)):
+            qkv = torch.randn(n_seq * S, 3 * heads * 64, generator=g).to(DT[fmt])
+            q, k, v = qkv.double().view(n_seq, S, 3, heads, 64).permute(2, 0, 3, 1, 4)
+            want = F.scaled_dot_product_attention(q, k, v, scale=1.0).permute(0, 2, 1, 3).reshape(n_seq * S, heads * 64)
+            contract, plain, flip = AO.long_attention_contract_ref(qkv, n_seq, S, heads, fmt)
+            assert torch.allclose(plain, want, rtol=0, atol=1e-10)
+            assert ((contract - plain).abs() <= REL[fmt] * 0.5 * 1.01 * v.abs().amax()).all()
+            assert (flip >= 0).all() and torch.isfinite(flip).all()
+            if S <= 64:                                       # one block: the short kernel's contract, bit for bit
+                short = attention_contract_ref(qkv, n_seq, S, heads, False, None, fmt)
+                assert torch.equal(contract, short[0]) and torch.equal(flip, short[2])
+            elif fmt == 0:                                    # rounded against m_b, not against the final maximum
+                assert not torch.equal(contract, attention_contract_ref(qkv, n_seq, S, heads, False, None, fmt)[0])
+            slack = AO.long_chain_slack(qkv, n_seq, S, heads)
+            assert (slack > 0).all() == (S > 64) and slack.max().item() < 1e-4
+            with monkeypatch.context() as mp:                 # rounding taken out: the block weights are exact
+                mp.setattr(AO, "_round_to", lambda x64, dt: x64)
+                assert torch.allclose(AO.long_attention_contract_ref(qkv, n_seq, S, heads, fmt)[0], want, rtol=0, atol=1e-10)
+            for causal, use_mask in ((False, False), (True, False), (True, True)):
+                mask = None
+                bias_mask = torch.zeros(n_seq, 1, S, S, dtype=torch.float64)
+                if use_mask:
+                    mask = (torch.rand(n_seq, S, generator=g) > 0.3).to(torch.int32)
+                    mask[:, 0] = 1
+                    bias_mask = bias_mask.masked_fill((mask == 0)[:, None, None, :], float("-inf"))
+                if causal:
+                    bias_mask = bias_mask + torch.full((S, S), float("-inf"), dtype=torch.float64).triu(1)
+                probs, rel = AO.probs_contract_ref(qkv, n_seq, S, heads, causal, mask)
+                want_p = torch.softmax(q @ k.transpose(-1, -2) + bias_mask, -1)
+                assert torch.allclose(probs, want_p, rtol=0, atol=1e-12)
+                assert torch.equal(rel > 0, want_p > 0) and rel.max().item() < 1e-3
+    # a row whose first block holds no visible key: no rescale link before its first key, probabilities from there on
+    S = 150
+    s = torch.full((1, S, S), float("-inf"), dtype=torch.float64)
+    s[0, :, 100:] = torch.linspace(0.0, 5.0, 50, dtype=torch.float64)
+    m_key, m_last, chain = AO.running_block_max(s)
+    assert torch.isinf(m_key[..., :64]).all() and (m_key[..., 64:128] == s[..., 127:128]).all()
+    assert (m_key[..., 128:] == 5.0).all() and (m_last == 5.0).all()
+    assert torch.allclose(chain, torch.full_like(chain, 2.0 ** -24 * 5.0 + 3 * U32), rtol=1e-12, atol=0)
+
+
 # ------------------------------------------------------------------------------------------------------------------
 # GEMM
 # ------------------------------------------------------------------------------------------------------------------
-SENT = -1536.0        # exactly representable in bf16, fp16 and fp32; no operand or result below comes near it
-
-
-def _bits(t):
-    return t.view(torch.int16 if t.element_size() == 2 else torch.int32)
-
-
 def assert_guards(buf, before, rows, cols, what, keep_rows=None):
     """Everything of `buf` outside [:rows, :cols] (pad columns, guard rows) — and, with keep_rows, those rows of the
     payload as well — still holds the bits it held before the launch."""
@@ -530,10 +498,6 @@ def test_gemm_rejections_launch_nothing(L):
 # ------------------------------------------------------------------------------------------------------------------
 # Attention
 # ------------------------------------------------------------------------------------------------------------------
-# Absolute slack of the attention output next to one ulp of the 16-bit result: the kernel's p carries ~1e-5 relative
-# error (fp32 scores of magnitude <= ~100, ex2.approx), so the output moves by that much of sum_k p_k |v_k| / rowsum
-# <= max |v| ~ 5 for N(0,1) inputs; the fp32 accumulation of P V adds 2^-23-ish of the same.  2e-4 covers both.
-ATT_ABS = 2e-4
 PLAIN_BOUNDS = {0: (0.03, 2e-3), 1: (6e-3, 4e-4)}   # (max, mean) |out - softmax(s) v| for N(0,1) inputs: P rounding
 
 
