@@ -32,7 +32,7 @@ extern "C" {
 
 #define PLIP_API __attribute__((visibility("default")))
 
-#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts, plip_window_mask_counts, plip_resize_region_*, plip_resize_filter_bounds, plip_sgd_*, plip_linear_decision, plip_densenet_*, plip_resize_crop_bilinear_u8 (new symbols only) */
+#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts, plip_window_mask_counts, plip_resize_region_*, plip_resize_filter_bounds, plip_sgd_*, plip_linear_decision, plip_densenet_*, plip_resize_crop_bilinear_u8, plip_warp_tiles_u8 (new symbols only) */
 
 /* Model constants (TF:configuration_clip.py:47-64,97-109,160-161). */
 #define PLIP_IMAGE_SIZE 224
@@ -256,6 +256,28 @@ PLIP_API int plip_resize_crop_u8(const void* src_dev, uint64_t src_bytes, const 
  * Accepts exactly the descriptors plip_resize_crop_u8 accepts. */
 PLIP_API int plip_resize_crop_bilinear_u8(const void* src_dev, uint64_t src_bytes, const plip_resize_desc_t* descs_host,
                                           int64_t n, void* tiles_dev, void* stream);
+
+/* The geometric steps of torchvision's RandomHorizontalFlip, RandomAffine(BILINEAR, fill) and
+ * RandomPerspective(BILINEAR, fill) on PIL images, the train-time transform of the reference
+ * (reproducibility/embedders/transform.py:18-42), on n RGB uint8 tiles [n,224,224,3]: tile i is mirrored
+ * left-right when descs[i].flip, then warped with PIL.Image.transform((224,224), AFFINE, affine, BILINEAR,
+ * fillcolor=(fill,)*3), then, when descs[i].apply_perspective, with Image.transform(..., PERSPECTIVE, perspective,
+ * BILINEAR, fillcolor=(fill,)*3) of that uint8 result — bit-identical to Pillow (IEEE double without FMA, results
+ * truncated to uint8).  The coefficients are Pillow's: the map from an output pixel centre to the source point
+ * (torchvision's inverse affine matrix and its float32 perspective coefficients).  src_dev / dst_dev: device tiles,
+ * 16-byte aligned, the same buffer (in place) or not overlapping.  descs_host: HOST array, consumed before the call
+ * returns.  Every argument is checked before anything is launched (n > 0, pointers, flags 0 / 1, fill 0..255, finite
+ * coefficients; the perspective ones when applied); an error names the offending value.  Stream-ordered. */
+typedef struct plip_warp_desc {
+  double affine[6];           /* source x = a0*x + a1*y + a2, y = a3*x + a4*y + a5 at pixel centres (x+0.5, y+0.5) */
+  double perspective[8];      /* x = (a0*x + a1*y + a2) / (a6*x + a7*y + 1), y = (a3*x + a4*y + a5) / (same) */
+  int32_t flip;               /* 1: mirror the columns before the affine warp */
+  int32_t apply_perspective;  /* 1: run the perspective warp after the affine one */
+  int32_t fill;               /* 0..255: every channel of a pixel whose source point lies outside the tile */
+  int32_t reserved;           /* 0 */
+} plip_warp_desc_t;
+PLIP_API int plip_warp_tiles_u8(const void* src_dev, void* dst_dev, const plip_warp_desc_t* descs_host, int64_t n,
+                                void* stream);
 
 /* Whole-image resize on the device, bit-identical to PIL.Image.fromarray(src).resize((new_width, new_height)) (BICUBIC,
  * no reducing_gap) for any ratio from upscaling to shrinks of over 64x (the horizontal filter must fit 64 columns in

@@ -54,6 +54,13 @@ class ResizeDesc(C.Structure):
     ]
 
 
+class WarpDesc(C.Structure):
+    """Mirror of ``plip_warp_desc_t`` (128 bytes; ``preprocess.WARP_DESC_DTYPE`` is the numpy twin)."""
+
+    _fields_ = [("affine", C.c_double * 6), ("perspective", C.c_double * 8), ("flip", C.c_int32),
+                ("apply_perspective", C.c_int32), ("fill", C.c_int32), ("reserved", C.c_int32)]
+
+
 class SgdProblem(C.Structure):
     """Mirror of ``plip_sgd_problem_t`` (32 bytes)."""
 
@@ -101,6 +108,7 @@ SIGNATURES = {
     "plip_window_mask_counts": (_i, [_vp, _i, _i, _i, _i64, _vp, _i64, _i, _vp, _vp]),
     "plip_resize_crop_u8": (_i, [_vp, _u64, _vp, _i64, _vp, _vp]),
     "plip_resize_crop_bilinear_u8": (_i, [_vp, _u64, _vp, _i64, _vp, _vp]),
+    "plip_warp_tiles_u8": (_i, [_vp, _vp, _vp, _i64, _vp]),
     "plip_resize_region_workspace": (_i, [_i, _i, _i, _i, _i, _i, C.POINTER(_u64)]),
     "plip_resize_region_u8": (_i, [_vp, _i64, _i, _i, _i, _i, _vp, _i64, _i, _i, _i, _i, _vp, _u64, _vp]),
     "plip_resize_filter_bounds": (_i, [_i, _i, _vp]),

@@ -1184,6 +1184,12 @@ PLIP_API int plip_resize_crop_bilinear_u8(const void* src_dev, uint64_t src_byte
                             static_cast<uint8_t*>(tiles_dev), static_cast<cudaStream_t>(stream), true);
 }
 
+PLIP_API int plip_warp_tiles_u8(const void* src_dev, void* dst_dev, const plip_warp_desc_t* descs_host, int64_t n,
+                                void* stream) {
+  return launch_warp_tiles(static_cast<const uint8_t*>(src_dev), static_cast<uint8_t*>(dst_dev), descs_host, n,
+                           static_cast<cudaStream_t>(stream));
+}
+
 PLIP_API int plip_resize_region_workspace(int height, int width, int new_height, int new_width, int out_row0,
                                           int out_row1, uint64_t* bytes) {
   PLIP_REQUIRE(bytes, "plip_resize_region_workspace: null argument");

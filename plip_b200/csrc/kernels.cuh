@@ -62,6 +62,10 @@ int launch_resize_region(const uint8_t* src, int64_t src_pitch, int src_row0, in
 // Per output index of one axis, its filter window: bounds[2 * xx] = first source index, bounds[2 * xx + 1] = count.
 int resize_filter_bounds(int in_size, int out_size, int32_t* bounds);
 
+// augment.cu: flip + affine + perspective warps of [n,224,224,3] uint8 tiles, Pillow-exact (plip_warp_tiles_u8; every
+// argument is checked before anything is launched; src == dst runs in place).
+int launch_warp_tiles(const uint8_t* src, uint8_t* dst, const plip_warp_desc_t* descs_host, int64_t n, cudaStream_t st);
+
 // attention.cu: softmax(q k^T [+causal/padding mask]) v per (sequence, head); q pre-scaled by dh^-0.5.
 // qkv: bf16 [n_seq*seq_len, 3*heads*64]; key_mask: optional int32 [n_seq, seq_len] (0 = masked key).
 // seq_len > 128 (up to kMaxVisSeq) runs the long-sequence kernel: no causal mask, no key mask.

@@ -20,7 +20,7 @@ import torch
 from .modeling import PlipCLIPModel
 from .tokenizer import find_tokenizer
 from .preprocess import decode_native_then_rgb, SIZE, chunks, decode_rgb, device_resizable, pack_rgb, to_uint8_tiles
-from .preprocess import to_uint8_tiles_bilinear
+from .preprocess import to_uint8_tiles_bilinear, TrainTransform
 
 
 class AbstractEmbedder(ABC):
@@ -53,7 +53,9 @@ class CLIPEmbedder(AbstractEmbedder):
 
     def __init__(self, model, preprocess, name, backbone, tokenize: Optional[Callable] = None):
         self.model = model
-        self.preprocess = preprocess  # kept for API parity; tiles are prepared by plip_b200.preprocess
+        # A TrainTransform runs the reference's train-time transform on the device; any other value is kept for API
+        # parity only (tiles are then prepared by plip_b200.preprocess).
+        self.preprocess = preprocess
         self.name = name
         self.backbone = backbone
         self.tokenize = tokenize or _default_tokenize(
@@ -66,9 +68,16 @@ class CLIPEmbedder(AbstractEmbedder):
         return self.embed_text(list_of_labels, device=device, num_workers=num_workers, batch_size=batch_size)
 
     def embed_images(self, list_of_images: Sequence, device="cuda", num_workers=1, batch_size=32) -> np.ndarray:
-        """``embedders/plip.py:37-54``: paths / PIL images -> normalised ``[N,512]`` float32."""
+        """``embedders/plip.py:37-54``: paths / PIL images -> normalised ``[N,512]`` float32.
+
+        With a :class:`~plip_b200.preprocess.TrainTransform` as ``preprocess`` the tiles are the reference's
+        ``DataLoader(CLIPImageDataset(images, _train_transform(...)), batch_size, num_workers)`` ones under the same
+        torch RNG state (``TrainTransform.tiles``); ``model.encode_image(tt.tiles(...))`` gives the un-normalised rows
+        that ``scripts/extract_embedding.py`` saves next to the normalised ones."""
         outs: List[torch.Tensor] = []
         eng = getattr(self.model, "engine", None)
+        if isinstance(self.preprocess, TrainTransform):
+            return self._embed_train_transform(list(list_of_images), device, int(num_workers), int(batch_size), eng)
         for chunk in chunks(list(list_of_images), max(int(batch_size), 256)):
             # torchvision's CenterCrop rounding (transform.py:45-52), not CLIPImageProcessor's floor
             if eng is not None:
@@ -86,6 +95,23 @@ class CLIPEmbedder(AbstractEmbedder):
                 tiles = to_uint8_tiles(chunk, int(num_workers), crop="round")
                 t = torch.from_numpy(tiles).to(device)
                 e = self.model.encode_image(t).detach().float().cpu()
+                outs.append(e / e.norm(dim=1, keepdim=True))
+        return torch.cat(outs, dim=0).numpy()
+
+    def _embed_train_transform(self, images: list, device, num_workers: int, batch_size: int, eng) -> np.ndarray:
+        """Chunks of decoded images -> tiles through the TrainTransform (one DataLoader pass of random draws over the
+        whole list) -> normalised rows."""
+        tt = self.preprocess
+        stream = tt.stream(num_workers, batch_size)
+        outs = [torch.empty(0, 512)]
+        for chunk in chunks(images, max(batch_size, 256)):
+            arrays = decode_rgb(chunk, num_workers)
+            params = stream.draw([(a.shape[1], a.shape[0]) for a in arrays])
+            tiles = tt.apply(arrays, params, eng.device if eng is not None else device, num_workers)
+            if eng is not None:
+                outs.append(eng.encode_images(tiles, normalize=True).cpu())
+            else:  # any OpenAI-clip-like model
+                e = self.model.encode_image(tiles).detach().float().cpu()
                 outs.append(e / e.norm(dim=1, keepdim=True))
         return torch.cat(outs, dim=0).numpy()
 

@@ -249,6 +249,58 @@ def resize_region(region: torch.Tensor, new_h: int, new_w: int, out: Optional[to
     return resize_rows(region, 0, h, int(new_h), int(new_w), (0, int(new_h)), out)
 
 
+def _device_tiles(t, what: str) -> int:
+    """``n`` of a contiguous CUDA uint8 ``[n,224,224,3]`` tensor; ``ValueError`` otherwise."""
+    if not (torch.is_tensor(t) and t.is_cuda and t.dtype == torch.uint8 and t.dim() == 4
+            and tuple(t.shape[1:]) == (IMAGE_SIZE, IMAGE_SIZE, 3) and t.is_contiguous()):
+        raise ValueError(f"{what} must be a contiguous CUDA uint8 [n,224,224,3] tensor, got "
+                         f"{getattr(t, 'dtype', type(t))} {tuple(getattr(t, 'shape', ()))}")
+    return int(t.shape[0])
+
+
+@torch.no_grad()
+def resize_crop(src: torch.Tensor, descs: np.ndarray, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Packed RGB uint8 images on the device + host descriptors (``preprocess.pack_rgb``) -> uint8 tiles
+    ``[n,224,224,3]`` on the same device; Pillow-exact bicubic resize and crop (``plip_resize_crop_u8``).  Needs no
+    engine."""
+    from .preprocess import RESIZE_DESC_DTYPE
+    assert src.is_cuda and src.dtype == torch.uint8 and src.is_contiguous() and src.dim() == 1
+    descs = np.ascontiguousarray(descs, dtype=RESIZE_DESC_DTYPE)
+    n = int(descs.shape[0])
+    if out is None:
+        out = torch.empty((n, 224, 224, 3), device=src.device, dtype=torch.uint8)
+    assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and out.numel() == n * 224 * 224 * 3
+    if n:
+        with torch.cuda.device(src.device):
+            check(lib().plip_resize_crop_u8(src.data_ptr(), int(src.numel()), descs.ctypes.data, n, out.data_ptr(),
+                                            torch.cuda.current_stream(src.device).cuda_stream), "plip_resize_crop_u8")
+    return out
+
+
+@torch.no_grad()
+def warp_tiles(tiles: torch.Tensor, params: np.ndarray, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Flip / affine / perspective warps of CUDA uint8 tiles ``[n,224,224,3]``, bit-identical to Pillow's
+    ``Image.transpose`` and ``Image.transform(AFFINE | PERSPECTIVE, BILINEAR, fillcolor)`` (``plip_warp_tiles_u8``).
+    ``params``: ``preprocess.WARP_DESC_DTYPE`` rows, one per tile (``TrainTransform`` draws them).  ``out``: a tensor
+    of the same shape on the same device, ``tiles`` itself (in place) or a new tensor.  Every argument is checked
+    before any launch (``ValueError``).  Needs no engine."""
+    from .preprocess import WARP_DESC_DTYPE
+    n = _device_tiles(tiles, "tiles")
+    params = np.ascontiguousarray(params, dtype=WARP_DESC_DTYPE).reshape(-1)
+    if params.shape[0] != n:
+        raise ValueError(f"warp_tiles: {params.shape[0]} descriptors for {n} tiles")
+    if out is None:
+        out = torch.empty_like(tiles)
+    elif _device_tiles(out, "out") != n or out.device != tiles.device:
+        raise ValueError(f"warp_tiles: out must be [{n},224,224,3] on {tiles.device}")
+    if n:
+        with torch.cuda.device(tiles.device):
+            _check_args(lib().plip_warp_tiles_u8(tiles.data_ptr(), out.data_ptr(), params.ctypes.data, n,
+                                                 torch.cuda.current_stream(tiles.device).cuda_stream),
+                        "plip_warp_tiles_u8")
+    return out
+
+
 @torch.no_grad()
 def window_mask_counts(mask: torch.Tensor, origins, threshold: int = 10) -> torch.Tensor:
     """Per window, the mask elements ``> threshold``: int32 ``[n]`` on the mask's device, exact
@@ -548,18 +600,7 @@ class Engine:
     def resize_crop(self, src: torch.Tensor, descs: np.ndarray, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Packed RGB uint8 images on the device + host descriptors (``preprocess.pack_rgb``) -> uint8 tiles
         ``[n,224,224,3]``; Pillow-exact bicubic resize and crop (``plip_resize_crop_u8``)."""
-        from .preprocess import RESIZE_DESC_DTYPE
-        assert src.is_cuda and src.dtype == torch.uint8 and src.is_contiguous() and src.dim() == 1
-        descs = np.ascontiguousarray(descs, dtype=RESIZE_DESC_DTYPE)
-        n = int(descs.shape[0])
-        if out is None:
-            out = torch.empty((n, 224, 224, 3), device=src.device, dtype=torch.uint8)
-        assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and out.numel() == n * 224 * 224 * 3
-        if n:
-            with torch.cuda.device(src.device):
-                check(self._L.plip_resize_crop_u8(src.data_ptr(), int(src.numel()), descs.ctypes.data, n,
-                                                  out.data_ptr(), self._stream()), "plip_resize_crop_u8")
-        return out
+        return resize_crop(src, descs, out)
 
     # ---- per-token outputs (output_hidden_states / output_attentions) ----------------------------------------------
     def _outputs(self, n: int, S: int, D: int, heads: int, output_hidden_states: bool, output_attentions: bool,
