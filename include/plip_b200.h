@@ -32,7 +32,7 @@ extern "C" {
 
 #define PLIP_API __attribute__((visibility("default")))
 
-#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts, plip_window_mask_counts, plip_resize_region_*, plip_resize_filter_bounds, plip_sgd_*, plip_linear_decision, plip_densenet_*, plip_resize_crop_bilinear_u8, plip_warp_tiles_u8 (new symbols only) */
+#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts, plip_window_mask_counts, plip_resize_region_*, plip_resize_filter_bounds, plip_sgd_*, plip_linear_decision, plip_densenet_*, plip_resize_crop_bilinear_u8, plip_warp_tiles_u8, plip_resize_crop_fill_u8, plip_mask_value_sets_u8 (new symbols only) */
 
 /* Model constants (TF:configuration_clip.py:47-64,97-109,160-161). */
 #define PLIP_IMAGE_SIZE 224
@@ -256,6 +256,26 @@ PLIP_API int plip_resize_crop_u8(const void* src_dev, uint64_t src_bytes, const 
  * Accepts exactly the descriptors plip_resize_crop_u8 accepts. */
 PLIP_API int plip_resize_crop_bilinear_u8(const void* src_dev, uint64_t src_bytes, const plip_resize_desc_t* descs_host,
                                           int64_t n, void* tiles_dev, void* stream);
+/* The bicubic resize with the crop window anywhere: new_width / new_height may be 1..65536 and left / top any int32.
+ * Tile pixel (x, y) is the resized image's pixel (left + x, top + y) when that lies inside it, else (0, 0, 0) —
+ * bit-identical to PIL.Image.resize((new_width,new_height), BICUBIC).crop((left, top, left + 224, top + 224)), which is
+ * what the reference's evaluation-tile resize (generate_validation_datasets/prepare_dataset_to_csv.py:40-63,
+ * resizeimg) saves for an RGB image.  Rows of the tile entirely outside the resized image read no source.  A
+ * descriptor whose filter tables and strip do not fit the kernel's 200 KB shared-memory plan (shrinks of roughly 25x
+ * and more; the error names the image and its sizes) is rejected, like every other invalid argument, before anything
+ * is launched.  Same call shape and stream semantics as plip_resize_crop_u8. */
+PLIP_API int plip_resize_crop_fill_u8(const void* src_dev, uint64_t src_bytes, const plip_resize_desc_t* descs_host,
+                                      int64_t n, void* tiles_dev, void* stream);
+
+/* The distinct byte values of every (image, channel) of a device uint8 array masks_dev [n, height, width, channels]
+ * (C order, channels 1..8, height * width * channels < 2^31, 16-byte aligned): sets_dev uint32 [n, channels, 8], bit
+ * (v & 31) of word (v >> 5) set iff value v occurs in that channel of that image.  The call zeroes sets_dev itself.
+ * len(np.unique(masks[i, ..., j])) is the set's popcount, and masks[i, ..., j] is all zero iff the set is exactly {0}
+ * (the reference's PanNuke labelling, generate_validation_datasets/preprocess/preprocess_PanNuke.py:39,56-59).  One
+ * pass over the array, which is read once; every argument is checked before anything is launched.  Stream-ordered,
+ * allocates nothing. */
+PLIP_API int plip_mask_value_sets_u8(const void* masks_dev, int64_t n, int height, int width, int channels,
+                                     uint32_t* sets_dev, void* stream);
 
 /* The geometric steps of torchvision's RandomHorizontalFlip, RandomAffine(BILINEAR, fill) and
  * RandomPerspective(BILINEAR, fill) on PIL images, the train-time transform of the reference

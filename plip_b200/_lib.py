@@ -108,6 +108,8 @@ SIGNATURES = {
     "plip_window_mask_counts": (_i, [_vp, _i, _i, _i, _i64, _vp, _i64, _i, _vp, _vp]),
     "plip_resize_crop_u8": (_i, [_vp, _u64, _vp, _i64, _vp, _vp]),
     "plip_resize_crop_bilinear_u8": (_i, [_vp, _u64, _vp, _i64, _vp, _vp]),
+    "plip_resize_crop_fill_u8": (_i, [_vp, _u64, _vp, _i64, _vp, _vp]),
+    "plip_mask_value_sets_u8": (_i, [_vp, _i64, _i, _i, _i, _vp, _vp]),
     "plip_warp_tiles_u8": (_i, [_vp, _vp, _vp, _i64, _vp]),
     "plip_resize_region_workspace": (_i, [_i, _i, _i, _i, _i, _i, C.POINTER(_u64)]),
     "plip_resize_region_u8": (_i, [_vp, _i64, _i, _i, _i, _i, _vp, _i64, _i, _i, _i, _i, _vp, _u64, _vp]),

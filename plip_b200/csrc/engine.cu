@@ -1184,6 +1184,20 @@ PLIP_API int plip_resize_crop_bilinear_u8(const void* src_dev, uint64_t src_byte
                             static_cast<uint8_t*>(tiles_dev), static_cast<cudaStream_t>(stream), true);
 }
 
+PLIP_API int plip_resize_crop_fill_u8(const void* src_dev, uint64_t src_bytes, const plip_resize_desc_t* descs_host,
+                                      int64_t n, void* tiles_dev, void* stream) {
+  PLIP_REQUIRE(src_dev && descs_host && tiles_dev, "plip_resize_crop_fill_u8: null argument");
+  PLIP_REQUIRE(n > 0, "plip_resize_crop_fill_u8: n must be positive (got %lld)", (long long)n);
+  return launch_resize_crop(static_cast<const uint8_t*>(src_dev), (size_t)src_bytes, descs_host, n,
+                            static_cast<uint8_t*>(tiles_dev), static_cast<cudaStream_t>(stream), false, true);
+}
+
+PLIP_API int plip_mask_value_sets_u8(const void* masks_dev, int64_t n, int height, int width, int channels,
+                                     uint32_t* sets_dev, void* stream) {
+  return launch_mask_value_sets(static_cast<const uint8_t*>(masks_dev), n, height, width, channels, sets_dev,
+                                static_cast<cudaStream_t>(stream));
+}
+
 PLIP_API int plip_warp_tiles_u8(const void* src_dev, void* dst_dev, const plip_warp_desc_t* descs_host, int64_t n,
                                 void* stream) {
   return launch_warp_tiles(static_cast<const uint8_t*>(src_dev), static_cast<uint8_t*>(dst_dev), descs_host, n,

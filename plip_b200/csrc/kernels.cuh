@@ -45,9 +45,13 @@ int launch_gather_rows(const __nv_bfloat16* a16, const float* x32, const int32_t
                        int64_t n, int dim, __nv_bfloat16* a16_out, float* x32_out, cudaStream_t st);
 
 // resize.cu: Pillow-exact bicubic resize + crop of packed RGB uint8 images into [n,224,224,3] tiles.
-// bilinear: Pillow's triangle filter instead of its bicubic one (plip_resize_crop_bilinear_u8).
+// bilinear: Pillow's triangle filter instead of its bicubic one (plip_resize_crop_bilinear_u8).  fill (bicubic only):
+// any resized size and crop origin, zeros outside the resized image (plip_resize_crop_fill_u8).
 int launch_resize_crop(const uint8_t* src, size_t src_bytes, const plip_resize_desc_t* descs_host, int64_t n,
-                       uint8_t* tiles, cudaStream_t st, bool bilinear = false);
+                       uint8_t* tiles, cudaStream_t st, bool bilinear = false, bool fill = false);
+// mask_sets.cu: the set of byte values present in every (image, channel) of a uint8 [n, h, w, c] array, as 256-bit
+// masks: sets uint32 [n, c, 8] (zeroed here, then filled; plip_mask_value_sets_u8).
+int launch_mask_value_sets(const uint8_t* masks, int64_t n, int h, int w, int c, uint32_t* sets, cudaStream_t st);
 
 int resize_filter_host(int in_size, int out_size, int xx, int32_t* k, int k_cap, int* xmin, int* count);
 int resize_filter_bilinear_host(int in_size, int out_size, int xx, int32_t* k, int k_cap, int* xmin, int* count);

@@ -187,7 +187,12 @@ __device__ __forceinline__ void hpass_pixel8(const uint8_t* p, const int4 k0, co
   hgroup<GUARD>(wp, prev, mis * 8, k1, end_w, end_b, a0, a1, a2);
 }
 
-template <bool BILINEAR>
+// FILL (plip_resize_crop_fill_u8): the crop window may reach past the resized image on any side, and pixels outside
+// it are (0, 0, 0), as PIL's crop fills them.  Only the tile columns [c_lo, c_hi) and this CTA's rows [r_lo, r_hi)
+// inside the resized image get filters; the other rows' vertical filters repeat the nearest inside row's (so the
+// strip holds only source rows that inside rows read) and their outputs are overwritten with zeros; the other
+// columns' strip entries are zeros, which the vertical pass turns into zeros.
+template <bool BILINEAR, bool FILL = false>
 __device__ __forceinline__ void resize_crop_body(const uint8_t* __restrict__ src, uint64_t src_bytes,
                                                  uint8_t* __restrict__ tiles, const ResizeBatch& batch,
                                                  int64_t first_image) {
@@ -196,6 +201,17 @@ __device__ __forceinline__ void resize_crop_body(const uint8_t* __restrict__ src
   const int row0 = blockIdx.x * kRsRowsPerCta;  // first output row of this CTA
   const AxisFilter fh = make_axis<BILINEAR>(im.w, im.new_w), fv = make_axis<BILINEAR>(im.h, im.new_h);
   const int ksh4 = (fh.ksize + 3) & ~3, ksv4 = (fv.ksize + 3) & ~3;  // filter rows zero-padded to 4 taps
+  int r_lo = 0, r_hi = kRsRowsPerCta, c_lo = 0, c_hi = kImage;
+  if (FILL) {
+    r_lo = max(0, -im.top - row0), r_hi = min(kRsRowsPerCta, im.new_h - im.top - row0);
+    c_lo = max(0, -im.left), c_hi = min(kImage, im.new_w - im.left);
+    if (r_lo >= r_hi || c_lo >= c_hi) {  // every pixel of these rows is outside: zeros, no source read
+      uint32_t* o = reinterpret_cast<uint32_t*>(tiles + ((first_image + blockIdx.y) * kImage + row0) *
+                                                            (int64_t)kTileRowBytes);
+      for (int i = threadIdx.x; i < kRsRowsPerCta * kTileRowBytes / 4; i += kRsThreads) o[i] = 0;
+      return;
+    }
+  }
 
   int* kh = reinterpret_cast<int*>(rs_smem);                 // [224][ksh4]
   int* kv = kh + kImage * ksh4;                              // [32][ksv4]
@@ -209,10 +225,12 @@ __device__ __forceinline__ void resize_crop_body(const uint8_t* __restrict__ src
     const int j = horiz ? t : t - kImage;
     int* k = horiz ? kh + j * ksh4 : kv + j * ksv4;
     int lo, cnt;
-    if (horiz)
+    if (FILL && horiz && (j < c_lo || j >= c_hi))
+      lo = 0, cnt = 0;
+    else if (horiz)
       filter_row<BILINEAR>(fh, im.w, im.left + j, k, lo, cnt);
     else
-      filter_row<BILINEAR>(fv, im.h, im.top + row0 + j, k, lo, cnt);
+      filter_row<BILINEAR>(fv, im.h, im.top + row0 + (FILL ? min(max(j, r_lo), r_hi - 1) : j), k, lo, cnt);
     for (int x = cnt; x < (horiz ? ksh4 : ksv4); ++x) k[x] = 0;
     int* bnd = horiz ? bh + 2 * j : bv + 2 * j;
     bnd[0] = lo;
@@ -228,13 +246,21 @@ __device__ __forceinline__ void resize_crop_body(const uint8_t* __restrict__ src
   const int rp = im.rows_per_pass;
   constexpr int kRowWords = kTileRowBytes / 4;  // 168
   for (int sub = 0; sub < kRsRowsPerCta; sub += rp) {
+    if (FILL && (sub + rp <= r_lo || sub >= r_hi)) {  // a strip of outside rows
+      for (int i = t; i < rp * kRowWords; i += kRsThreads)
+        reinterpret_cast<uint32_t*>(out + sub * kTileRowBytes)[i] = 0;
+      continue;
+    }
     const int s0 = bv[2 * sub];
     const int s1 = bv[2 * (sub + rp - 1)] + bv[2 * (sub + rp - 1) + 1];
     const int nrows = s1 - s0;
     if (nrows > im.strip_rows) __trap();  // host sizing bug: never expected
     // horizontal pass: strip[r][xx][0..2] for the source rows [s0, s1).  Thread t owns output column t (window,
     // weights and pointers are then loop invariants) and walks down the rows; threads 224..255 sit this out.
-    if (t < kImage) {
+    if (FILL && t < kImage && (t < c_lo || t >= c_hi)) {
+      for (int r = 0; r < nrows; ++r) strip[r * kTileRowBytes + 3 * t] = strip[r * kTileRowBytes + 3 * t + 1] =
+                                          strip[r * kTileRowBytes + 3 * t + 2] = 0;
+    } else if (t < kImage) {
       const uint8_t* p = img + (int64_t)s0 * src_row_bytes + (int64_t)bh[2 * t] * 3;
       const uint8_t* lim = reinterpret_cast<const uint8_t*>(end_w);
       uint8_t* d = strip + t * 3;
@@ -283,8 +309,9 @@ __device__ __forceinline__ void resize_crop_body(const uint8_t* __restrict__ src
         a2 += byte_of(w0, 2) * kk.x + byte_of(w1, 2) * kk.y + byte_of(w2, 2) * kk.z + byte_of(w3, 2) * kk.w;
         a3 += byte_of(w0, 3) * kk.x + byte_of(w1, 3) * kk.y + byte_of(w2, 3) * kk.z + byte_of(w3, 3) * kk.w;
       }
-      reinterpret_cast<uint32_t*>(out + (sub + j) * kTileRowBytes)[e] =
-          clip8(a0) | (clip8(a1) << 8) | (clip8(a2) << 16) | (clip8(a3) << 24);
+      uint32_t v = clip8(a0) | (clip8(a1) << 8) | (clip8(a2) << 16) | (clip8(a3) << 24);
+      if (FILL && (sub + j < r_lo || sub + j >= r_hi)) v = 0;
+      reinterpret_cast<uint32_t*>(out + (sub + j) * kTileRowBytes)[e] = v;
     }
     __syncthreads();
   }
@@ -303,6 +330,16 @@ __global__ void __launch_bounds__(kRsThreads) resize_crop_bilinear_kernel(const 
                                                                           const ResizeBatch batch,
                                                                           int64_t first_image) {
   resize_crop_body<true>(src, src_bytes, tiles, batch, first_image);
+}
+
+// Bicubic resize to any size and a 224 x 224 window anywhere, zeros outside the resized image: the reference's
+// evaluation-tile resize (resizeimg) and PIL's crop past the image edge.
+__global__ void __launch_bounds__(kRsThreads) resize_crop_fill_kernel(const uint8_t* __restrict__ src,
+                                                                      uint64_t src_bytes,
+                                                                      uint8_t* __restrict__ tiles,
+                                                                      const ResizeBatch batch,
+                                                                      int64_t first_image) {
+  resize_crop_body<false, true>(src, src_bytes, tiles, batch, first_image);
 }
 
 constexpr size_t kRsSmemHard = 200 * 1024;
@@ -340,20 +377,27 @@ int resize_filter_bilinear_host(int in_size, int out_size, int xx, int32_t* k, i
 
 // Validates descriptor `idx` and fills the kernel-side plan (strip height, shared memory need).
 // Tables and strips are sized for the bicubic filter; the bilinear one's windows lie inside the bicubic ones, so the
-// same plan also holds it (with some shared memory to spare).  `fn` names the entry point in errors.
+// same plan also holds it (with some shared memory to spare).  `fn` names the entry point in errors.  `fill`: any
+// resized size and crop origin (plip_resize_crop_fill_u8); an origin that puts the whole window outside on one axis
+// is clamped to one that still does, so the kernel's index arithmetic stays in int32.
 static int plan_image(const char* fn, const plip_resize_desc_t& s, long long idx, size_t src_bytes, ResizeImg& o,
-                      size_t& need_out) {
+                      size_t& need_out, bool fill = false) {
   PLIP_REQUIRE(s.width > 0 && s.height > 0 && s.width <= 65536 && s.height <= 65536,
                "%s: image %lld has invalid size %dx%d", fn, idx, s.width, s.height);
   PLIP_REQUIRE(s.offset >= 0 && (uint64_t)s.offset + (uint64_t)s.width * s.height * 3 <= src_bytes,
                "%s: image %lld (%dx%d at byte %lld) exceeds the %llu-byte source buffer", fn, idx,
                s.width, s.height, (long long)s.offset, (unsigned long long)src_bytes);
-  PLIP_REQUIRE(s.new_width >= kImage && s.new_height >= kImage && s.new_width <= 65536 && s.new_height <= 65536,
-               "%s: image %lld: resized size %dx%d is smaller than the %dx%d tile", fn, idx,
-               s.new_width, s.new_height, kImage, kImage);
-  PLIP_REQUIRE(s.left >= 0 && s.top >= 0 && s.left + kImage <= s.new_width && s.top + kImage <= s.new_height,
-               "%s: image %lld: crop origin (%d,%d) leaves the %dx%d resized image", fn, idx, s.left,
-               s.top, s.new_width, s.new_height);
+  if (fill) {
+    PLIP_REQUIRE(s.new_width >= 1 && s.new_height >= 1 && s.new_width <= 65536 && s.new_height <= 65536,
+                 "%s: image %lld: resized size %dx%d is outside 1..65536", fn, idx, s.new_width, s.new_height);
+  } else {
+    PLIP_REQUIRE(s.new_width >= kImage && s.new_height >= kImage && s.new_width <= 65536 && s.new_height <= 65536,
+                 "%s: image %lld: resized size %dx%d is smaller than the %dx%d tile", fn, idx,
+                 s.new_width, s.new_height, kImage, kImage);
+    PLIP_REQUIRE(s.left >= 0 && s.top >= 0 && s.left + kImage <= s.new_width && s.top + kImage <= s.new_height,
+                 "%s: image %lld: crop origin (%d,%d) leaves the %dx%d resized image", fn, idx, s.left,
+                 s.top, s.new_width, s.new_height);
+  }
   const int ksh = axis_ksize(s.width, s.new_width), ksv = axis_ksize(s.height, s.new_height);
   const size_t tb = table_bytes(ksh, ksv);
   // Strip height: taller strips re-read fewer source rows (adjacent strips overlap by the filter support),
@@ -379,13 +423,17 @@ static int plan_image(const char* fn, const plip_resize_desc_t& s, long long idx
   o.src_off = s.offset;
   o.w = s.width, o.h = s.height, o.new_w = s.new_width, o.new_h = s.new_height;
   o.left = s.left, o.top = s.top, o.rows_per_pass = rp, o.strip_rows = rows;
+  if (fill) {
+    o.left = s.left < -kImage ? -kImage : (s.left > s.new_width ? s.new_width : s.left);
+    o.top = s.top < -kImage ? -kImage : (s.top > s.new_height ? s.new_height : s.top);
+  }
   need_out = tb + (size_t)(rows + kStripPadRows) * kTileRowBytes;
   return 0;
 }
 
 int launch_resize_crop(const uint8_t* src, size_t src_bytes, const plip_resize_desc_t* d, int64_t n, uint8_t* tiles,
-                       cudaStream_t st, bool bilinear) {
-  const char* fn = bilinear ? "plip_resize_crop_bilinear_u8" : "plip_resize_crop_u8";
+                       cudaStream_t st, bool bilinear, bool fill) {
+  const char* fn = fill ? "plip_resize_crop_fill_u8" : bilinear ? "plip_resize_crop_bilinear_u8" : "plip_resize_crop_u8";
   PLIP_REQUIRE(reinterpret_cast<uintptr_t>(src) % 4 == 0 && reinterpret_cast<uintptr_t>(tiles) % 4 == 0,
                "%s: src_dev and tiles_dev must be 4-byte aligned", fn);
   // every descriptor is checked before anything is launched: a bad one leaves the output untouched
@@ -393,11 +441,11 @@ int launch_resize_crop(const uint8_t* src, size_t src_bytes, const plip_resize_d
     ResizeImg scratch;
     size_t need;
     for (int64_t i = 0; i < n; ++i)
-      if (int rc = plan_image(fn, d[i], (long long)i, src_bytes, scratch, need)) return rc;
+      if (int rc = plan_image(fn, d[i], (long long)i, src_bytes, scratch, need, fill)) return rc;
   }
-  auto kernel = bilinear ? resize_crop_bilinear_kernel : resize_crop_kernel;
-  static unsigned long long configured[2] = {0, 0};
-  if (first_use_on_device(configured[bilinear]))
+  auto kernel = fill ? resize_crop_fill_kernel : bilinear ? resize_crop_bilinear_kernel : resize_crop_kernel;
+  static unsigned long long configured[3] = {0, 0, 0};
+  if (first_use_on_device(configured[fill ? 2 : bilinear]))
     PLIP_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRsSmemHard));
   for (int64_t base = 0; base < n; base += kRsBatch) {
     const int cnt = (int)((n - base) < kRsBatch ? (n - base) : kRsBatch);
@@ -405,7 +453,7 @@ int launch_resize_crop(const uint8_t* src, size_t src_bytes, const plip_resize_d
     size_t smem = 0;
     for (int i = 0; i < cnt; ++i) {
       size_t need = 0;
-      if (int rc = plan_image(fn, d[base + i], (long long)(base + i), src_bytes, b.img[i], need)) return rc;
+      if (int rc = plan_image(fn, d[base + i], (long long)(base + i), src_bytes, b.img[i], need, fill)) return rc;
       smem = need > smem ? need : smem;
     }
     PLIP_CUDA_CHECK(launch_kernel(kernel, dim3(kImage / kRsRowsPerCta, cnt), dim3(kRsThreads), smem, st, 1,

@@ -278,6 +278,53 @@ def resize_crop(src: torch.Tensor, descs: np.ndarray, out: Optional[torch.Tensor
 
 
 @torch.no_grad()
+def resize_crop_fill(src: torch.Tensor, descs: np.ndarray, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """:func:`resize_crop` with the resized size and crop origin unrestricted (``plip_resize_crop_fill_u8``): tile pixel
+    ``(x, y)`` is the resized image's ``(left + x, top + y)`` when that lies inside it, else ``(0, 0, 0)`` — PIL's
+    ``resize(...).crop(...)`` past the image edge.  Every descriptor is checked before any launch (``ValueError``).
+    Needs no engine."""
+    from .preprocess import RESIZE_DESC_DTYPE
+    if not (torch.is_tensor(src) and src.is_cuda and src.dtype == torch.uint8 and src.is_contiguous()
+            and src.dim() == 1):
+        raise ValueError("resize_crop_fill: src must be a contiguous 1-D CUDA uint8 tensor")
+    descs = np.ascontiguousarray(descs, dtype=RESIZE_DESC_DTYPE).reshape(-1)
+    n = int(descs.shape[0])
+    if out is None:
+        out = torch.empty((n, IMAGE_SIZE, IMAGE_SIZE, 3), device=src.device, dtype=torch.uint8)
+    elif _device_tiles(out, "out") != n or out.device != src.device:
+        raise ValueError(f"resize_crop_fill: out must be [{n},224,224,3] on {src.device}")
+    if n:
+        with torch.cuda.device(src.device):
+            _check_args(lib().plip_resize_crop_fill_u8(src.data_ptr(), int(src.numel()), descs.ctypes.data, n,
+                                                       out.data_ptr(), torch.cuda.current_stream(src.device).cuda_stream),
+                        "plip_resize_crop_fill_u8")
+    return out
+
+
+@torch.no_grad()
+def mask_value_sets(masks: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The byte values present in every (image, channel) of a contiguous CUDA uint8 ``[n, h, w, c]`` array (``c`` 1..8)
+    as 256-bit sets: int32 ``[n, c, 8]`` on the same device (the bits of uint32 words; bit ``v & 31`` of word ``v >> 5``
+    is value ``v``), one pass over the array (``plip_mask_value_sets_u8``).  ``out``: a contiguous int32 ``[n, c, 8]``
+    tensor to fill.  Needs no engine."""
+    if not (torch.is_tensor(masks) and masks.is_cuda and masks.dtype == torch.uint8 and masks.dim() == 4
+            and masks.is_contiguous()):
+        raise ValueError("mask_value_sets: masks must be a contiguous CUDA uint8 [n, h, w, c] tensor")
+    n, h, w, c = (int(x) for x in masks.shape)
+    if out is None:
+        out = torch.empty((n, c, 8), dtype=torch.int32, device=masks.device)
+    elif not (out.is_cuda and out.dtype == torch.int32 and tuple(out.shape) == (n, c, 8) and out.is_contiguous()
+              and out.device == masks.device):
+        raise ValueError(f"mask_value_sets: out must be a contiguous int32 [{n}, {c}, 8] tensor on {masks.device}")
+    if n:
+        with torch.cuda.device(masks.device):
+            _check_args(lib().plip_mask_value_sets_u8(masks.data_ptr(), n, h, w, c, out.data_ptr(),
+                                                      torch.cuda.current_stream(masks.device).cuda_stream),
+                        "plip_mask_value_sets_u8")
+    return out
+
+
+@torch.no_grad()
 def warp_tiles(tiles: torch.Tensor, params: np.ndarray, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Flip / affine / perspective warps of CUDA uint8 tiles ``[n,224,224,3]``, bit-identical to Pillow's
     ``Image.transpose`` and ``Image.transform(AFFINE | PERSPECTIVE, BILINEAR, fillcolor)`` (``plip_warp_tiles_u8``).

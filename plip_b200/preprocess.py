@@ -78,9 +78,15 @@ def device_resizable(w: int, h: int, size: int = SIZE) -> bool:
     """Whether ``plip_resize_crop_u8`` takes a ``w x h`` image: its filter banks (224 horizontal + 32 vertical rows of
     ``2*ceil(2*scale)+1`` taps, padded to 4) plus one output row's strip of source rows must fit 200 KB of shared
     memory — shortest edges up to ~6,000 px at ordinary aspect ratios.  Larger images go through PIL."""
-    import math
     nw, nh, _, _ = resize_plan(w, h, size)
-    if min(w, h) < 1 or max(w, h) > 65536 or max(nw, nh) > 65536:
+    return resize_fits_device(w, h, nw, nh, size)
+
+
+def resize_fits_device(w: int, h: int, nw: int, nh: int, size: int = SIZE) -> bool:
+    """Whether the tile resize kernels take a ``w x h`` image resized to ``nw x nh`` (sizes 1..65536; the shared-memory
+    plan of :func:`device_resizable`)."""
+    import math
+    if min(w, h, nw, nh) < 1 or max(w, h, nw, nh) > 65536:
         return False
 
     def taps4(i, o):

@@ -163,3 +163,80 @@ def token_ids(n: int, seed: int = 1235, full_length: bool = False, min_len: int 
     ids = torch.where(ar >= (lens[:, None] - 1), torch.full_like(ids, EOS), ids)
     mask = (ar < lens[:, None]).to(torch.int64)
     return ids, mask
+
+
+# The 19 tissue types of PanNuke's types.npy.
+PANNUKE_TISSUES = ("Adrenal_gland", "Bile-duct", "Bladder", "Breast", "Cervix", "Colon", "Esophagus", "HeadNeck",
+                   "Kidney", "Liver", "Lung", "Ovarian", "Pancreatic", "Prostate", "Skin", "Stomach", "Testis",
+                   "Thyroid", "Uterus")
+
+
+def _pannuke_counts(rng: np.random.Generator, n: int) -> list:
+    """Per image, the nucleus instances of channels 0..4 and what the rest of the mask does: the labelling rule's
+    edge cases first (in a fixed rotation), then random draws."""
+    cases = [
+        dict(counts=(0, 0, 0, 0, 0)),                          # no cells: dropped
+        dict(counts=(10, 5, 5, 7, 5)),                         # n0 = 10, 10 / 33 > 0.3 (with channel 5's id)
+        dict(counts=(10, 5, 5, 8, 5)),                         # n0 = 10, 10 / 34 < 0.3
+        dict(counts=(9, 2, 0, 0, 0)),                          # n0 = 9: neither malignant nor benign
+        dict(counts=(0, 4, 3, 0, 2)),                          # benign
+        dict(counts=(12, 3, 0, 0, 0), big_ids=True),           # float ids past 255 (they wrap in the uint8 cast)
+        dict(counts=(0, 3, 2, 0, 0), no_zero=1),               # channel 1 has no zero anywhere
+        dict(counts=(15, 0, 0, 2, 0), background=False),       # channel 5 all zero
+        dict(counts=(0, 0, 0, 0, 0), background=False, no_zero=5),  # background only: dropped
+    ]
+    out = [cases[i] if i < len(cases) else None for i in range(n)]
+    for i in range(len(cases), n):
+        kind = rng.integers(0, 3)
+        n0 = (0, int(rng.integers(1, 10)), int(rng.integers(10, 20)))[kind]
+        out[i] = dict(counts=(n0, *(int(x) for x in rng.integers(0, 8, size=4))), big_ids=bool(rng.integers(0, 4) == 0),
+                      background=bool(rng.integers(0, 5) != 0))
+    return out
+
+
+def make_pannuke_folds(seed: int = 0, sizes=(20, 16, 12), size: int = 256, dtype=np.float64):
+    """Seeded synthetic PanNuke folds: a list of ``(images [n, size, size, 3], masks [n, size, size, 6], types [n])``
+    as ``np.load`` returns PanNuke's ``images.npy`` / ``masks.npy`` / ``types.npy`` (float64 arrays, ``<U`` types).
+
+    Every mask channel 0..4 holds a drawn number of nucleus instances as disks of distinct ids, each in its own cell
+    of a 6 x 6 grid while the cells last (so the edge cases' counts are exact); channel 5 is 1 where no nucleus is (the background channel) or all
+    zero.  The first images of each fold are the labelling rule's edge cases (no cells, ``n0 = 10`` at ratios just
+    above and below 0.3, ``n0 = 9``, ids past 255, a channel without a zero, channel 5 empty); every one of the 19
+    tissue strings occurs.  ``dtype``: of the image and mask arrays (``np.uint8`` for large runs)."""
+    rng = np.random.default_rng(seed)
+    grid = 6
+    cell = size // grid
+    yy, xx = np.mgrid[0:cell, 0:cell]
+    folds = []
+    tissue_at = 0
+    for n in sizes:
+        images = np.empty((n, size, size, 3), dtype=dtype)
+        masks = np.zeros((n, size, size, 6), dtype=dtype)
+        types = []
+        for i, spec in enumerate(_pannuke_counts(rng, n)):
+            base = rng.integers(120, 230, size=3)
+            img = base + rng.integers(-25, 26, size=(size, size, 3))
+            slots = rng.permutation(grid * grid)
+            s = 0
+            for ch, cnt in enumerate(spec["counts"]):
+                ids = rng.choice(np.arange(1, 600 if spec.get("big_ids") else 250), size=cnt, replace=False)
+                for inst in ids:
+                    cy, cx = divmod(int(slots[s % (grid * grid)]), grid)
+                    s += 1
+                    r = int(rng.integers(3, cell // 2))
+                    disk = (yy - cell // 2) ** 2 + (xx - cell // 2) ** 2 <= r * r
+                    tile = masks[i, cy * cell:(cy + 1) * cell, cx * cell:(cx + 1) * cell, ch]
+                    tile[disk] = inst
+                    img[cy * cell:(cy + 1) * cell, cx * cell:(cx + 1) * cell][disk] -= 60 + 20 * ch
+            if "no_zero" in spec:
+                ch = spec["no_zero"]
+                masks[i, ..., ch][masks[i, ..., ch] == 0] = 7
+            if spec.get("background", True):
+                masks[i, ..., 5] = np.all(masks[i, ..., :5] == 0, axis=-1)
+            images[i] = np.clip(img, 0, 255)
+            # every tissue once, then mostly the first four, so that some (tissue, label) subsets split
+            types.append(PANNUKE_TISSUES[tissue_at] if tissue_at < len(PANNUKE_TISSUES) else
+                         PANNUKE_TISSUES[int(rng.integers(0, 4))])
+            tissue_at += 1
+        folds.append((images, masks, np.array(types)))
+    return folds
