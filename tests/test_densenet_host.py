@@ -36,7 +36,9 @@ def test_weights_checksum_and_bn_statistics(sd, golden):
 def test_oracle_matches_torchvision_golden(sd, golden):
     out = O.forward_u8(sd, torch.from_numpy(golden["tiles"]))
     ref = torch.from_numpy(golden["outputs"])
-    assert torch.allclose(out, ref, rtol=1e-4, atol=1e-4 * ref.abs().max().item())
+    # two fp32 evaluations of the same network that differ only in their convolution algorithms: 1.8e-5 apart at
+    # most on these features (largest 17), far inside 1e-4 per element
+    assert torch.allclose(out, ref, rtol=1e-4, atol=1e-4)
 
 
 def test_emulation_is_close_to_fp32(sd, golden):

@@ -1,7 +1,6 @@
-"""MuDiPath DenseNet-121 on the GPU: every kernel against a float64 restatement on identical bf16 operands, the whole
+"""MuDiPath DenseNet-121 on the GPU: every kernel against its float64 contract (densenet_contract.py), the whole
 network against the fp32 oracle (bound from the bf16 emulation) and the torchvision golden outputs, and the
 ``mudipath`` branch of ``EmbedderFactory``."""
-import ctypes as C
 import os
 from argparse import Namespace
 
@@ -10,6 +9,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import densenet_contract as C
 import densenet_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -63,14 +63,6 @@ def _bf_rand(shape, g, scale=1.0):
     return (scale * torch.randn(shape, generator=g)).to(torch.bfloat16).cuda()
 
 
-def _close_bf16(out, ref):
-    """Outputs rounded to bf16 from a different fp32 summation order: 1 bf16 ulp of each element plus a hair."""
-    out, ref = out.double(), ref.double()
-    tol = ref.abs() * 2.0 ** -7 + 1e-4 * ref.abs().max()
-    bad = (out - ref).abs() > tol
-    assert not bad.any(), f"{int(bad.sum())} of {bad.numel()} differ; max {(out - ref).abs().max().item():.3e}"
-
-
 def test_stem_with_padded_corners(L):
     g = torch.Generator().manual_seed(1)
     n = 2
@@ -79,14 +71,16 @@ def test_stem_with_padded_corners(L):
     tiles[:, -8:, -8:] = 0
     w4 = (0.1 * torch.randn(64, 3, 7, 7, generator=g)).to(torch.bfloat16)
     wk = torch.zeros(64, 160, dtype=torch.bfloat16)
-    wk[:, :147] = w4.permute(0, 2, 3, 1).reshape(64, 147)
+    wk[:, :147] = C.conv_weight_k(w4)
     s, b = _bn(64, g)
     out = torch.empty(n * 112 * 112, 64, dtype=torch.bfloat16, device="cuda")
     _op(L, 0, tiles.cuda(), 0, n, 112, 3, wk.cuda(), None, None, s, b, out, 64)
-    x = O.normalize_u8(tiles).to(torch.bfloat16).double().cuda()
-    y = F.conv2d(x, w4.double().cuda(), stride=2, padding=3)
-    ref = torch.relu(y * s.double().view(1, -1, 1, 1) + b.double().view(1, -1, 1, 1)).permute(0, 2, 3, 1)
-    _close_bf16(out.view(n, 112, 112, 64), ref)
+    acc, slack = C.acc_ref(C.stem_a(tiles.cuda()), wk.cuda())
+    ref, sl, pre = C.bn_relu_ref(acc, slack, s, b)
+    C.check_out(out, ref, sl, "densenet stem (kAStem, kEpiBnRelu)", "stem, padded corners", pre)
+    # the contract's operand is the emulation's normalised input, and its accumulator F.conv2d's
+    y = F.conv2d(O.normalize_u8(tiles).to(torch.bfloat16).double().cuda(), w4.double().cuda(), stride=2, padding=3)
+    assert torch.allclose(acc, y.permute(0, 2, 3, 1).reshape(-1, 64), rtol=0, atol=1e-12)
 
 
 def test_maxpool_exact(L):
@@ -111,9 +105,9 @@ def test_conv1_preactivation(L, c_in, side, lda):
     e_s, e_b = _bn(128, g)
     out = torch.empty(n * side * side, 128, dtype=torch.bfloat16, device="cuda")
     _op(L, 2, x, lda, n, side, c_in, w, a_s, a_b, e_s, e_b, out, 128)
-    a = torch.relu(x[..., :c_in].float().reshape(-1, c_in) * a_s + a_b).to(torch.bfloat16).double()
-    acc = a @ w.double().t()
-    _close_bf16(out, torch.relu(acc * e_s.double() + e_b.double()))
+    acc, slack = C.acc_ref(C.preact_a(x.view(-1, lda), c_in, a_s, a_b), w)
+    ref, sl, pre = C.bn_relu_ref(acc, slack, e_s, e_b)
+    C.check_out(out, ref, sl, "densenet conv1 (kAPreact, kEpiBnRelu)", f"conv1 c_in={c_in} side={side}", pre)
 
 
 @pytest.mark.parametrize("side", [56, 28, 14, 7])
@@ -122,12 +116,14 @@ def test_conv2_3x3_borders(L, side):
     n = 3
     x = torch.relu(_bf_rand((n, side, side, 128), g))
     w4 = _bf_rand((32, 128, 3, 3), g, 1152 ** -0.5)
-    wk = w4.permute(0, 2, 3, 1).reshape(32, 1152).contiguous()
+    wk = C.conv_weight_k(w4).contiguous()
     ldo = 64
     out = torch.zeros(n * side * side, ldo, dtype=torch.bfloat16, device="cuda")
     _op(L, 3, x, 128, n, side, 128, wk, None, None, None, None, out, ldo)
+    acc, slack = C.acc_ref(C.tap3_a(x), wk)
+    C.check_out(out[:, :32], acc, slack, "densenet conv2 (kATap3, kEpiStore)", f"conv2 side={side}")
     ref = F.conv2d(x.permute(0, 3, 1, 2).double(), w4.double(), padding=1).permute(0, 2, 3, 1).reshape(-1, 32)
-    _close_bf16(out[:, :32], ref)
+    assert torch.allclose(acc, ref, rtol=0, atol=1e-12)
     assert not out[:, 32:].any()
 
 
@@ -140,10 +136,8 @@ def test_transition_pool_first(L, c_in, side):
     a_s, a_b = _bn(c_in, g)
     out = torch.empty(n * side * side, c_in // 2, dtype=torch.bfloat16, device="cuda")
     _op(L, 4, x, c_in, n, side, c_in, w, a_s, a_b, None, None, out, c_in // 2)
-    r = torch.relu(x.float() * a_s + a_b)
-    p = ((r[:, 0::2, 0::2] + r[:, 0::2, 1::2]) + r[:, 1::2, 0::2]) + r[:, 1::2, 1::2]
-    a = (p * 0.25).to(torch.bfloat16).double().reshape(-1, c_in)
-    _close_bf16(out, a @ w.double().t())
+    acc, slack = C.acc_ref(C.pool_a(x, c_in, a_s, a_b), w)
+    C.check_out(out, acc, slack, "densenet transition (kAPool, kEpiStore)", f"transition c_in={c_in}")
 
 
 def test_tail(L):
@@ -153,8 +147,7 @@ def test_tail(L):
     s, b = _bn(1024, g)
     out = torch.empty(n, 1024, dtype=torch.float32, device="cuda")
     _op(L, 5, x, 1024, n, 7, 1024, None, None, None, s, b, out, 1024)
-    ref = x.double().mean(1) * s.double() + b.double()
-    assert torch.allclose(out.double(), ref, rtol=1e-5, atol=1e-5)
+    assert torch.equal(out.cpu(), C.tail_ref(x.cpu(), s.cpu(), b.cpu()))   # the kernel's fp32 order, bit for bit
 
 
 def _network_tiles(n, seed=11):
