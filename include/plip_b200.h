@@ -32,7 +32,7 @@ extern "C" {
 
 #define PLIP_API __attribute__((visibility("default")))
 
-#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts, plip_window_mask_counts, plip_resize_region_*, plip_resize_filter_bounds, plip_sgd_*, plip_linear_decision, plip_densenet_*, plip_resize_crop_bilinear_u8, plip_warp_tiles_u8, plip_resize_crop_fill_u8, plip_mask_value_sets_u8 (new symbols only) */
+#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts, plip_window_mask_counts, plip_resize_region_*, plip_resize_filter_bounds, plip_sgd_*, plip_linear_decision, plip_densenet_*, plip_resize_crop_bilinear_u8, plip_warp_tiles_u8, plip_resize_crop_fill_u8, plip_mask_value_sets_u8, plip_encode_pair (new symbols only) */
 
 /* Model constants (TF:configuration_clip.py:47-64,97-109,160-161). */
 #define PLIP_IMAGE_SIZE 224
@@ -93,7 +93,9 @@ PLIP_API uint64_t plip_weights_blob_bytes(void);
 /* ---- engine lifetime ----------------------------------------------------------------------- */
 /* host_blob: packed weights (layout above), plus exp(logit_scale) passed separately.
  * max_micro_batch: largest number of images / captions processed per internal pass; larger calls
- * are looped in micro-batches.  Device memory: blob + plip_workspace_bytes(max_micro_batch). */
+ * are looped in micro-batches.  Device memory: blob + plip_workspace_bytes(max_micro_batch), and from the first
+ * plip_encode_pair call that runs both towers at once a second, text-only workspace (the text tower's activations
+ * while the vision tower's occupy the first): about 0.87 MB per unit of max_micro_batch, 0.9 GB at 1024. */
 PLIP_API int plip_create(const void* host_blob, uint64_t blob_bytes, float logit_scale_exp, int device,
                          int max_micro_batch, plip_engine_t** out);
 /* Same with an explicit operand format: the 16-bit entries of host_blob must have been packed in that format. */
@@ -182,6 +184,16 @@ PLIP_API int plip_encode_text(plip_engine_t* e, const void* ids_dev, int ids_dty
 PLIP_API int plip_encode_text_prefix(plip_engine_t* e, const void* ids_dev, int ids_dtype,
                                      const void* attention_mask_dev, int64_t n, int seq_len, int prefix_len,
                                      float* out_dev, int normalize, void* stream);
+
+/* Both towers: n_img 224 x 224 images (plip_encode_images' formats) -> img_out_dev [n_img,512] and n_txt captions
+ * (plip_encode_text's arguments) -> txt_out_dev [n_txt,512], bit for bit what those two calls return.  When each side
+ * fits one micro-batch and is larger than the graph-replayed small batches (PLIP_GRAPH_MAX), the text tower runs on
+ * the engine's own stream and workspace at the same time as the vision tower on `stream`, so each tower's kernels fill
+ * the SMs the other's leave idle at kernel tails and between launches; `stream` waits for both.  Otherwise it makes
+ * the two calls, text first. */
+PLIP_API int plip_encode_pair(plip_engine_t* e, const void* pixels_dev, int pixel_format, int64_t n_img,
+                              const void* ids_dev, int ids_dtype, const void* attention_mask_dev, int64_t n_txt,
+                              int seq_len, float* img_out_dev, float* txt_out_dev, int normalize, void* stream);
 
 /* ---- per-token outputs: output_hidden_states / output_attentions ------------------------------ */
 /* Device buffers (float32, caller-owned) filled by ONE pass of a tower: CLIPModel.vision_model(...) /

@@ -100,6 +100,7 @@ SIGNATURES = {
     "plip_window_background_counts": (_i, [_vp, _i, _i, _i64, _vp, _i64, _i, _vp, _vp]),
     "plip_encode_text": (_i, [_vp, _vp, _i, _vp, _i64, _i, _fp, _i, _vp]),
     "plip_encode_text_prefix": (_i, [_vp, _vp, _i, _vp, _i64, _i, _i, _fp, _i, _vp]),
+    "plip_encode_pair": (_i, [_vp, _vp, _i, _i64, _vp, _i, _vp, _i64, _i, _fp, _fp, _i, _vp]),
     "plip_vision_outputs": (_i, [_vp, _vp, _i, _i64, _i, _i, C.POINTER(TowerOutputs), _vp]),
     "plip_text_outputs": (_i, [_vp, _vp, _i, _vp, _i64, _i, C.POINTER(TowerOutputs), _vp]),
     "plip_similarity": (_i, [_fp, _i64, _fp, _i64, _f, _i, _i, _fp, _i64, _vp]),

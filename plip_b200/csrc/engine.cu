@@ -159,6 +159,19 @@ struct GraphKey {
   bool operator<(const GraphKey& o) const { return fields() < o.fields(); }
 };
 
+// One tower's activations: what a forward pass writes besides its outputs.
+struct Workspace {
+  float* X = nullptr;            // residual stream fp32 [rows, D]
+  __nv_bfloat16* Xn = nullptr;   // bf16 copy of the residual stream (A operand of the LN-folded GEMMs) [rows, D]
+  __nv_bfloat16* AO = nullptr;   // attention output [rows, D]
+  float2* stats = nullptr;       // per-row (sum, sumsq) partials of X [rows, kStatSlots]
+  __nv_bfloat16* QKV = nullptr;  // [rows, 3D]
+  __nv_bfloat16* H = nullptr;    // fc1 output [rows, FF]; aliases the im2col matrix [mb*49, 3072]
+  __nv_bfloat16* pooled = nullptr;  // [mb, 768]
+  int32_t* row_idx = nullptr;       // [mb] EOS rows
+  int32_t* kmask = nullptr;         // [mb*77] key padding mask
+};
+
 struct Graph {
   cudaGraphExec_t exec = nullptr;
   unsigned long long kernels = 0;  // kernel nodes: what one replay adds to g_launch_count
@@ -185,16 +198,11 @@ struct plip_engine {
   // text
   const float *t_tok = nullptr, *t_pos = nullptr, *t_fin_g = nullptr, *t_fin_b = nullptr;
   const __nv_bfloat16* t_proj = nullptr;
-  // workspace (sized for max_mb)
-  float* X = nullptr;            // residual stream fp32 [rows, D]
-  __nv_bfloat16* Xn = nullptr;   // bf16 copy of the residual stream (A operand of the LN-folded GEMMs) [rows, D]
-  __nv_bfloat16* AO = nullptr;   // attention output [rows, D]
-  float2* stats = nullptr;       // per-row (sum, sumsq) partials of X [rows, kStatSlots]
-  __nv_bfloat16* QKV = nullptr;  // [rows, 3D]
-  __nv_bfloat16* H = nullptr;    // fc1 output [rows, FF]; aliases the im2col matrix [mb*49, 3072]
-  __nv_bfloat16* pooled = nullptr;  // [mb, 768]
-  int32_t* row_idx = nullptr;       // [mb] EOS rows
-  int32_t* kmask = nullptr;         // [mb*77] key padding mask
+  // workspace (sized for max_mb): every call but plip_encode_pair, which runs the vision tower on it and, at the same
+  // time, the text tower on ws_txt (a text-only workspace) and its own stream; all three allocated on its first call
+  Workspace ws, ws_txt;
+  cudaStream_t s_txt = nullptr;
+  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   // last use of the shared workspace through the device-pointer API (any caller stream): the host-buffer
   // path, which runs on the engine's own streams, waits for it before touching the workspace
   cudaEvent_t ev_last = nullptr;
@@ -224,7 +232,7 @@ struct plip_engine {
   // in-step kernel timing (plip_profile_*): a CUDA event pair around every launch of a forward pass, recorded on
   // the launch stream, so bench.py can report each kernel's average duration INSIDE the step it belongs to
   bool prof_on = false;
-  int prof_tower = 0;  // 0 vision, 1 text (set by the forward that is running)
+  int prof_tower = 0;  // 0 vision, 1 text (set by the stage that is running)
   std::vector<cudaEvent_t> prof_ev;    // event pool, two per recorded launch
   struct ProfRec { int kind; int tower; double flops, bytes; };
   std::vector<ProfRec> prof_rec;
@@ -290,8 +298,9 @@ struct WsLayout {
   size_t x, xn, ao, stats, qkv, h, pooled, rowidx, kmask, total;
 };
 
-WsLayout ws_layout(int mb) {
-  const size_t rv = (size_t)mb * kVisSeq, rt = (size_t)mb * kTxtSeq;
+// vision false: a text tower's workspace alone (plip_encode_pair's second one)
+WsLayout ws_layout(int mb, bool vision = true) {
+  const size_t rv = vision ? (size_t)mb * kVisSeq : 0, rt = (size_t)mb * kTxtSeq;
   auto mx = [](size_t a, size_t b) { return a > b ? a : b; };
   auto al = [](size_t a) { return (a + 1023) & ~(size_t)1023; };
   WsLayout w;
@@ -301,12 +310,27 @@ WsLayout ws_layout(int mb) {
   w.ao = off; off += al(mx(rv * kVisDim, rt * kTxtDim) * 2);
   w.stats = off; off += al(mx(rv, rt) * kStatSlots * sizeof(float2));
   w.qkv = off; off += al(mx(rv * 3 * kVisDim, rt * 3 * kTxtDim) * 2);
-  w.h = off; off += al(mx(mx(rv * kVisFF, rt * kTxtFF), (size_t)mb * kPatches * kPatchK) * 2);
+  w.h = off; off += al(mx(mx(rv * kVisFF, rt * kTxtFF), vision ? (size_t)mb * kPatches * kPatchK : 0) * 2);
   w.pooled = off; off += al((size_t)mb * kVisDim * 2);
   w.rowidx = off; off += al((size_t)mb * 4);
   w.kmask = off; off += al(rt * 4);
   w.total = off;
   return w;
+}
+
+// The buffers of a workspace laid out at `base`.
+Workspace bind_workspace(uint8_t* base, const WsLayout& w) {
+  Workspace ws;
+  ws.X = reinterpret_cast<float*>(base + w.x);
+  ws.Xn = reinterpret_cast<__nv_bfloat16*>(base + w.xn);
+  ws.AO = reinterpret_cast<__nv_bfloat16*>(base + w.ao);
+  ws.stats = reinterpret_cast<float2*>(base + w.stats);
+  ws.QKV = reinterpret_cast<__nv_bfloat16*>(base + w.qkv);
+  ws.H = reinterpret_cast<__nv_bfloat16*>(base + w.h);
+  ws.pooled = reinterpret_cast<__nv_bfloat16*>(base + w.pooled);
+  ws.row_idx = reinterpret_cast<int32_t*>(base + w.rowidx);
+  ws.kmask = reinterpret_cast<int32_t*>(base + w.kmask);
+  return ws;
 }
 
 // One GEMM of a forward pass in the engine's operand format, profiled as `kind` with its algorithmic work
@@ -320,26 +344,103 @@ int gemm(plip_engine* e, int kind, GemmArgs g, cudaStream_t st) {
   return launch_gemm(g, st);
 }
 
-// The rest of an encoder layer after attention, on `rows` rows of the attention output `ao` and the fp32 residual
-// stream `x`:  x = x + out_proj(ao);  x = x + fc2(quick_gelu(fc1(LN2(x))))            TF:modeling_clip.py:370-382
-// The residual GEMMs leave Xn / stats (the input of the next LayerNorm-folded GEMM) and the number of statistics
-// partials in np; the last layer's fc2 does not, its output only feeds the pooled-row LayerNorm (fp32 x).
-int layer_tail(plip_engine* e, const LayerW& w, int rows, int D, int FF, const __nv_bfloat16* ao, float* x, bool last,
-               int& np, cudaStream_t st) {
+// One tower's pass through its encoder layers: weights, workspace and shapes.  np is the number of statistics partials
+// the last residual GEMM left in w.stats.  The stages below are the launches of one layer, in order:
+//   qkv(l) -> attn(l) -> out(l) -> fc1(l) -> fc2(l)                         TF:modeling_clip.py:370-382
+struct Tower {
+  int id;  // 0 vision, 1 text (profiling)
+  const LayerW* L;
+  Workspace w;
+  int64_t n_seq;
+  int S, D, FF, heads;
+  bool causal;
+  const int32_t* kmask;
+  int np;
+  int64_t rows() const { return n_seq * S; }
+};
+
+Tower vision_tower(const plip_engine* e, const Workspace& w, int64_t mb, int S) {
+  return Tower{0, e->vis, w, mb, S, kVisDim, kVisFF, kVisHeads, false, nullptr, 1};
+}
+
+Tower text_tower(const plip_engine* e, const Workspace& w, int64_t mb, int S, const int32_t* kmask) {
+  return Tower{1, e->txt, w, mb, S, kTxtDim, kTxtFF, kTxtHeads, true, kmask, 1};
+}
+
+// Xn / stats derived from X: on entry to the layers, X holds the residual stream.
+int stage_rowstats(plip_engine* e, Tower& t, cudaStream_t st) {
+  e->prof_tower = t.id;
+  const int64_t M = t.rows();
+  ProfScope ps(e, st, PK_ROWSTATS, 0, (double)M * t.D * 6 + (double)M * 8);
+  t.np = 1;
+  return launch_rowstats_cast(t.w.X, M, t.D, t.w.Xn, t.w.stats, e->f16, st);
+}
+
+// LN1 + q/k/v projection
+GemmArgs qkv_args(const Tower& t, int l) {
+  const LayerW& w = t.L[l];
   GemmArgs g;
-  g.A = ao; g.lda = D; g.W = w.wo; g.ldw = D; g.M = rows; g.N = D; g.K = D;
-  g.bias = w.bo; g.out = x; g.ldo = D; g.epi = EPI_BIAS_RESID_F32;
-  g.xb_out = e->Xn; g.stats_out = e->stats; g.n_tiles_used = &np;
-  if (int rc = gemm(e, PK_OUT, g, st)) return rc;
-  g = GemmArgs();
-  g.A = e->Xn; g.lda = D; g.W = w.w1; g.ldw = D; g.M = rows; g.N = FF; g.K = D;
-  g.bias = w.b1; g.colsum = w.s1; g.stats_in = e->stats; g.n_partials = np;
-  g.out = e->H; g.ldo = FF; g.epi = EPI_LN_BIAS_GELU_BF16;
-  if (int rc = gemm(e, PK_FC1, g, st)) return rc;
-  g = GemmArgs();
-  g.A = e->H; g.lda = FF; g.W = w.w2; g.ldw = FF; g.M = rows; g.N = D; g.K = FF;
-  g.bias = w.b2; g.out = x; g.ldo = D; g.epi = EPI_BIAS_RESID_F32;
-  if (!last) { g.xb_out = e->Xn; g.stats_out = e->stats; g.n_tiles_used = &np; }
+  g.A = t.w.Xn; g.lda = t.D; g.W = w.wqkv; g.ldw = t.D; g.M = (int)t.rows(); g.N = 3 * t.D; g.K = t.D;
+  g.bias = w.bqkv; g.colsum = w.sqkv; g.stats_in = t.w.stats; g.n_partials = t.np;
+  g.out = t.w.QKV; g.ldo = 3 * t.D; g.epi = EPI_LN_BIAS_BF16;
+  return g;
+}
+
+// x = x + out_proj(ao), leaving Xn / stats for fc1
+GemmArgs out_args(Tower& t, int l) {
+  const LayerW& w = t.L[l];
+  GemmArgs g;
+  g.A = t.w.AO; g.lda = t.D; g.W = w.wo; g.ldw = t.D; g.M = (int)t.rows(); g.N = t.D; g.K = t.D;
+  g.bias = w.bo; g.out = t.w.X; g.ldo = t.D; g.epi = EPI_BIAS_RESID_F32;
+  g.xb_out = t.w.Xn; g.stats_out = t.w.stats; g.n_tiles_used = &t.np;
+  return g;
+}
+
+int stage_qkv(plip_engine* e, Tower& t, int l, cudaStream_t st) {
+  e->prof_tower = t.id;
+  return gemm(e, PK_QKV, qkv_args(t, l), st);
+}
+
+// attention of layer l; with attn, its probabilities as well (reads Q and K of QKV, intact until the next layer's QKV
+// GEMM, writes heads * S^2 fp32 per sequence)
+int stage_attn(plip_engine* e, Tower& t, int l, float* attn, cudaStream_t st) {
+  e->prof_tower = t.id;
+  const int64_t M = t.rows();
+  const double b_att = (double)M * 3 * t.D * 2 + (double)M * t.D * 2;
+  const double f_att = 4.0 * (double)t.n_seq * t.heads * t.S * t.S * kHeadDim;
+  {
+    ProfScope ps(e, st, t.S > 128 ? PK_ATTN_LONG : PK_ATTN, f_att, b_att);
+    if (int rc = launch_attention(t.w.QKV, t.n_seq, t.S, t.heads, t.causal, t.kmask, t.w.AO, e->f16, st)) return rc;
+  }
+  if (!attn) return 0;
+  ProfScope ps(e, st, PK_ATTN_PROBS, 0.5 * f_att, (double)M * 2 * t.D * 2 + (double)t.n_seq * t.heads * t.S * t.S * 4);
+  return launch_attention_probs(t.w.QKV, t.n_seq, t.S, t.heads, t.causal, t.kmask, attn, e->f16, st);
+}
+
+int stage_out(plip_engine* e, Tower& t, int l, cudaStream_t st) {
+  e->prof_tower = t.id;
+  return gemm(e, PK_OUT, out_args(t, l), st);
+}
+
+// LN2 + fc1 + QuickGELU
+int stage_fc1(plip_engine* e, Tower& t, int l, cudaStream_t st) {
+  e->prof_tower = t.id;
+  const LayerW& w = t.L[l];
+  GemmArgs g;
+  g.A = t.w.Xn; g.lda = t.D; g.W = w.w1; g.ldw = t.D; g.M = (int)t.rows(); g.N = t.FF; g.K = t.D;
+  g.bias = w.b1; g.colsum = w.s1; g.stats_in = t.w.stats; g.n_partials = t.np;
+  g.out = t.w.H; g.ldo = t.FF; g.epi = EPI_LN_BIAS_GELU_BF16;
+  return gemm(e, PK_FC1, g, st);
+}
+
+// x = x + fc2(h).  The last layer's fc2 leaves no Xn / stats: its output only feeds the pooled-row LayerNorm (fp32 x).
+int stage_fc2(plip_engine* e, Tower& t, int l, bool last, cudaStream_t st) {
+  e->prof_tower = t.id;
+  const LayerW& w = t.L[l];
+  GemmArgs g;
+  g.A = t.w.H; g.lda = t.FF; g.W = w.w2; g.ldw = t.FF; g.M = (int)t.rows(); g.N = t.D; g.K = t.FF;
+  g.bias = w.b2; g.out = t.w.X; g.ldo = t.D; g.epi = EPI_BIAS_RESID_F32;
+  if (!last) { g.xb_out = t.w.Xn; g.stats_out = t.w.stats; g.n_tiles_used = &t.np; }
   return gemm(e, PK_FC2, g, st);
 }
 
@@ -385,73 +486,57 @@ PassOut embeds_only(float* out, int normalize) {
 // alone (gathered into compact buffers) instead of all n_seq*S rows — same arithmetic per row, identical embeddings.
 // pool_idx: device row indices of the pooled rows (null = row i*S).  A pruned pass sets *pooled_x to the compact fp32
 // [n_seq, D] pooled rows and writes no per-layer outputs.
-int run_layers(plip_engine* e, const LayerW* L, int64_t n_seq, int S, int D, int FF, int heads, bool causal,
-               const int32_t* kmask, int num_layers, cudaStream_t st, bool prune = false,
+int run_layers(plip_engine* e, Tower& t, int num_layers, cudaStream_t st, bool prune = false,
                const int32_t* pool_idx = nullptr, const PassOut& out = PassOut(), const float** pooled_x = nullptr) {
-  const int64_t M = n_seq * S;
+  const int64_t M = t.rows();
   PLIP_REQUIRE(M <= 0x7fffffff / 4, "micro-batch too large");
   PLIP_REQUIRE(!prune || (pooled_x && !out.hidden && !out.attn), "internal: per-layer outputs of a pruned pass");
-  const size_t x_bytes = (size_t)M * D * 4;
-  if (out.hidden) PLIP_CUDA_CHECK(cudaMemcpyAsync(out.hidden, e->X, x_bytes, cudaMemcpyDeviceToDevice, st));
+  const size_t x_bytes = (size_t)M * t.D * 4;
+  if (out.hidden) PLIP_CUDA_CHECK(cudaMemcpyAsync(out.hidden, t.w.X, x_bytes, cudaMemcpyDeviceToDevice, st));
   if (num_layers <= 0) return 0;
-  {
-    ProfScope ps(e, st, PK_ROWSTATS, 0, (double)M * D * 6 + (double)M * 8);
-    if (int rc = launch_rowstats_cast(e->X, M, D, e->Xn, e->stats, e->f16, st)) return rc;
-  }
-  const double b_att = (double)M * 3 * D * 2 + (double)M * D * 2;
-  const double f_att = 4.0 * (double)n_seq * heads * S * S * kHeadDim;
-  int np = 1;
+  if (int rc = stage_rowstats(e, t, st)) return rc;
   for (int l = 0; l < num_layers; ++l) {
-    const LayerW& w = L[l];
     const bool last = l + 1 == num_layers;
-    // LN1 + q/k/v projection, attention                                   TF:modeling_clip.py:370-376
-    GemmArgs g;
-    g.A = e->Xn; g.lda = D; g.W = w.wqkv; g.ldw = D; g.M = (int)M; g.N = 3 * D; g.K = D;
-    g.bias = w.bqkv; g.colsum = w.sqkv; g.stats_in = e->stats; g.n_partials = np;
-    g.out = e->QKV; g.ldo = 3 * D; g.epi = EPI_LN_BIAS_BF16;
-    if (int rc = gemm(e, PK_QKV, g, st)) return rc;
-    {
-      ProfScope ps(e, st, S > 128 ? PK_ATTN_LONG : PK_ATTN, f_att, b_att);
-      if (int rc = launch_attention(e->QKV, n_seq, S, heads, causal, kmask, e->AO, e->f16, st)) return rc;
-    }
-    if (out.attn) {
-      // reads Q and K of QKV (intact until the next layer's QKV GEMM), writes heads * S^2 fp32 per sequence
-      ProfScope ps(e, st, PK_ATTN_PROBS, 0.5 * f_att, (double)M * 2 * D * 2 + (double)n_seq * heads * S * S * 4);
-      if (int rc = launch_attention_probs(e->QKV, n_seq, S, heads, causal, kmask, out.attn + l * out.attn_stride,
-                                          e->f16, st)) return rc;
-    }
+    if (int rc = stage_qkv(e, t, l, st)) return rc;
+    if (int rc = stage_attn(e, t, l, out.attn ? out.attn + l * out.attn_stride : nullptr, st)) return rc;
     if (!(prune && last)) {
-      if (int rc = layer_tail(e, w, (int)M, D, FF, e->AO, e->X, last, np, st)) return rc;
+      if (int rc = stage_out(e, t, l, st)) return rc;
+      if (int rc = stage_fc1(e, t, l, st)) return rc;
+      if (int rc = stage_fc2(e, t, l, last, st)) return rc;
       if (out.hidden)
-        PLIP_CUDA_CHECK(cudaMemcpyAsync(out.hidden + (l + 1) * out.hidden_stride, e->X, x_bytes,
+        PLIP_CUDA_CHECK(cudaMemcpyAsync(out.hidden + (l + 1) * out.hidden_stride, t.w.X, x_bytes,
                                         cudaMemcpyDeviceToDevice, st));
       continue;
     }
     // compact copies of the pooled rows: attention output -> head of the (now free) QKV buffer, residual rows behind it
-    __nv_bfloat16* ao_p = e->QKV;
-    float* x_p = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(e->QKV) + (((size_t)n_seq * D * 2 + 1023) & ~(size_t)1023));
+    Tower c = t;
+    c.S = 1;
+    c.w.AO = t.w.QKV;
+    c.w.X = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(t.w.QKV) +
+                                     (((size_t)t.n_seq * t.D * 2 + 1023) & ~(size_t)1023));
     {
-      ProfScope ps(e, st, PK_MISC, 0, (double)n_seq * D * 12);
-      if (int rc = launch_gather_rows(e->AO, e->X, pool_idx, S, n_seq, D, ao_p, x_p, st)) return rc;
+      ProfScope ps(e, st, PK_MISC, 0, (double)t.n_seq * t.D * 12);
+      if (int rc = launch_gather_rows(t.w.AO, t.w.X, pool_idx, t.S, t.n_seq, t.D, c.w.AO, c.w.X, st)) return rc;
     }
-    if (int rc = layer_tail(e, w, (int)n_seq, D, FF, ao_p, x_p, true, np, st)) return rc;
-    *pooled_x = x_p;
+    if (int rc = stage_out(e, c, l, st)) return rc;
+    if (int rc = stage_fc1(e, c, l, st)) return rc;
+    if (int rc = stage_fc2(e, c, l, true, st)) return rc;
+    *pooled_x = c.w.X;
   }
   return 0;
 }
 
-// Vision tower up to (and including) `num_layers` encoder layers; X holds the residual stream [mb * geo.S, 768].
-int vision_trunk(plip_engine* e, const VisInput& in, int64_t mb, const VisGeom& geo, int num_layers,
-                 cudaStream_t st, bool prune = false, const PassOut& out = PassOut(),
-                 const float** pooled_x = nullptr) {
+// Vision embeddings of mb images: X = pre_layrnorm(patch embeddings + position table, class rows) [mb * geo.S, 768].
+int vision_embed(plip_engine* e, const VisInput& in, int64_t mb, const VisGeom& geo, cudaStream_t st) {
   e->prof_tower = 0;
+  const Workspace& w = e->ws;
   const double dmb = (double)mb;
   const int patches = geo.gh * geo.gw;
   // Position table of the grid.  An interpolated one goes to the QKV buffer, which nothing reads before the first
   // layer's QKV GEMM: [geo.S, 768] fp32 fits, since S <= kVisSeq * max_mb and QKV holds that many rows of 2 x 2304 B.
   const float* pos = e->v_pos;
   if (geo.gh != kGrid || geo.gw != kGrid) {
-    float* table = reinterpret_cast<float*>(e->QKV);
+    float* table = reinterpret_cast<float*>(w.QKV);
     ProfScope ps(e, st, PK_MISC, 0, (double)kVisSeq * kVisDim * 4 + (double)geo.S * kVisDim * 4);
     if (int rc = launch_pos_interp(e->v_pos, geo.gh, geo.gw, table, st)) return rc;
     pos = table;
@@ -459,44 +544,49 @@ int vision_trunk(plip_engine* e, const VisInput& in, int64_t mb, const VisGeom& 
   {
     // windows: fmt is PLIP_PIX_U8_NHWC and geo 224 x 224, so the bytes are those of the same windows as tiles
     ProfScope ps(e, st, PK_IM2COL, 0, dmb * (double)pixel_bytes(in.fmt, geo.H, geo.W) + dmb * patches * kPatchK * 2);
-    const int rc = in.win.region ? launch_window_im2col(in.win, mb, e->H, e->f16, st)
-                                 : launch_im2col(in.pixels, in.fmt, mb, geo.H, geo.W, e->H, e->f16, st);
+    const int rc = in.win.region ? launch_window_im2col(in.win, mb, w.H, e->f16, st)
+                                 : launch_im2col(in.pixels, in.fmt, mb, geo.H, geo.W, w.H, e->f16, st);
     if (rc) return rc;
   }
   GemmArgs g;
-  g.A = e->H; g.lda = kPatchK; g.W = e->v_patch_w; g.ldw = kPatchK;
+  g.A = w.H; g.lda = kPatchK; g.W = e->v_patch_w; g.ldw = kPatchK;
   g.M = (int)(mb * patches); g.N = kVisDim; g.K = kPatchK;
-  g.out = e->X; g.ldo = kVisDim; g.pos = pos; g.patches = patches; g.seq = geo.S; g.epi = EPI_PATCH_F32;
+  g.out = w.X; g.ldo = kVisDim; g.pos = pos; g.patches = patches; g.seq = geo.S; g.epi = EPI_PATCH_F32;
   if (int rc = gemm(e, PK_PATCH, g, st)) return rc;
   {
     ProfScope ps(e, st, PK_MISC, 0, dmb * kVisDim * 4);
-    if (int rc = launch_cls_rows(e->v_cls, pos, mb, geo.S, e->X, st)) return rc;
+    if (int rc = launch_cls_rows(e->v_cls, pos, mb, geo.S, w.X, st)) return rc;
   }
   const int64_t M = mb * geo.S;
-  {
-    ProfScope ps(e, st, PK_LN, 0, (double)M * kVisDim * 8);
-    if (int rc = launch_layernorm(e->X, nullptr, kVisDim, M, kVisDim, e->v_pre_g, e->v_pre_b, e->X, nullptr, e->f16, st)) return rc;
-  }
-  return run_layers(e, e->vis, mb, geo.S, kVisDim, kVisFF, kVisHeads, false, nullptr, num_layers, st, prune, nullptr,
-                    out, pooled_x);
+  ProfScope ps(e, st, PK_LN, 0, (double)M * kVisDim * 8);
+  return launch_layernorm(w.X, nullptr, kVisDim, M, kVisDim, e->v_pre_g, e->v_pre_b, w.X, nullptr, e->f16, st);
+}
+
+// Vision tower up to (and including) `num_layers` encoder layers; X holds the residual stream [mb * geo.S, 768].
+int vision_trunk(plip_engine* e, const VisInput& in, int64_t mb, const VisGeom& geo, int num_layers,
+                 cudaStream_t st, bool prune = false, const PassOut& out = PassOut(),
+                 const float** pooled_x = nullptr) {
+  if (int rc = vision_embed(e, in, mb, geo, st)) return rc;
+  Tower t = vision_tower(e, e->ws, mb, geo.S);
+  return run_layers(e, t, num_layers, st, prune, nullptr, out, pooled_x);
 }
 
 // Tower head: LayerNorm of the pooled rows -> projection [-> L2 normalise].  The pooled rows are the compact
-// pooled_x rows when the last layer was pruned, else rows pool_idx[i] of X (null: row i*S).
+// pooled_x rows when the last layer was pruned, else rows pool_idx[i] of w.X (null: row i*S).
 // pooled_f32 (optional): the LayerNorm-ed pooled rows in fp32 as well, [mb, D] (pooler_output); out null: no projection.
-int pooled_head(plip_engine* e, const float* pooled_x, const int32_t* pool_idx, int64_t mb, int S, int D,
-                const float* gamma, const float* beta, const __nv_bfloat16* proj, float* out, int normalize,
+int pooled_head(plip_engine* e, const Workspace& w, const float* pooled_x, const int32_t* pool_idx, int64_t mb, int S,
+                int D, const float* gamma, const float* beta, const __nv_bfloat16* proj, float* out, int normalize,
                 cudaStream_t st, float* pooled_f32) {
   {
     ProfScope ps(e, st, PK_LN, 0, (double)mb * D * (pooled_f32 ? 10 : 6));
     const bool compact = pooled_x != nullptr;
-    if (int rc = launch_layernorm(compact ? pooled_x : e->X, compact ? nullptr : pool_idx,
+    if (int rc = launch_layernorm(compact ? pooled_x : w.X, compact ? nullptr : pool_idx,
                                   compact || pool_idx ? (int64_t)D : (int64_t)S * D, mb, D, gamma, beta, pooled_f32,
-                                  e->pooled, e->f16, st)) return rc;
+                                  w.pooled, e->f16, st)) return rc;
   }
   if (!out) return 0;
   GemmArgs g;
-  g.A = e->pooled; g.lda = D; g.W = proj; g.ldw = D;
+  g.A = w.pooled; g.lda = D; g.W = proj; g.ldw = D;
   g.M = (int)mb; g.N = kProj; g.K = D; g.out = out; g.ldo = kProj; g.epi = EPI_F32;
   if (int rc = gemm(e, PK_PROJ, g, st)) return rc;
   if (normalize) {
@@ -506,6 +596,13 @@ int pooled_head(plip_engine* e, const float* pooled_x, const int32_t* pool_idx, 
   return 0;
 }
 
+// pooled = post_layernorm(last_hidden_state[:, 0, :])                    TF:modeling_clip.py:685-686
+int vision_head(plip_engine* e, const float* pooled_x, int64_t mb, int S, const PassOut& out, cudaStream_t st) {
+  e->prof_tower = 0;
+  return pooled_head(e, e->ws, pooled_x, nullptr, mb, S, kVisDim, e->v_post_g, e->v_post_b, e->v_proj, out.embeds,
+                     out.normalize, st, out.pooled);
+}
+
 // One vision pass over mb images: the whole tower, then what `out` asks for.  prune: see run_layers (the embedding
 // calls only).  last_hidden_state is the residual stream after the last layer, before post_layernorm (TF:680-686).
 int vision_pass(plip_engine* e, const VisInput& in, int64_t mb, const VisGeom& geo, const PassOut& out, bool prune,
@@ -513,50 +610,88 @@ int vision_pass(plip_engine* e, const VisInput& in, int64_t mb, const VisGeom& g
   const float* pooled_x = nullptr;
   if (int rc = vision_trunk(e, in, mb, geo, kLayers, st, prune, out, &pooled_x)) return rc;
   if (out.last_hidden)
-    PLIP_CUDA_CHECK(cudaMemcpyAsync(out.last_hidden, e->X, (size_t)mb * geo.S * kVisDim * 4, cudaMemcpyDeviceToDevice,
-                                    st));
+    PLIP_CUDA_CHECK(cudaMemcpyAsync(out.last_hidden, e->ws.X, (size_t)mb * geo.S * kVisDim * 4,
+                                    cudaMemcpyDeviceToDevice, st));
   if (!out.embeds && !out.pooled) return 0;
-  // pooled = post_layernorm(last_hidden_state[:, 0, :])                  TF:modeling_clip.py:685-686
-  return pooled_head(e, pooled_x, nullptr, mb, geo.S, kVisDim, e->v_post_g, e->v_post_b, e->v_proj, out.embeds,
-                     out.normalize, st, out.pooled);
+  return vision_head(e, pooled_x, mb, geo.S, out, st);
 }
 
+// Text embeddings of mb captions into w: X = token + position embeddings, the pooled (first EOS) rows, the key mask.
 // S = number of leading token positions actually processed (<= stride, the row length of ids / mask).
 // Causality makes rows after a caption's first EOS irrelevant to its pooled output (TF:571-584), so callers
 // that know the longest caption of the batch may pass a shorter S: same result, proportionally less work.
-int text_trunk(plip_engine* e, const void* ids, int ids_dtype, const void* mask, int64_t mb, int S, int stride,
-               int num_layers, cudaStream_t st, bool prune = false, const PassOut& out = PassOut(),
-               const float** pooled_x = nullptr) {
+// Returns the tower with the mask it needs (null: none).
+int text_embed(plip_engine* e, const Workspace& w, const void* ids, int ids_dtype, const void* mask, int64_t mb, int S,
+               int stride, cudaStream_t st, Tower* t) {
   e->prof_tower = 1;
   {
     ProfScope ps(e, st, PK_EMBED, 0, (double)mb * S * kTxtDim * 8);
-    if (int rc = launch_text_embed(ids, ids_dtype, mb, S, stride, e->t_tok, e->t_pos, e->X, e->row_idx, kEosId, e->text_pool_argmax, st)) return rc;
+    if (int rc = launch_text_embed(ids, ids_dtype, mb, S, stride, e->t_tok, e->t_pos, w.X, w.row_idx, kEosId,
+                                   e->text_pool_argmax, st)) return rc;
   }
   const int32_t* km = nullptr;
   if (mask) {
     ProfScope ps(e, st, PK_MISC, 0, (double)mb * S * 12);
-    if (int rc = launch_mask_to_i32(mask, ids_dtype, mb * S, S, stride, e->kmask, st)) return rc;
-    km = e->kmask;
+    if (int rc = launch_mask_to_i32(mask, ids_dtype, mb * S, S, stride, w.kmask, st)) return rc;
+    km = w.kmask;
   }
-  return run_layers(e, e->txt, mb, S, kTxtDim, kTxtFF, kTxtHeads, true, km, num_layers, st, prune, e->row_idx, out,
-                    pooled_x);
+  *t = text_tower(e, w, mb, S, km);
+  return 0;
 }
 
-// One text pass over mb captions (the first S of `stride` positions), then what `out` asks for.
+int text_trunk(plip_engine* e, const Workspace& w, const void* ids, int ids_dtype, const void* mask, int64_t mb,
+               int S, int stride, int num_layers, cudaStream_t st, bool prune = false, const PassOut& out = PassOut(),
+               const float** pooled_x = nullptr) {
+  Tower t;
+  if (int rc = text_embed(e, w, ids, ids_dtype, mask, mb, S, stride, st, &t)) return rc;
+  return run_layers(e, t, num_layers, st, prune, w.row_idx, out, pooled_x);
+}
+
+// pooled = final_layer_norm(last_hidden_state)[b, first eos]              TF:modeling_clip.py:562-584
+int text_head(plip_engine* e, const Workspace& w, const float* pooled_x, int64_t mb, int S, const PassOut& out,
+              cudaStream_t st) {
+  e->prof_tower = 1;
+  return pooled_head(e, w, pooled_x, w.row_idx, mb, S, kTxtDim, e->t_fin_g, e->t_fin_b, e->t_proj, out.embeds,
+                     out.normalize, st, out.pooled);
+}
+
+// One text pass over mb captions (the first S of `stride` positions) on workspace w, then what `out` asks for.
 // last_hidden_state = final_layer_norm of every row (TF:562).
-int text_pass(plip_engine* e, const void* ids, int ids_dtype, const void* mask, int64_t mb, int S, int stride,
-              const PassOut& out, bool prune, cudaStream_t st) {
+int text_pass(plip_engine* e, const Workspace& w, const void* ids, int ids_dtype, const void* mask, int64_t mb, int S,
+              int stride, const PassOut& out, bool prune, cudaStream_t st) {
   const float* pooled_x = nullptr;
-  if (int rc = text_trunk(e, ids, ids_dtype, mask, mb, S, stride, kLayers, st, prune, out, &pooled_x)) return rc;
+  if (int rc = text_trunk(e, w, ids, ids_dtype, mask, mb, S, stride, kLayers, st, prune, out, &pooled_x)) return rc;
   if (out.last_hidden) {
     ProfScope ps(e, st, PK_LN, 0, (double)mb * S * kTxtDim * 8);
-    if (int rc = launch_layernorm(e->X, nullptr, kTxtDim, mb * S, kTxtDim, e->t_fin_g, e->t_fin_b, out.last_hidden,
+    if (int rc = launch_layernorm(w.X, nullptr, kTxtDim, mb * S, kTxtDim, e->t_fin_g, e->t_fin_b, out.last_hidden,
                                   nullptr, e->f16, st)) return rc;
   }
   if (!out.embeds && !out.pooled) return 0;
-  // pooled = final_layer_norm(last_hidden_state)[b, first eos]            TF:modeling_clip.py:562-584
-  return pooled_head(e, pooled_x, e->row_idx, mb, S, kTxtDim, e->t_fin_g, e->t_fin_b, e->t_proj, out.embeds,
-                     out.normalize, st, out.pooled);
+  return text_head(e, w, pooled_x, mb, S, out, st);
+}
+
+// Both towers of one micro-batch at once: mb_txt captions of seq_len ids on the engine's text stream with the text
+// workspace, mb_img 224 x 224 images on st with the main one, st waiting for the text tower at the end.  Nothing of one
+// tower reads what the other writes, so the two launch sequences may run side by side: a tower's kernels start on the
+// SMs the other tower's kernel leaves at its tail and in the gaps between its launches.  Each kernel does the same
+// work on the same data as in a tower pass of its own, so the embeddings are bit for bit those of the two calls.
+// Profiling runs both on st, one after the other, so that each launch's time is its own.
+int pair_pass(plip_engine* e, const void* pixels, int fmt, int64_t mb_img, const void* ids, int ids_dtype,
+              const void* mask, int64_t mb_txt, int seq_len, float* out_img, float* out_txt, int normalize, bool prune,
+              cudaStream_t st) {
+  cudaStream_t s_txt = st;
+  if (!e->prof_on) {
+    s_txt = e->s_txt;
+    PLIP_CUDA_CHECK(cudaEventRecord(e->ev_fork, st));
+    PLIP_CUDA_CHECK(cudaStreamWaitEvent(s_txt, e->ev_fork, 0));
+  }
+  if (int rc = text_pass(e, e->ws_txt, ids, ids_dtype, mask, mb_txt, seq_len, seq_len, embeds_only(out_txt, normalize),
+                         prune, s_txt)) return rc;
+  if (s_txt != st) PLIP_CUDA_CHECK(cudaEventRecord(e->ev_join, s_txt));
+  if (int rc = vision_pass(e, tiles(pixels, fmt), mb_img, VisGeom(), embeds_only(out_img, normalize), prune, st))
+    return rc;
+  if (s_txt != st) PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_join, 0));
+  return 0;
 }
 
 int ensure_host_path(plip_engine* e) {
@@ -836,8 +971,8 @@ int dbg_hidden_states(const char* fn, plip_engine* e, int tower, const void* in,
                (long long)per_pass);
   return micro_batches(e, n, n, st, [&](int64_t, int64_t) {
     if (int rc = tower == 0 ? vision_trunk(e, tiles(in, fmt), n, geo, num_layers, st)
-                            : text_trunk(e, in, fmt, mask, n, kTxtSeq, kTxtSeq, num_layers, st)) return rc;
-    PLIP_CUDA_CHECK(cudaMemcpyAsync(hidden, e->X, (size_t)n * S * D * 4, cudaMemcpyDeviceToDevice, st));
+                            : text_trunk(e, e->ws, in, fmt, mask, n, kTxtSeq, kTxtSeq, num_layers, st)) return rc;
+    PLIP_CUDA_CHECK(cudaMemcpyAsync(hidden, e->ws.X, (size_t)n * S * D * 4, cudaMemcpyDeviceToDevice, st));
     return 0;
   });
 }
@@ -908,7 +1043,7 @@ PLIP_API int plip_create_ex(const void* host_blob, uint64_t nbytes, float logit_
   cudaError_t ce = cudaEventCreateWithFlags(&e->ev_last, cudaEventDisableTiming);
   if (ce == cudaSuccess) ce = cudaMalloc(&e->d_blob, nbytes);
   if (ce == cudaSuccess) ce = cudaMalloc(&ws, w.total);
-  e->X = reinterpret_cast<float*>(ws);  // workspace base (w.x == 0): what plip_destroy frees
+  e->ws.X = reinterpret_cast<float*>(ws);  // workspace base (w.x == 0): what plip_destroy frees
   if (ce != cudaSuccess) {
     set_last_error("plip_create: allocating %llu (weights) + %llu (workspace) bytes on device %d failed: %s",
                    (unsigned long long)nbytes, (unsigned long long)w.total, device, cudaGetErrorString(ce));
@@ -916,14 +1051,7 @@ PLIP_API int plip_create_ex(const void* host_blob, uint64_t nbytes, float logit_
     plip_destroy(e);
     return -1;
   }
-  e->Xn = reinterpret_cast<__nv_bfloat16*>(ws + w.xn);
-  e->AO = reinterpret_cast<__nv_bfloat16*>(ws + w.ao);
-  e->stats = reinterpret_cast<float2*>(ws + w.stats);
-  e->QKV = reinterpret_cast<__nv_bfloat16*>(ws + w.qkv);
-  e->H = reinterpret_cast<__nv_bfloat16*>(ws + w.h);
-  e->pooled = reinterpret_cast<__nv_bfloat16*>(ws + w.pooled);
-  e->row_idx = reinterpret_cast<int32_t*>(ws + w.rowidx);
-  e->kmask = reinterpret_cast<int32_t*>(ws + w.kmask);
+  e->ws = bind_workspace(ws, w);
   ce = cudaMemcpy(e->d_blob, host_blob, nbytes, cudaMemcpyHostToDevice);
   if (ce != cudaSuccess) {
     set_last_error("plip_create: weight upload failed: %s", cudaGetErrorString(ce));
@@ -943,7 +1071,11 @@ PLIP_API int plip_destroy(plip_engine_t* e) {
   cudaSetDevice(e->device);
   cudaDeviceSynchronize();
   if (e->d_blob) cudaFree(e->d_blob);
-  if (e->X) cudaFree(e->X);  // base of the workspace allocation
+  if (e->ws.X) cudaFree(e->ws.X);  // base of the workspace allocation
+  if (e->ws_txt.X) cudaFree(e->ws_txt.X);
+  if (e->s_txt) cudaStreamDestroy(e->s_txt);
+  if (e->ev_fork) cudaEventDestroy(e->ev_fork);
+  if (e->ev_join) cudaEventDestroy(e->ev_join);
   for (int i = 0; i < 2; ++i) {
     if (e->d_in[i]) cudaFree(e->d_in[i]);
     if (e->h_stage[i]) cudaFreeHost(e->h_stage[i]);
@@ -1104,14 +1236,51 @@ PLIP_API int plip_encode_text_prefix(plip_engine_t* e, const void* ids_dev, int 
                        e->text_pool_argmax, e->prune_last};
     return graph_call(e, key, {{{ids_dev, n * row}, {attention_mask_dev, n * row}}}, out_dev, st,
                       [&](cudaStream_t s, const void* ids, const void* mask, float* out) {
-                        return text_pass(e, ids, ids_dtype, mask, n, prefix_len, seq_len, embeds_only(out, normalize),
+                        return text_pass(e, e->ws, ids, ids_dtype, mask, n, prefix_len, seq_len, embeds_only(out, normalize),
                                          prune, s);
                       });
   }
   return micro_batches(e, n, e->max_mb, st, [&](int64_t i, int64_t mb) {
     const uint8_t* mask = attention_mask_dev ? static_cast<const uint8_t*>(attention_mask_dev) + i * row : nullptr;
-    return text_pass(e, static_cast<const uint8_t*>(ids_dev) + i * row, ids_dtype, mask, mb, prefix_len, seq_len,
+    return text_pass(e, e->ws, static_cast<const uint8_t*>(ids_dev) + i * row, ids_dtype, mask, mb, prefix_len, seq_len,
                      embeds_only(out_dev + i * kProj, normalize), prune, st);
+  });
+}
+
+PLIP_API int plip_encode_pair(plip_engine_t* e, const void* pixels_dev, int pixel_format, int64_t n_img,
+                              const void* ids_dev, int ids_dtype, const void* attention_mask_dev, int64_t n_txt,
+                              int seq_len, float* img_out_dev, float* txt_out_dev, int normalize, void* stream) {
+  if (int rc = check_pixels("plip_encode_pair", e, pixels_dev, img_out_dev, pixel_format, n_img, kImage, kImage))
+    return rc;
+  if (int rc = check_ids("plip_encode_pair", e, ids_dev, txt_out_dev, ids_dtype, n_txt, seq_len, seq_len)) return rc;
+  // One micro-batch of each tower, neither of them small enough for the graph-replayed path: the two calls otherwise
+  // (the text tower first, as the sharded forward orders them).
+  if (n_img > e->max_mb || n_txt > e->max_mb || graph_eligible(e, n_img) || graph_eligible(e, n_txt)) {
+    if (int rc = plip_encode_text(e, ids_dev, ids_dtype, attention_mask_dev, n_txt, seq_len, txt_out_dev, normalize,
+                                  stream)) return rc;
+    return plip_encode_images(e, pixels_dev, pixel_format, n_img, img_out_dev, normalize, stream);
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!e->ws_txt.X) {
+    const WsLayout w = ws_layout(e->max_mb, false);
+    uint8_t* base = nullptr;
+    const cudaError_t ce = cudaMalloc(&base, w.total);
+    if (ce != cudaSuccess) {
+      cudaGetLastError();
+      set_last_error("plip_encode_pair: allocating the %llu-byte text workspace failed: %s",
+                     (unsigned long long)w.total, cudaGetErrorString(ce));
+      return -1;
+    }
+    e->ws_txt = bind_workspace(base, w);
+  }
+  if (!e->s_txt) {
+    PLIP_CUDA_CHECK(cudaStreamCreateWithFlags(&e->s_txt, cudaStreamNonBlocking));
+    PLIP_CUDA_CHECK(cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
+    PLIP_CUDA_CHECK(cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming));
+  }
+  return micro_batches(e, 1, 1, st, [&](int64_t, int64_t) {
+    return pair_pass(e, pixels_dev, pixel_format, n_img, ids_dev, ids_dtype, attention_mask_dev, n_txt, seq_len,
+                     img_out_dev, txt_out_dev, normalize, e->prune_last != 0, st);
   });
 }
 
@@ -1136,7 +1305,7 @@ PLIP_API int plip_text_outputs(plip_engine_t* e, const void* ids_dev, int ids_dt
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   return micro_batches(e, n, e->max_mb, st, [&](int64_t i, int64_t mb) {
     const uint8_t* mask = attention_mask_dev ? static_cast<const uint8_t*>(attention_mask_dev) + i * row : nullptr;
-    return text_pass(e, static_cast<const uint8_t*>(ids_dev) + i * row, ids_dtype, mask, mb, seq_len, seq_len,
+    return text_pass(e, e->ws, static_cast<const uint8_t*>(ids_dev) + i * row, ids_dtype, mask, mb, seq_len, seq_len,
                      pass_out(*outputs, n, i, seq_len, kTxtDim, kTxtHeads), false, st);
   });
 }

@@ -97,9 +97,10 @@ class ShardedCLIP:
     partitioning / gathering; image arguments may be one tensor or an iterable of chunks."""
 
     def __init__(self, encode_images: Callable, encode_text: Callable, similarity: Callable, logit_scale_exp: float,
-                 topk: Optional[Callable] = None):
+                 topk: Optional[Callable] = None, encode_pair: Optional[Callable] = None):
         self.encode_images = encode_images
         self.encode_text = encode_text
+        self.encode_pair = encode_pair  # (pixels, ids) -> (image, text) embeddings, both towers at once
         self.similarity = similarity
         self.topk = topk
         self.logit_scale_exp = float(logit_scale_exp)
@@ -113,12 +114,18 @@ class ShardedCLIP:
                    lambda a, b, s: engine.similarity(a, b, scale=s, normalize_image=False, normalize_text=False),
                    engine.logit_scale_exp,
                    topk=lambda q, sp, k: engine.similarity_topk(q, sp, k, scale=1.0, normalize_query=False,
-                                                                normalize_space=False))
+                                                                normalize_space=False),
+                   encode_pair=lambda x, ids: engine.encode_pair(x, ids, normalize=True))
 
     def clip_forward(self, local_pixels, local_ids):
         """``CLIPModel.forward`` over a batch sharded across the ranks (TF:867-944): returns this rank's row block
         ``logits_per_image[n_local, n_text_total]``.  The text embeddings travel (async all-gather on NCCL's stream)
-        while the vision tower runs, so the exchange and any skew between ranks hide behind ~9 ms of compute."""
+        while the vision tower runs, so the exchange and any skew between ranks hide behind ~9 ms of compute.  On one
+        rank with both inputs single tensors, the two towers run side by side (``encode_pair``) when available."""
+        if self.world_size == 1 and self.encode_pair is not None and torch.is_tensor(local_pixels) \
+                and torch.is_tensor(local_ids):
+            img, txt = self.encode_pair(local_pixels, local_ids)
+            return self.similarity(img, txt, self.logit_scale_exp)
         txt = self.encode_text(local_ids)
         txt_all, work = all_gather_rows_async(txt)
         img = _encode_chunks(self.encode_images, local_pixels)

@@ -196,6 +196,9 @@ class PlipCLIPModel:
                 torch.cuda.current_stream(self.device).wait_event(uploaded)
                 embs.append(self.engine.encode_images(chunk, normalize=True, interpolate_pos_encoding=ipe))
             img = embs[0] if len(embs) == 1 else torch.cat(embs, dim=0)
+        elif not ipe:
+            # both towers side by side (one call each where that does not apply, see Engine.encode_pair)
+            img, txt = self.engine.encode_pair(pixel_values, input_ids, attention_mask, normalize=True)
         else:
             img = self.engine.encode_images(pixel_values, normalize=True, interpolate_pos_encoding=ipe)
             txt = self.engine.encode_text(input_ids, attention_mask, normalize=True)
