@@ -338,10 +338,11 @@ PLIP_API int plip_resize_filter_bounds(int in_size, int out_size, int32_t* bound
 /* ---- linear probe: scikit-learn's SGD logistic regression (no engine) ------------------------- */
 /* The reference's linear probe (reproducibility/evaluation/linear_probing/linear_classifier.py) fits
  * SGDClassifier(loss="log_loss", penalty="l2", class_weight="balanced", learning_rate="optimal") on float32 [n,512]
- * embeddings: one-vs-rest binary problems, each a sequential pass of sklearn 1.9's _plain_sgd (32-bit instantiation)
- * over a shuffled order per epoch.  plip_sgd_fit runs that algorithm, cast for cast, for many binary problems at once
- * (every class of a fit, every alpha of a sweep): one warp per problem runs all its epochs on the device.  The
- * results equal sklearn's up to the order of the 512-term double sums and CUDA's exp / log1p against the C library's.
+ * (PLIP, CLIP) or [n,1024] (MuDiPath's DenseNet-121) embeddings: one-vs-rest binary problems, each a sequential pass
+ * of sklearn 1.9's _plain_sgd (32-bit instantiation) over a shuffled order per epoch.  plip_sgd_fit runs that
+ * algorithm, cast for cast, for many binary problems at once (every class of a fit, every alpha of a sweep): one warp
+ * per problem runs all its epochs on the device.  The results equal sklearn's up to the order of the D-term double
+ * sums (D = dim) and CUDA's exp / log1p against the C library's.
  *
  * One binary problem: labels y = (class_host[i] == pos_class), positive / negative sample weight pos_weight /
  * neg_weight (rounded to float, as sklearn's class_weight local), regularisation alpha (> 0, finite), t starting at 1,
@@ -359,11 +360,11 @@ typedef struct plip_sgd_problem {
 PLIP_API int plip_sgd_shuffle_permutation(int64_t n, uint32_t seed, int32_t* sigma_host);
 /* Device workspace bytes of plip_sgd_fit (problem table, labels, sigma rows and two epoch orders per problem). */
 PLIP_API int plip_sgd_workspace_bytes(int64_t n, int n_sigma, int n_problems, uint64_t* bytes);
-/* x_dev: device float32 [n,512], rows contiguous, 16-byte aligned; 2 <= n < 2^31.  class_host: HOST int32 [n] class ids
- * in 0..n_classes-1.  problems_host: HOST [n_problems].  sigma_host: HOST int32 [n_sigma, n], every entry in 0..n-1.
+/* x_dev: device float32 [n,dim], dim = 512 or 1024, rows contiguous, 16-byte aligned; 2 <= n < 2^31.  class_host:
+ * HOST int32 [n] class ids in 0..n_classes-1.  problems_host: HOST [n_problems].  sigma_host: HOST int32 [n_sigma, n], every entry in 0..n-1.
  * Host arrays are consumed before the call returns.  max_iter >= 1 epochs; an epoch whose mean objective exceeds the
  * best so far minus tol counts towards n_iter_no_change (>= 1) epochs without improvement, which stop the problem
- * (tol = -INFINITY disables the test).  Outputs (device): coef_dev float32 [n_problems,512], intercept_dev float64
+ * (tol = -INFINITY disables the test).  Outputs (device): coef_dev float32 [n_problems,dim], intercept_dev float64
  * [n_problems], n_iter_dev int32 [n_problems] (epochs run), overflow_dev int32 [n_problems]: 1 if the weights or the
  * intercept were not finite at the end of epoch n_iter (sklearn raises there; coef / intercept are then undefined).
  * workspace_dev: 16-byte aligned device memory of at least plip_sgd_workspace_bytes(n, n_sigma, n_problems); the call
@@ -376,8 +377,8 @@ PLIP_API int plip_sgd_fit(const float* x_dev, int64_t n, int dim, const int32_t*
                           uint64_t workspace_bytes, void* stream);
 /* decision_function and predict of a fitted linear classifier: scores_dev float32 [n, n_out] = x . coef^T + intercept
  * (products and sums in double, rounded once), pred_dev int32 [n]: n_out > 1, the first index of the largest score;
- * n_out == 1, 1 where the score is > 0, else 0.  x_dev float32 [n,512] and coef_dev float32 [n_out,512] 16-byte
- * aligned, intercept_dev float64 [n_out].  Stream-ordered, one launch. */
+ * n_out == 1, 1 where the score is > 0, else 0.  x_dev float32 [n,dim] and coef_dev float32 [n_out,dim] (dim =
+ * 512 or 1024) 16-byte aligned, intercept_dev float64 [n_out].  Stream-ordered, one launch. */
 PLIP_API int plip_linear_decision(const float* x_dev, int64_t n, int dim, const float* coef_dev,
                                   const double* intercept_dev, int n_out, float* scores_dev, int32_t* pred_dev,
                                   void* stream);

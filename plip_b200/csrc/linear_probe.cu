@@ -12,8 +12,10 @@
 //     recomputes it right away, here it is taken at the start of the next step, from the same weights);
 //   - runs sklearn's scalar step in fp64, lane-uniform (every lane holds the bit-identical reduced sums: a butterfly
 //     reduction adds the same two values in every lane);
-//   - applies scale / add to its 16 weights (lane l holds elements 4 * (l + 32 k) .. + 3, k = 0..3) with sklearn's
-//     casts: scale takes a float, add takes a float coefficient and divides it by a float copy of wscale.
+//   - applies scale / add to its D / 32 weights (lane l holds elements 4 * (l + 32 k) .. + 3, k = 0..D/128-1) with
+//     sklearn's casts: scale takes a float, add takes a float coefficient and divides it by a float copy of wscale.
+// Both kernels are instantiated for the two embedding widths the reference probes, D = 512 (CLIP) and D = 1024
+// (MuDiPath's DenseNet-121); at 1024 the cp.async ring holds 8 x 4 KB rows, 32 KB of static shared memory.
 // The weights never leave registers until the problem stops.  At the end of an epoch the warp gathers the next order
 // through sigma into its own buffer, checks for non-finite values and runs the stop test itself.
 //
@@ -29,8 +31,9 @@ namespace plip {
 
 namespace {
 
-constexpr int kSgdDim = kProj;                // embedding width
-constexpr int kSgdVec = kSgdDim / (32 * 4);   // float4 per lane
+// The embedding widths a fit runs at: 512 (the CLIP projection) and 1024 (MuDiPath's DenseNet-121 features).
+constexpr int kSgdDimClip = kProj;
+constexpr int kSgdDimDenseNet = 1024;
 constexpr int kRing = 8;                      // rows in flight per problem
 constexpr double kResetWscale = 1e-6;         // WeightVector32
 constexpr double kMaxDloss = 1e12;
@@ -74,13 +77,15 @@ __device__ __forceinline__ double half_binomial_gradient(double y, double p) {
 
 __device__ __forceinline__ float& comp(float4& v, int c) { return c == 0 ? v.x : c == 1 ? v.y : c == 2 ? v.z : v.w; }
 
+template <int D>
 __global__ void __launch_bounds__(32) sgd_fit_kernel(const float* __restrict__ X, int n, const int32_t* __restrict__ cls,
                                                     const SgdProblem* __restrict__ problems,
                                                     const int32_t* __restrict__ sigma, int32_t* orders, int max_iter,
                                                     double tol, int n_iter_no_change, float* __restrict__ coef,
                                                     double* __restrict__ intercept_out, int32_t* __restrict__ n_iter_out,
                                                     int32_t* __restrict__ overflow_out) {
-  __shared__ __align__(16) float4 ring[kRing][kSgdDim / 4];
+  constexpr int kSgdVec = D / (32 * 4);  // float4 per lane
+  __shared__ __align__(16) float4 ring[kRing][D / 4];
   const int lane = threadIdx.x;
   const int pid = blockIdx.x;
   const SgdProblem pr = problems[pid];
@@ -131,7 +136,7 @@ __global__ void __launch_bounds__(32) sgd_fit_kernel(const float* __restrict__ X
       if (s < n) {
         float4* slot = ring[s % kRing];
 #pragma unroll
-        for (int j = 0; j < kSgdVec; ++j) cp_async_16(slot + lane + 32 * j, X4 + (size_t)row * (kSgdDim / 4) + lane + 32 * j);
+        for (int j = 0; j < kSgdVec; ++j) cp_async_16(slot + lane + 32 * j, X4 + (size_t)row * (D / 4) + lane + 32 * j);
       }
       cp_async_commit();
     };
@@ -226,7 +231,7 @@ __global__ void __launch_bounds__(32) sgd_fit_kernel(const float* __restrict__ X
   }
 
   const float s = __double2float_rn(wscale);  // w.reset_wscale
-  float4* out = reinterpret_cast<float4*>(coef + (size_t)pid * kSgdDim);
+  float4* out = reinterpret_cast<float4*>(coef + (size_t)pid * D);
 #pragma unroll
   for (int j = 0; j < kSgdVec; ++j)
     out[lane + 32 * j] = make_float4(__fmul_rn(w[j].x, s), __fmul_rn(w[j].y, s), __fmul_rn(w[j].z, s),
@@ -242,22 +247,24 @@ constexpr int kDecWarps = 8;
 
 // One warp per row: scores[row, c] = x . coef_c + intercept_c (exact float products, double sums, one rounding), the
 // first arg-max (n_out > 1) or score > 0 (n_out == 1).
+template <int D>
 __global__ void __launch_bounds__(kDecWarps * 32) linear_decision_kernel(const float* __restrict__ X, int64_t n,
                                                                          const float* __restrict__ coef,
                                                                          const double* __restrict__ intercept,
                                                                          int n_out, float* __restrict__ scores,
                                                                          int32_t* __restrict__ pred) {
+  constexpr int kSgdVec = D / (32 * 4);
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * kDecWarps + (threadIdx.x >> 5);
   if (row >= n) return;
-  const float4* x4 = reinterpret_cast<const float4*>(X) + row * (kSgdDim / 4);
+  const float4* x4 = reinterpret_cast<const float4*>(X) + row * (D / 4);
   float4 x[kSgdVec];
 #pragma unroll
   for (int j = 0; j < kSgdVec; ++j) x[j] = __ldg(x4 + lane + 32 * j);
   float best = -INFINITY, score = 0.f;
   int arg = 0;
   for (int c = 0; c < n_out; ++c) {
-    const float4* w4 = reinterpret_cast<const float4*>(coef) + (size_t)c * (kSgdDim / 4);
+    const float4* w4 = reinterpret_cast<const float4*>(coef) + (size_t)c * (D / 4);
     double acc = 0.0;
 #pragma unroll
     for (int j = 0; j < kSgdVec; ++j) {
@@ -343,7 +350,8 @@ int launch_sgd_fit(const float* x, int64_t n, int dim, const int32_t* class_host
   PLIP_REQUIRE(x && class_host && problems_host && sigma_host && coef && intercept && n_iter && overflow && ws,
                "plip_sgd_fit: null argument");
   PLIP_REQUIRE(n >= 2 && n <= INT32_MAX, "plip_sgd_fit: n = %lld samples; a fit needs 2..2^31-1", (long long)n);
-  PLIP_REQUIRE(dim == kSgdDim, "plip_sgd_fit: dim = %d; the embeddings must be %d wide", dim, kSgdDim);
+  PLIP_REQUIRE(dim == kSgdDimClip || dim == kSgdDimDenseNet,
+               "plip_sgd_fit: dim = %d; the embeddings must be %d or %d wide", dim, kSgdDimClip, kSgdDimDenseNet);
   PLIP_REQUIRE(n_classes >= 2, "plip_sgd_fit: n_classes = %d; a fit needs at least 2", n_classes);
   PLIP_REQUIRE(n_problems >= 1 && n_sigma >= 1, "plip_sgd_fit: n_problems = %d and n_sigma = %d must be >= 1",
                n_problems, n_sigma);
@@ -389,7 +397,8 @@ int launch_sgd_fit(const float* x, int64_t n, int dim, const int32_t* class_host
                                   st));
   PLIP_CUDA_CHECK(cudaMemcpyAsync(base + lay.sigma, sigma_host, sizeof(int32_t) * (size_t)n * n_sigma,
                                   cudaMemcpyHostToDevice, st));
-  PLIP_CUDA_CHECK(launch_kernel(sgd_fit_kernel, dim3((unsigned)n_problems), dim3(32), 0, st, 1, x, (int)n,
+  auto* kernel = dim == kSgdDimClip ? sgd_fit_kernel<kSgdDimClip> : sgd_fit_kernel<kSgdDimDenseNet>;
+  PLIP_CUDA_CHECK(launch_kernel(kernel, dim3((unsigned)n_problems), dim3(32), 0, st, 1, x, (int)n,
                                 reinterpret_cast<const int32_t*>(base + lay.classes),
                                 reinterpret_cast<const SgdProblem*>(base + lay.problems),
                                 reinterpret_cast<const int32_t*>(base + lay.sigma),
@@ -401,14 +410,16 @@ int launch_sgd_fit(const float* x, int64_t n, int dim, const int32_t* class_host
 int launch_linear_decision(const float* x, int64_t n, int dim, const float* coef, const double* intercept, int n_out,
                            float* scores, int32_t* pred, cudaStream_t st) {
   PLIP_REQUIRE(x && coef && intercept && scores && pred, "plip_linear_decision: null argument");
-  PLIP_REQUIRE(dim == kSgdDim, "plip_linear_decision: dim = %d; the embeddings must be %d wide", dim, kSgdDim);
+  PLIP_REQUIRE(dim == kSgdDimClip || dim == kSgdDimDenseNet,
+               "plip_linear_decision: dim = %d; the embeddings must be %d or %d wide", dim, kSgdDimClip, kSgdDimDenseNet);
   PLIP_REQUIRE(n >= 0, "plip_linear_decision: n = %lld is negative", (long long)n);
   PLIP_REQUIRE(n_out >= 1, "plip_linear_decision: n_out = %d must be >= 1", n_out);
   PLIP_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)coef & 15) == 0,
                "plip_linear_decision: x_dev %p and coef_dev %p must be 16-byte aligned", (const void*)x,
                (const void*)coef);
   if (n == 0) return 0;
-  PLIP_CUDA_CHECK(launch_kernel(linear_decision_kernel, dim3((unsigned)((n + kDecWarps - 1) / kDecWarps)),
+  auto* kernel = dim == kSgdDimClip ? linear_decision_kernel<kSgdDimClip> : linear_decision_kernel<kSgdDimDenseNet>;
+  PLIP_CUDA_CHECK(launch_kernel(kernel, dim3((unsigned)((n + kDecWarps - 1) / kDecWarps)),
                                 dim3(kDecWarps * 32), 0, st, 1, x, n, coef, intercept, n_out, scores, pred));
   return 0;
 }

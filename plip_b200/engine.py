@@ -15,6 +15,9 @@ from .weights import operand_format, pack_state_dict
 PIX_F32_NCHW, PIX_BF16_NCHW, PIX_U8_NHWC = 0, 1, 2
 IDS_I32, IDS_I64 = 0, 1
 EMBED_DIM = 512
+# Embedding widths the linear probe (plip_sgd_fit / plip_linear_decision) runs at: the CLIP projection and MuDiPath's
+# DenseNet-121 features.
+PROBE_DIMS = (EMBED_DIM, 1024)
 IMAGE_SIZE = 224
 MAX_TEXT_LEN = 77
 
@@ -406,9 +409,15 @@ def sgd_shuffle_permutation(n: int, seed: int) -> np.ndarray:
     return out
 
 
+def probe_widths() -> str:
+    """The accepted probe widths as an error message names them: ``"512 or 1024"``."""
+    return " or ".join(map(str, PROBE_DIMS))
+
+
 def _device_embeddings(x: torch.Tensor, what: str) -> Tuple[int, int]:
-    if not (torch.is_tensor(x) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and x.is_contiguous()):
-        raise ValueError(f"{what} must be a contiguous CUDA float32 [n, {EMBED_DIM}] tensor")
+    if not (torch.is_tensor(x) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and x.is_contiguous()
+            and x.shape[1] in PROBE_DIMS):
+        raise ValueError(f"{what} must be a contiguous CUDA float32 [n, d] tensor, d = {probe_widths()}")
     return int(x.shape[0]), int(x.shape[1])
 
 
@@ -416,10 +425,10 @@ def _device_embeddings(x: torch.Tensor, what: str) -> Tuple[int, int]:
 def sgd_fit(x: torch.Tensor, class_ids, n_classes: int, problems, sigma, max_iter: int = 10000, tol: float = 1e-3,
             n_iter_no_change: int = 5):
     """scikit-learn's SGD logistic regression for many binary problems in one launch (``plip_sgd_fit``; needs no
-    engine).  ``x``: CUDA float32 ``[n, 512]``; ``class_ids``: int ``[n]`` in ``0..n_classes-1``; ``problems``: one
-    ``(alpha, pos_class, pos_weight, neg_weight, sigma_index)`` per problem; ``sigma``: int32 ``[n_sigma, n]`` epoch
-    permutations (``sgd_shuffle_permutation``).  Returns device tensors ``(coef f32 [P, 512], intercept f64 [P],
-    n_iter int32 [P], overflow int32 [P])``; bad arguments raise ``ValueError`` before anything is launched."""
+    engine).  ``x``: CUDA float32 ``[n, d]``, ``d`` in ``PROBE_DIMS`` (512 or 1024); ``class_ids``: int ``[n]`` in
+    ``0..n_classes-1``; ``problems``: one ``(alpha, pos_class, pos_weight, neg_weight, sigma_index)`` per problem;
+    ``sigma``: int32 ``[n_sigma, n]`` epoch permutations (``sgd_shuffle_permutation``).  Returns device tensors
+    ``(coef f32 [P, d], intercept f64 [P], n_iter int32 [P], overflow int32 [P])``; bad arguments raise ``ValueError`` before anything is launched."""
     n, d = _device_embeddings(x, "x")
     cls = np.ascontiguousarray(np.asarray(class_ids), dtype=np.int32)
     sig = np.ascontiguousarray(np.asarray(sigma), dtype=np.int32)
@@ -433,7 +442,7 @@ def sgd_fit(x: torch.Tensor, class_ids, n_classes: int, problems, sigma, max_ite
     _check_args(L.plip_sgd_workspace_bytes(n, int(sig.shape[0]), p, C.byref(need)), "plip_sgd_workspace_bytes")
     dev = x.device
     ws = torch.empty(int(need.value), dtype=torch.uint8, device=dev)
-    coef = torch.empty(p, EMBED_DIM, dtype=torch.float32, device=dev)
+    coef = torch.empty(p, d, dtype=torch.float32, device=dev)
     intercept = torch.empty(p, dtype=torch.float64, device=dev)
     n_iter = torch.empty(p, dtype=torch.int32, device=dev)
     overflow = torch.empty(p, dtype=torch.int32, device=dev)
@@ -448,8 +457,9 @@ def sgd_fit(x: torch.Tensor, class_ids, n_classes: int, problems, sigma, max_ite
 @torch.no_grad()
 def linear_decision(x: torch.Tensor, coef: torch.Tensor, intercept: torch.Tensor):
     """``decision_function`` and the predicted index of a linear classifier (``plip_linear_decision``; needs no engine):
-    ``x`` CUDA float32 ``[n, 512]``, ``coef`` float32 ``[C, 512]``, ``intercept`` ``[C]`` on the same device.  Returns
-    ``(scores f32 [n, C], pred int32 [n])``: the first arg-max for ``C > 1``, ``score > 0`` for ``C == 1``."""
+    ``x`` CUDA float32 ``[n, d]``, ``coef`` float32 ``[C, d]`` (``d`` 512 or 1024), ``intercept`` ``[C]`` on the same
+    device.  Returns ``(scores f32 [n, C], pred int32 [n])``: the first arg-max for ``C > 1``, ``score > 0`` for
+    ``C == 1``."""
     n, d = _device_embeddings(x, "x")
     c, dc = _device_embeddings(coef, "coef")
     b = intercept.to(device=x.device, dtype=torch.float64).contiguous()

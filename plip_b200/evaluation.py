@@ -7,7 +7,8 @@ similarity kernels (fp32).  The sklearn metrics of the reference (``metrics.py``
 hot path: pass ``eval_metrics=`` to reuse them; the p@10 / p@50 retrieval metric is restated here because it is a
 pure function of the top-k indices.
 
-``LinearProber`` (``evaluation/linear_probing/linear_classifier.py``) fits the reference's
+``LinearProber`` (``evaluation/linear_probing/linear_classifier.py``) fits, on ``[N,512]`` PLIP / CLIP or ``[N,1024]``
+MuDiPath (DenseNet-121) features, the reference's
 ``SGDClassifier(loss="log_loss", penalty="l2", max_iter=10000, class_weight="balanced")`` with scikit-learn 1.9's
 algorithm restated on the device (``plip_sgd_fit``): same shuffles, same casts, every one-vs-rest problem at once;
 ``linear_probe_sweep`` fits a whole alpha sweep in one launch.
@@ -20,7 +21,7 @@ from typing import Callable, List, Optional, Sequence
 import numpy as np
 import torch
 
-from .engine import EMBED_DIM, Engine, linear_decision, sgd_fit, sgd_shuffle_permutation, similarity_topk
+from .engine import PROBE_DIMS, Engine, linear_decision, probe_widths, sgd_fit, sgd_shuffle_permutation, similarity_topk
 
 
 def _t(x) -> torch.Tensor:
@@ -102,15 +103,16 @@ def _device(engine: Optional[Engine]) -> torch.device:
 
 
 def _embeddings(x, device: torch.device) -> torch.Tensor:
-    """float32 ``[n, 512]`` (numpy or torch, host or device) as a contiguous tensor on ``device``.  Other dtypes raise:
-    scikit-learn runs float64 input through its 64-bit instantiation, which is not restated here."""
+    """float32 ``[n, 512]`` or ``[n, 1024]`` (numpy or torch, host or device) as a contiguous tensor on ``device``.
+    Other dtypes raise: scikit-learn runs float64 input through its 64-bit instantiation, which is not restated here."""
+    want = f"float32 [n, d] with d = {probe_widths()}"
     if not torch.is_tensor(x):
         x = np.asarray(x)
         if x.dtype != np.float32:
-            raise ValueError(f"the embeddings must be float32 [n, {EMBED_DIM}], got {x.dtype}")
+            raise ValueError(f"the embeddings must be {want}, got {x.dtype}")
         x = torch.from_numpy(np.ascontiguousarray(x))
-    if x.dtype != torch.float32 or x.dim() != 2 or x.shape[1] != EMBED_DIM:
-        raise ValueError(f"the embeddings must be float32 [n, {EMBED_DIM}], got {x.dtype} {tuple(x.shape)}")
+    if x.dtype != torch.float32 or x.dim() != 2 or x.shape[1] not in PROBE_DIMS:
+        raise ValueError(f"the embeddings must be {want}, got {x.dtype} {tuple(x.shape)}")
     x = x.to(device).contiguous()
     if x.shape[0] and not bool(torch.isfinite(x).all()):
         kind = "NaN" if bool(torch.isnan(x).any()) else "infinity or a value too large for dtype('float32')"
@@ -132,14 +134,21 @@ def _problem_seeds(n_classes: int, seed: int) -> List[int]:
 
 class SGDLinearClassifier:
     """A fitted one-vs-rest logistic regression with ``SGDClassifier``'s attributes: ``classes_``, ``coef_`` float32
-    ``[C, 512]`` (``[1, 512]`` for two classes), ``intercept_`` (float32 ``[C]``, float64 ``[1]`` for two classes, as
-    scikit-learn keeps them), ``n_iter_`` and ``alpha``.  ``decision_function`` / ``predict`` run on the device."""
+    ``[C, d]`` (``[1, d]`` for two classes; ``d`` the width of the training features, 512 or 1024), ``intercept_``
+    (float32 ``[C]``, float64 ``[1]`` for two classes, as scikit-learn keeps them), ``n_features_in_`` (``d``),
+    ``n_iter_`` and ``alpha``.  ``decision_function`` / ``predict`` run on the device; features of another width raise
+    scikit-learn's ``ValueError`` before anything is copied or launched."""
 
     def __init__(self, classes, coef, intercept, n_iter: int, alpha: float, device: torch.device):
         self.classes_, self.coef_, self.intercept_, self.n_iter_, self.alpha = classes, coef, intercept, n_iter, alpha
+        self.n_features_in_ = int(coef.shape[1])
         self.device = device
 
     def _decide(self, X):
+        shape = tuple(X.shape) if hasattr(X, "shape") else np.shape(X)
+        if len(shape) == 2 and shape[1] != self.n_features_in_:
+            raise ValueError(f"X has {shape[1]} features, but SGDClassifier is expecting {self.n_features_in_} "
+                             "features as input.")
         x = _embeddings(X, self.device)
         coef = torch.from_numpy(self.coef_).to(self.device)
         return linear_decision(x, coef, torch.from_numpy(self.intercept_.astype(np.float64)))

@@ -1,11 +1,14 @@
 """The linear probe on one GPU, on a Kather-shaped synthetic problem: 100 k training and 7 k test rows of float32
-[., 512] embeddings, 9 classes, and ``reproduce.sh``'s alphas (1e-4, 1e-3, 1e-2, 1e-1).  Reports the wall time of
+[., 512] embeddings (unit-norm, like PLIP's), or with ``--dim 1024`` of [., 1024] features shaped like MuDiPath's
+DenseNet-121 ones (un-normalised, non-negative, a positive offset and a scale of a few units), 9 classes, and
+``reproduce.sh``'s alphas (1e-4, 1e-3, 1e-2, 1e-1).  Reports the wall time of
 ``evaluation.linear_probe_sweep`` (all 4 x 9 binary problems in one launch, ending in a device synchronise), the
 epochs per alpha, and ns per sample step along the longest problem's chain (the kernel is bound by that dependent
-chain, not by a roofline).  When scikit-learn imports, also the host time of the same 4 ``SGDClassifier`` fits and
-whether the predictions agree.  Prints the card name and power limit with the numbers.  GPU only.
+chain, not by a roofline).  When scikit-learn imports, also the host time of the same 4 ``SGDClassifier`` fits,
+whether the predictions agree and the fraction of bit-identical ``coef_`` entries.  Prints the card name and power
+limit with the numbers.  GPU only.
 
-    python tools/linear_probe_probe.py [out.json] [--no-sklearn]
+    python tools/linear_probe_probe.py [out.json] [--dim 1024] [--no-sklearn]
 """
 import json
 import os
@@ -27,13 +30,18 @@ N_TRAIN, N_TEST, CLASSES = 100_000, 7_000, 9
 ALPHAS = [1e-4, 1e-3, 1e-2, 1e-1]
 
 
-def kather_like(n, seed):
-    """Unit-norm embeddings around 9 class means with class sizes as uneven as Kather's (about 2:1)."""
+def kather_like(n, seed, dim=512):
+    """Embeddings around 9 class means with class sizes as uneven as Kather's (about 2:1).  ``dim`` 512: unit-norm
+    rows.  ``dim`` 1024: DenseNet-like pooled features, un-normalised: non-negative around a positive offset of 1 with
+    a spread of about 0.5."""
     rs = np.random.RandomState(seed)
     p = np.linspace(1.0, 2.0, CLASSES)
     y = rs.choice(CLASSES, size=n, p=p / p.sum())
-    means = np.random.RandomState(0).standard_normal((CLASSES, 512))
-    x = means[y] * 0.05 + rs.standard_normal((n, 512)) * 0.3
+    means = np.random.RandomState(0).standard_normal((CLASSES, dim))
+    if dim == 1024:
+        x = np.maximum(1.0 + means[y] * 0.1 + rs.standard_normal((n, dim)) * 0.5, 0.0)
+        return x.astype(np.float32), y
+    x = means[y] * 0.05 + rs.standard_normal((n, dim)) * 0.3
     x /= np.linalg.norm(x, axis=1, keepdims=True)
     return x.astype(np.float32), y
 
@@ -41,10 +49,14 @@ def kather_like(n, seed):
 def main():
     if not torch.cuda.is_available():
         sys.exit("linear_probe_probe: needs a CUDA device")
-    out_path = next((a for a in sys.argv[1:] if not a.startswith("--")), None)
-    xtr, ytr = kather_like(N_TRAIN, 1)
-    xte, yte = kather_like(N_TEST, 2)
-    res = {"card": card(), "n_train": N_TRAIN, "n_test": N_TEST, "classes": CLASSES, "alphas": ALPHAS}
+    args = sys.argv[1:]
+    dim = int(args[args.index("--dim") + 1]) if "--dim" in args else 512
+    if "--dim" in args:
+        del args[args.index("--dim"):args.index("--dim") + 2]
+    out_path = next((a for a in args if not a.startswith("--")), None)
+    xtr, ytr = kather_like(N_TRAIN, 1, dim)
+    xte, yte = kather_like(N_TEST, 2, dim)
+    res = {"card": card(), "dim": dim, "n_train": N_TRAIN, "n_test": N_TEST, "classes": CLASSES, "alphas": ALPHAS}
 
     fit_sgd_classifiers(xtr[:2000], ytr[:2000], ALPHAS)          # module load, first launches
     dtr, dte = torch.from_numpy(xtr).cuda(), torch.from_numpy(xte).cuda()
@@ -68,7 +80,7 @@ def main():
         except ImportError:
             res["sklearn"] = "not installed"
         else:
-            sk_s, agree, sk_epochs, dcoef = 0.0, [], [], []
+            sk_s, agree, sk_epochs, dcoef, same = 0.0, [], [], [], []
             for a, (clf, _) in zip(ALPHAS, sweep):
                 sk = SGDClassifier(random_state=7, loss="log_loss", alpha=a, penalty="l2", max_iter=10000,
                                    class_weight="balanced")
@@ -80,10 +92,12 @@ def main():
                 sk_epochs.append(int(sk.n_iter_))
                 agree.append(float(np.mean(sk.predict(xte) == clf.predict(dte))))
                 dcoef.append(float(np.abs(sk.coef_ - clf.coef_).max() / np.abs(sk.coef_).max()))
+                same.append(float(np.mean(sk.coef_ == clf.coef_)))
             res["sklearn_fit_s"] = sk_s
             res["sklearn_epochs_per_alpha"] = sk_epochs
             res["prediction_agreement"] = agree
             res["max_abs_dcoef_over_max_coef"] = dcoef
+            res["coef_bit_identical_fraction"] = same
     print(json.dumps(res, indent=1))
     if out_path:
         with open(out_path, "w") as f:
