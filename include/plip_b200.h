@@ -32,7 +32,7 @@ extern "C" {
 
 #define PLIP_API __attribute__((visibility("default")))
 
-#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts, plip_window_mask_counts, plip_resize_region_*, plip_resize_filter_bounds, plip_sgd_*, plip_linear_decision, plip_densenet_*, plip_resize_crop_bilinear_u8, plip_warp_tiles_u8, plip_resize_crop_fill_u8, plip_mask_value_sets_u8, plip_encode_pair (new symbols only) */
+#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts, plip_window_mask_counts, plip_resize_region_*, plip_resize_filter_bounds, plip_sgd_*, plip_linear_decision, plip_densenet_*, plip_resize_crop_bilinear_u8, plip_warp_tiles_u8, plip_resize_crop_fill_u8, plip_mask_value_sets_u8, plip_encode_pair, plip_sgd_fit_f64, plip_linear_decision_f64 (new symbols only) */
 
 /* Model constants (TF:configuration_clip.py:47-64,97-109,160-161). */
 #define PLIP_IMAGE_SIZE 224
@@ -337,15 +337,17 @@ PLIP_API int plip_resize_filter_bounds(int in_size, int out_size, int32_t* bound
 
 /* ---- linear probe: scikit-learn's SGD logistic regression (no engine) ------------------------- */
 /* The reference's linear probe (reproducibility/evaluation/linear_probing/linear_classifier.py) fits
- * SGDClassifier(loss="log_loss", penalty="l2", class_weight="balanced", learning_rate="optimal") on float32 [n,512]
- * (PLIP, CLIP) or [n,1024] (MuDiPath's DenseNet-121) embeddings: one-vs-rest binary problems, each a sequential pass
- * of sklearn 1.9's _plain_sgd (32-bit instantiation) over a shuffled order per epoch.  plip_sgd_fit runs that
- * algorithm, cast for cast, for many binary problems at once (every class of a fit, every alpha of a sweep): one warp
- * per problem runs all its epochs on the device.  The results equal sklearn's up to the order of the D-term double
+ * SGDClassifier(loss="log_loss", penalty="l2", class_weight="balanced", learning_rate="optimal") on [n,512] (PLIP,
+ * CLIP; float16 when the reference embeds on a GPU) or [n,1024] (MuDiPath's DenseNet-121) embeddings: one-vs-rest
+ * binary problems, each a sequential pass of sklearn 1.9's _plain_sgd over a shuffled order per epoch.  plip_sgd_fit
+ * runs its 32-bit instantiation (float32 input), plip_sgd_fit_f64 its 64-bit one (float16 / float64 input), cast for
+ * cast, for many binary problems at once (every class of a fit, every alpha of a sweep): one warp per problem runs all
+ * its epochs on the device.  The results equal sklearn's up to the order of the D-term double
  * sums (D = dim) and CUDA's exp / log1p against the C library's.
  *
  * One binary problem: labels y = (class_host[i] == pos_class), positive / negative sample weight pos_weight /
- * neg_weight (rounded to float, as sklearn's class_weight local), regularisation alpha (> 0, finite), t starting at 1,
+ * neg_weight (rounded to float by plip_sgd_fit, kept in double by plip_sgd_fit_f64, as sklearn's class_weight
+ * local), regularisation alpha (> 0, finite), t starting at 1,
  * and the epoch order order_e[i] = order_{e-1}[sigma[i]] (order_0 = identity) with sigma row sigma_index of
  * sigma_host: the permutation sklearn's dataset.shuffle(seed) applies every epoch (plip_sgd_shuffle_permutation). */
 typedef struct plip_sgd_problem {
@@ -358,7 +360,8 @@ typedef struct plip_sgd_problem {
 /* Host-only: sklearn's Fisher-Yates shuffle (utils/_seq_dataset.pyx.tp, our_rand_r xorshift, j = i + r % (n - i))
  * applied to the identity: sigma_host int32 [n].  1 <= n < 2^31; seed 0 behaves as our_rand_r's default 1. */
 PLIP_API int plip_sgd_shuffle_permutation(int64_t n, uint32_t seed, int32_t* sigma_host);
-/* Device workspace bytes of plip_sgd_fit (problem table, labels, sigma rows and two epoch orders per problem). */
+/* Device workspace bytes of plip_sgd_fit and plip_sgd_fit_f64 (problem table, labels, sigma rows and two epoch orders
+ * per problem); one size serves both precisions. */
 PLIP_API int plip_sgd_workspace_bytes(int64_t n, int n_sigma, int n_problems, uint64_t* bytes);
 /* x_dev: device float32 [n,dim], dim = 512 or 1024, rows contiguous, 16-byte aligned; 2 <= n < 2^31.  class_host:
  * HOST int32 [n] class ids in 0..n_classes-1.  problems_host: HOST [n_problems].  sigma_host: HOST int32 [n_sigma, n], every entry in 0..n-1.
@@ -382,6 +385,24 @@ PLIP_API int plip_sgd_fit(const float* x_dev, int64_t n, int dim, const int32_t*
 PLIP_API int plip_linear_decision(const float* x_dev, int64_t n, int dim, const float* coef_dev,
                                   const double* intercept_dev, int n_out, float* scores_dev, int32_t* pred_dev,
                                   void* stream);
+/* The 64-bit instantiation of _plain_sgd, which sklearn runs on float64 input and on float16 input (its check_array
+ * widens anything that is not float32 to float64): WeightVector64's double weights, dot returning the double
+ * sum * wscale unrounded, scale and add taking double coefficients, the wscale reset below 1e-9 (not 1e-6), and
+ * pos_weight / neg_weight kept in double.  Same arguments and contract as plip_sgd_fit, with x_dev float64 [n,dim]
+ * (float16 embeddings widened exactly by the caller) and coef_dev float64 [n_problems,dim]; the same workspace
+ * (plip_sgd_workspace_bytes).  The results equal sklearn's up to the order of the D-term double sums (dot and sum(w^2)
+ * are reduced per lane, then across the warp; sklearn sums in index order) and CUDA's exp / log1p. */
+PLIP_API int plip_sgd_fit_f64(const double* x_dev, int64_t n, int dim, const int32_t* class_host, int n_classes,
+                              const plip_sgd_problem_t* problems_host, int n_problems, const int32_t* sigma_host,
+                              int n_sigma, int max_iter, double tol, int n_iter_no_change, double* coef_dev,
+                              double* intercept_dev, int32_t* n_iter_dev, int32_t* overflow_dev, void* workspace_dev,
+                              uint64_t workspace_bytes, void* stream);
+/* decision_function and predict in float64: scores_dev float64 [n, n_out] = x . coef^T + intercept (double products and
+ * sums), pred_dev int32 [n] by plip_linear_decision's rule.  x_dev float64 [n,dim] and coef_dev float64 [n_out,dim]
+ * (dim = 512 or 1024) 16-byte aligned, intercept_dev float64 [n_out].  Stream-ordered, one launch. */
+PLIP_API int plip_linear_decision_f64(const double* x_dev, int64_t n, int dim, const double* coef_dev,
+                                      const double* intercept_dev, int n_out, double* scores_dev, int32_t* pred_dev,
+                                      void* stream);
 
 /* ---- MuDiPath DenseNet-121 image embedder (separate handle) ----------------------------------- */
 /* The reference's third embedder (reproducibility/embedders/factory.py:34-47, mudipath.py:125-130,205-215): torchvision's

@@ -120,6 +120,9 @@ SIGNATURES = {
     "plip_sgd_fit": (_i, [_fp, _i64, _i, _vp, _i, _vp, _i, _vp, _i, _i, C.c_double, _i, _fp, _vp, _vp, _vp, _vp, _u64,
                           _vp]),
     "plip_linear_decision": (_i, [_fp, _i64, _i, _fp, _vp, _i, _fp, _vp, _vp]),
+    "plip_sgd_fit_f64": (_i, [_vp, _i64, _i, _vp, _i, _vp, _i, _vp, _i, _i, C.c_double, _i, _vp, _vp, _vp, _vp, _vp,
+                              _u64, _vp]),
+    "plip_linear_decision_f64": (_i, [_vp, _i64, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     "plip_densenet_num_tensors": (_i, []),
     "plip_densenet_tensor_info": (_i, [_i, C.POINTER(TensorInfo)]),
     "plip_densenet_blob_bytes": (_u64, []),

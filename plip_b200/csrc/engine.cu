@@ -1421,6 +1421,23 @@ PLIP_API int plip_linear_decision(const float* x_dev, int64_t n, int dim, const 
                                 static_cast<cudaStream_t>(stream));
 }
 
+PLIP_API int plip_sgd_fit_f64(const double* x_dev, int64_t n, int dim, const int32_t* class_host, int n_classes,
+                              const plip_sgd_problem_t* problems_host, int n_problems, const int32_t* sigma_host,
+                              int n_sigma, int max_iter, double tol, int n_iter_no_change, double* coef_dev,
+                              double* intercept_dev, int32_t* n_iter_dev, int32_t* overflow_dev, void* workspace_dev,
+                              uint64_t workspace_bytes, void* stream) {
+  return launch_sgd_fit_f64(x_dev, n, dim, class_host, n_classes, problems_host, n_problems, sigma_host, n_sigma,
+                            max_iter, tol, n_iter_no_change, coef_dev, intercept_dev, n_iter_dev, overflow_dev,
+                            workspace_dev, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+PLIP_API int plip_linear_decision_f64(const double* x_dev, int64_t n, int dim, const double* coef_dev,
+                                      const double* intercept_dev, int n_out, double* scores_dev, int32_t* pred_dev,
+                                      void* stream) {
+  return launch_linear_decision_f64(x_dev, n, dim, coef_dev, intercept_dev, n_out, scores_dev, pred_dev,
+                                    static_cast<cudaStream_t>(stream));
+}
+
 PLIP_API int plip_dbg_resize_filter(int in_size, int out_size, int xx, int32_t* k_host, int k_cap, int* xmin,
                                     int* count) {
   PLIP_REQUIRE(k_host && xmin && count && in_size > 0 && out_size > 0 && xx >= 0 && xx < out_size,

@@ -88,7 +88,7 @@ int launch_similarity_topk(const float* q, int64_t n, const float* s, int64_t m,
                            bool norm_s, int k, int32_t* idx, float* val, cudaStream_t st);
 
 // linear_probe.cu: sklearn's SGD logistic regression, one warp per binary problem, and the linear decision (the
-// plip_sgd_* / plip_linear_decision contracts of plip_b200.h; every argument is checked before anything is launched).
+// plip_sgd_* / plip_linear_decision* contracts of plip_b200.h; every argument is checked before anything is launched).
 int sgd_shuffle_permutation(int64_t n, uint32_t seed, int32_t* sigma);
 int sgd_workspace_bytes(int64_t n, int n_sigma, int n_problems, uint64_t* bytes);
 int launch_sgd_fit(const float* x, int64_t n, int dim, const int32_t* class_host, int n_classes,
@@ -97,5 +97,11 @@ int launch_sgd_fit(const float* x, int64_t n, int dim, const int32_t* class_host
                    int32_t* overflow, void* ws, uint64_t ws_bytes, cudaStream_t st);
 int launch_linear_decision(const float* x, int64_t n, int dim, const float* coef, const double* intercept, int n_out,
                            float* scores, int32_t* pred, cudaStream_t st);
+int launch_sgd_fit_f64(const double* x, int64_t n, int dim, const int32_t* class_host, int n_classes,
+                       const plip_sgd_problem_t* problems_host, int n_problems, const int32_t* sigma_host, int n_sigma,
+                       int max_iter, double tol, int n_iter_no_change, double* coef, double* intercept,
+                       int32_t* n_iter, int32_t* overflow, void* ws, uint64_t ws_bytes, cudaStream_t st);
+int launch_linear_decision_f64(const double* x, int64_t n, int dim, const double* coef, const double* intercept,
+                               int n_out, double* scores, int32_t* pred, cudaStream_t st);
 
 }  // namespace plip

@@ -475,6 +475,65 @@ def linear_decision(x: torch.Tensor, coef: torch.Tensor, intercept: torch.Tensor
     return scores, pred
 
 
+def _device_embeddings_f64(x: torch.Tensor, what: str) -> Tuple[int, int]:
+    if not (torch.is_tensor(x) and x.is_cuda and x.dtype == torch.float64 and x.dim() == 2 and x.is_contiguous()
+            and x.shape[1] in PROBE_DIMS):
+        raise ValueError(f"{what} must be a contiguous CUDA float64 [n, d] tensor, d = {probe_widths()}")
+    return int(x.shape[0]), int(x.shape[1])
+
+
+@torch.no_grad()
+def sgd_fit_f64(x: torch.Tensor, class_ids, n_classes: int, problems, sigma, max_iter: int = 10000,
+                tol: float = 1e-3, n_iter_no_change: int = 5):
+    """``sgd_fit`` in scikit-learn's 64-bit instantiation (``plip_sgd_fit_f64``), the one it runs on float16 and
+    float64 input: ``x`` CUDA float64 ``[n, d]`` (widen float16 exactly first), the other arguments as ``sgd_fit``.
+    Returns device tensors ``(coef f64 [P, d], intercept f64 [P], n_iter int32 [P], overflow int32 [P])``."""
+    n, d = _device_embeddings_f64(x, "x")
+    cls = np.ascontiguousarray(np.asarray(class_ids), dtype=np.int32)
+    sig = np.ascontiguousarray(np.asarray(sigma), dtype=np.int32)
+    if cls.shape != (n,) or sig.ndim != 2 or sig.shape[1] != n:
+        raise ValueError(f"class ids {cls.shape} and sigma {sig.shape} do not match n = {n}")
+    table = (_SgdProblem * len(problems))(*[_SgdProblem(float(a), float(wp), float(wn), int(pc), int(si))
+                                            for a, pc, wp, wn, si in problems])
+    p = len(problems)
+    L = lib()
+    need = C.c_uint64(0)
+    _check_args(L.plip_sgd_workspace_bytes(n, int(sig.shape[0]), p, C.byref(need)), "plip_sgd_workspace_bytes")
+    dev = x.device
+    ws = torch.empty(int(need.value), dtype=torch.uint8, device=dev)
+    coef = torch.empty(p, d, dtype=torch.float64, device=dev)
+    intercept = torch.empty(p, dtype=torch.float64, device=dev)
+    n_iter = torch.empty(p, dtype=torch.int32, device=dev)
+    overflow = torch.empty(p, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _check_args(L.plip_sgd_fit_f64(x.data_ptr(), n, d, cls.ctypes.data, int(n_classes), table, p, sig.ctypes.data,
+                                       int(sig.shape[0]), int(max_iter), C.c_double(tol), int(n_iter_no_change),
+                                       coef.data_ptr(), intercept.data_ptr(), n_iter.data_ptr(), overflow.data_ptr(),
+                                       ws.data_ptr(), ws.numel(), torch.cuda.current_stream(dev).cuda_stream),
+                    "plip_sgd_fit_f64")
+    return coef, intercept, n_iter, overflow
+
+
+@torch.no_grad()
+def linear_decision_f64(x: torch.Tensor, coef: torch.Tensor, intercept: torch.Tensor):
+    """``linear_decision`` in float64 (``plip_linear_decision_f64``): ``x`` CUDA float64 ``[n, d]``, ``coef`` float64
+    ``[C, d]``, ``intercept`` ``[C]`` on the same device.  Returns ``(scores f64 [n, C], pred int32 [n])``."""
+    n, d = _device_embeddings_f64(x, "x")
+    c, dc = _device_embeddings_f64(coef, "coef")
+    b = intercept.to(device=x.device, dtype=torch.float64).contiguous()
+    if coef.device != x.device or dc != d or b.shape != (c,):
+        raise ValueError(f"coef {tuple(coef.shape)} on {coef.device} and intercept {tuple(intercept.shape)} do not "
+                         f"match x on {x.device}")
+    scores = torch.empty(n, c, dtype=torch.float64, device=x.device)
+    pred = torch.empty(n, dtype=torch.int32, device=x.device)
+    with torch.cuda.device(x.device):
+        _check_args(lib().plip_linear_decision_f64(x.data_ptr(), n, d, coef.data_ptr(), b.data_ptr(), c,
+                                                   scores.data_ptr(), pred.data_ptr(),
+                                                   torch.cuda.current_stream(x.device).cuda_stream),
+                    "plip_linear_decision_f64")
+    return scores, pred
+
+
 class Engine:
     """One engine per CUDA device: packed bf16/fp32 weights + workspace for ``max_micro_batch``."""
 

@@ -11,7 +11,9 @@ pure function of the top-k indices.
 MuDiPath (DenseNet-121) features, the reference's
 ``SGDClassifier(loss="log_loss", penalty="l2", max_iter=10000, class_weight="balanced")`` with scikit-learn 1.9's
 algorithm restated on the device (``plip_sgd_fit``): same shuffles, same casts, every one-vs-rest problem at once;
-``linear_probe_sweep`` fits a whole alpha sweep in one launch.
+``linear_probe_sweep`` fits a whole alpha sweep in one launch.  The training features' dtype picks the instantiation, as
+in scikit-learn: float32 runs the 32-bit one (``plip_sgd_fit``), float16 and float64 the 64-bit one
+(``plip_sgd_fit_f64``; the reference's ``plip`` and ``clip`` embedders return float16 rows when they run on a GPU).
 """
 from __future__ import annotations
 
@@ -21,7 +23,8 @@ from typing import Callable, List, Optional, Sequence
 import numpy as np
 import torch
 
-from .engine import PROBE_DIMS, Engine, linear_decision, probe_widths, sgd_fit, sgd_shuffle_permutation, similarity_topk
+from .engine import (PROBE_DIMS, Engine, linear_decision, linear_decision_f64, probe_widths, sgd_fit, sgd_fit_f64,
+                     sgd_shuffle_permutation, similarity_topk)
 
 
 def _t(x) -> torch.Tensor:
@@ -120,6 +123,41 @@ def _embeddings(x, device: torch.device) -> torch.Tensor:
     return x
 
 
+_WIDE = (np.float16, np.float64)          # the dtypes scikit-learn's check_array widens to float64
+_NUMPY_DTYPE = {torch.float16: np.dtype(np.float16), torch.float32: np.dtype(np.float32),
+                torch.float64: np.dtype(np.float64)}
+
+
+def _dtype_of(x):
+    """``x``'s dtype as numpy names it (``np.asarray``'s for anything that is not an array or a tensor; other torch
+    dtypes stay torch dtypes)."""
+    if torch.is_tensor(x):
+        return _NUMPY_DTYPE.get(x.dtype, x.dtype)
+    return x.dtype if isinstance(x, np.ndarray) else np.asarray(x).dtype
+
+
+def _probe_input(x, device: torch.device) -> torch.Tensor:
+    """The probe's features as scikit-learn's ``SGDClassifier`` takes them, as a contiguous tensor on ``device``:
+    float32 ``[n, d]`` through ``_embeddings``, float16 or float64 ``[n, d]`` (numpy or torch, host or device) in their
+    own dtype, ``d`` 512 or 1024.  Other dtypes raise; non-finite float16 / float64 input raises scikit-learn's message,
+    which names ``dtype('float64')``, the dtype it converts both to."""
+    dt = _dtype_of(x)
+    if dt == np.float32:
+        return _embeddings(x, device)
+    want = f"float32, float16 or float64 [n, d] with d = {probe_widths()}"
+    if dt not in _WIDE:
+        raise ValueError(f"the embeddings must be {want}, got {dt}")
+    if not torch.is_tensor(x):
+        x = torch.from_numpy(np.ascontiguousarray(x))
+    if x.dim() != 2 or x.shape[1] not in PROBE_DIMS:
+        raise ValueError(f"the embeddings must be {want}, got {dt} {tuple(x.shape)}")
+    x = x.to(device).contiguous()
+    if x.shape[0] and not bool(torch.isfinite(x).all()):
+        kind = "NaN" if bool(torch.isnan(x).any()) else "infinity or a value too large for dtype('float64')"
+        raise ValueError(f"Input X contains {kind}.")
+    return x
+
+
 def _problem_seeds(n_classes: int, seed: int) -> List[int]:
     """The ``seed`` scikit-learn hands to ``_plain_sgd`` per binary problem: ``fit_binary`` draws it after
     ``make_dataset``'s draw, from ``RandomState(seed)`` for two classes, else from one ``RandomState`` per class
@@ -136,8 +174,11 @@ class SGDLinearClassifier:
     """A fitted one-vs-rest logistic regression with ``SGDClassifier``'s attributes: ``classes_``, ``coef_`` float32
     ``[C, d]`` (``[1, d]`` for two classes; ``d`` the width of the training features, 512 or 1024), ``intercept_``
     (float32 ``[C]``, float64 ``[1]`` for two classes, as scikit-learn keeps them), ``n_features_in_`` (``d``),
-    ``n_iter_`` and ``alpha``.  ``decision_function`` / ``predict`` run on the device; features of another width raise
-    scikit-learn's ``ValueError`` before anything is copied or launched."""
+    ``n_iter_`` and ``alpha``.  A fit on float16 or float64 features keeps scikit-learn's 64-bit attributes: ``coef_``
+    float64 ``[C, d]`` or ``[1, d]``, ``intercept_`` float64 ``[C]`` or ``[1]``.  ``decision_function`` / ``predict`` run
+    on the device, with numpy's promotion of ``X . coef_.T``: float64 scores when ``X`` or ``coef_`` is float64, float32
+    otherwise (float16 ``X`` on a float32 model is widened to float32).  Features of another width raise scikit-learn's
+    ``ValueError`` before anything is copied or launched."""
 
     def __init__(self, classes, coef, intercept, n_iter: int, alpha: float, device: torch.device):
         self.classes_, self.coef_, self.intercept_, self.n_iter_, self.alpha = classes, coef, intercept, n_iter, alpha
@@ -149,12 +190,20 @@ class SGDLinearClassifier:
         if len(shape) == 2 and shape[1] != self.n_features_in_:
             raise ValueError(f"X has {shape[1]} features, but SGDClassifier is expecting {self.n_features_in_} "
                              "features as input.")
-        x = _embeddings(X, self.device)
-        coef = torch.from_numpy(self.coef_).to(self.device)
-        return linear_decision(x, coef, torch.from_numpy(self.intercept_.astype(np.float64)))
+        if self.coef_.dtype == np.float32 and _dtype_of(X) == np.float32:
+            x = _embeddings(X, self.device)
+            coef = torch.from_numpy(self.coef_).to(self.device)
+            return linear_decision(x, coef, torch.from_numpy(self.intercept_.astype(np.float64)))
+        x = _probe_input(X, self.device)
+        b = torch.from_numpy(self.intercept_.astype(np.float64))
+        if self.coef_.dtype == np.float32 and x.dtype == torch.float16:        # float16 . float32 -> float32
+            return linear_decision(x.to(torch.float32), torch.from_numpy(self.coef_).to(self.device), b)
+        coef = torch.from_numpy(self.coef_.astype(np.float64)).to(self.device)
+        return linear_decision_f64(x.to(torch.float64), coef, b)
 
     def decision_function(self, X) -> np.ndarray:
-        """``X . coef_.T + intercept_``: float32 ``[n, C]``, or ``[n]`` for two classes."""
+        """``X . coef_.T + intercept_``: ``[n, C]``, or ``[n]`` for two classes; float64 when ``X`` or ``coef_`` is
+        float64, else float32."""
         scores = self._decide(X)[0].cpu().numpy()
         return scores[:, 0] if scores.shape[1] == 1 else scores
 
@@ -167,10 +216,14 @@ def fit_sgd_classifiers(X, y, alphas: Sequence[float], seed: int = 7, max_iter: 
                         n_iter_no_change: int = 5, engine: Optional[Engine] = None) -> List[SGDLinearClassifier]:
     """``SGDClassifier(random_state=seed, loss="log_loss", alpha=a, penalty="l2", max_iter=max_iter, tol=tol,
     class_weight="balanced").fit(X, y)`` for every ``a`` in ``alphas``, all binary problems in one ``plip_sgd_fit``
-    launch.  ``y``: any labels (``classes_ = np.unique(y)``).  A problem whose weights overflow raises scikit-learn's
+    launch.  ``y``: any labels (``classes_ = np.unique(y)``).  ``X``: float32 runs scikit-learn's 32-bit instantiation,
+    float16 / float64 its 64-bit one (``plip_sgd_fit_f64``).  A problem whose weights overflow raises scikit-learn's
     ``ValueError`` (the first alpha and class in order)."""
     dev = _device(engine)
-    x = _embeddings(X, dev)
+    x = _probe_input(X, dev)
+    wide = x.dtype != torch.float32
+    if wide:
+        x = x.to(torch.float64)          # float16 widens exactly: one storage type for the 64-bit kernel
     classes, y_ind = np.unique(np.asarray(y), return_inverse=True)
     n, n_classes = int(x.shape[0]), len(classes)
     if y_ind.shape != (n,):
@@ -183,8 +236,9 @@ def fit_sgd_classifiers(X, y, alphas: Sequence[float], seed: int = 7, max_iter: 
     per_alpha = [(1, cw[1], cw[0], 0)] if n_classes == 2 else [(i, cw[i], 1.0, i) for i in range(n_classes)]
     problems = [(float(a), pc, wp, wn, si) for a in alphas for pc, wp, wn, si in per_alpha]
     sigma = np.stack([sgd_shuffle_permutation(n, s) for s in seeds])
-    coef, intercept, n_iter, overflow = (t.cpu().numpy() for t in sgd_fit(x, y_ind, n_classes, problems, sigma,
-                                                                           max_iter, tol, n_iter_no_change))
+    fit = sgd_fit_f64 if wide else sgd_fit
+    coef, intercept, n_iter, overflow = (t.cpu().numpy() for t in fit(x, y_ind, n_classes, problems, sigma,
+                                                                       max_iter, tol, n_iter_no_change))
     out, k = [], len(per_alpha)
     for i, a in enumerate(alphas):
         rows = slice(i * k, (i + 1) * k)
@@ -196,7 +250,7 @@ def fit_sgd_classifiers(X, y, alphas: Sequence[float], seed: int = 7, max_iter: 
         if max_iter > 1 and it == max_iter:
             warnings.warn("Maximum number of iteration reached before convergence. Consider increasing max_iter to "
                           "improve the fit.", ConvergenceWarning)
-        b = intercept[rows] if n_classes == 2 else intercept[rows].astype(np.float32)
+        b = intercept[rows] if n_classes == 2 or wide else intercept[rows].astype(np.float32)
         out.append(SGDLinearClassifier(classes, coef[rows].copy(), b.copy(), it, float(a), dev))
     return out
 
@@ -230,7 +284,7 @@ def linear_probe_sweep(train_x, train_y, test_x, test_y, alphas: Sequence[float]
     bit-identical to the single-alpha call."""
     ytr, yte = _encode_labels(train_y, test_y)
     dev = _device(engine)
-    xtr, xte = _embeddings(train_x, dev), _embeddings(test_x, dev)
+    xtr, xte = _probe_input(train_x, dev), _probe_input(test_x, dev)
     clfs = fit_sgd_classifiers(xtr, ytr, alphas, seed=seed, max_iter=10000, engine=engine)
     return [(clf, _probe_metrics(clf, xtr, ytr, xte, yte, eval_metrics)) for clf in clfs]
 

@@ -8,7 +8,11 @@ chain, not by a roofline).  When scikit-learn imports, also the host time of the
 whether the predictions agree and the fraction of bit-identical ``coef_`` entries.  Prints the card name and power
 limit with the numbers.  GPU only.
 
-    python tools/linear_probe_probe.py [out.json] [--dim 1024] [--no-sklearn]
+``--dtype float16`` gives the rows as the reference's ``plip`` / ``clip`` embedders return them on a GPU (float16,
+normalised in float16), ``--dtype float64`` as float64; both run scikit-learn's 64-bit instantiation
+(``plip_sgd_fit_f64``), and scikit-learn is timed on the same float16 / float64 array.
+
+    python tools/linear_probe_probe.py [out.json] [--dim 1024] [--dtype float16|float64] [--no-sklearn]
 """
 import json
 import os
@@ -30,33 +34,42 @@ N_TRAIN, N_TEST, CLASSES = 100_000, 7_000, 9
 ALPHAS = [1e-4, 1e-3, 1e-2, 1e-1]
 
 
-def kather_like(n, seed, dim=512):
+def kather_like(n, seed, dim=512, dtype=np.float32):
     """Embeddings around 9 class means with class sizes as uneven as Kather's (about 2:1).  ``dim`` 512: unit-norm
-    rows.  ``dim`` 1024: DenseNet-like pooled features, un-normalised: non-negative around a positive offset of 1 with
-    a spread of about 0.5."""
+    rows (float16 rows are normalised in float16, as ``embedders/plip.py`` does).  ``dim`` 1024: DenseNet-like pooled
+    features, un-normalised: non-negative around a positive offset of 1 with a spread of about 0.5."""
     rs = np.random.RandomState(seed)
     p = np.linspace(1.0, 2.0, CLASSES)
     y = rs.choice(CLASSES, size=n, p=p / p.sum())
     means = np.random.RandomState(0).standard_normal((CLASSES, dim))
     if dim == 1024:
         x = np.maximum(1.0 + means[y] * 0.1 + rs.standard_normal((n, dim)) * 0.5, 0.0)
-        return x.astype(np.float32), y
+        return x.astype(dtype), y
     x = means[y] * 0.05 + rs.standard_normal((n, dim)) * 0.3
+    if dtype == np.float16:
+        x = x.astype(dtype)
+        return x / np.linalg.norm(x, axis=1, keepdims=True), y
     x /= np.linalg.norm(x, axis=1, keepdims=True)
-    return x.astype(np.float32), y
+    return x.astype(dtype), y
 
 
 def main():
     if not torch.cuda.is_available():
         sys.exit("linear_probe_probe: needs a CUDA device")
     args = sys.argv[1:]
-    dim = int(args[args.index("--dim") + 1]) if "--dim" in args else 512
-    if "--dim" in args:
-        del args[args.index("--dim"):args.index("--dim") + 2]
+    opts = {"--dim": "512", "--dtype": "float32"}
+    for key in opts:
+        if key in args:
+            opts[key] = args[args.index(key) + 1]
+            del args[args.index(key):args.index(key) + 2]
+    dim, dtype = int(opts["--dim"]), np.dtype(opts["--dtype"])
+    if dtype not in (np.float32, np.float16, np.float64):
+        sys.exit("linear_probe_probe: --dtype is float32, float16 or float64")
     out_path = next((a for a in args if not a.startswith("--")), None)
-    xtr, ytr = kather_like(N_TRAIN, 1, dim)
-    xte, yte = kather_like(N_TEST, 2, dim)
-    res = {"card": card(), "dim": dim, "n_train": N_TRAIN, "n_test": N_TEST, "classes": CLASSES, "alphas": ALPHAS}
+    xtr, ytr = kather_like(N_TRAIN, 1, dim, dtype)
+    xte, yte = kather_like(N_TEST, 2, dim, dtype)
+    res = {"card": card(), "dim": dim, "dtype": dtype.name, "n_train": N_TRAIN, "n_test": N_TEST, "classes": CLASSES,
+           "alphas": ALPHAS}
 
     fit_sgd_classifiers(xtr[:2000], ytr[:2000], ALPHAS)          # module load, first launches
     dtr, dte = torch.from_numpy(xtr).cuda(), torch.from_numpy(xte).cuda()
