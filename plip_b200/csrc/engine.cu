@@ -1314,6 +1314,7 @@ PLIP_API int plip_similarity(const float* img_dev, int64_t n, const float* txt_d
                              int normalize_img, int normalize_txt, float* logits_dev, int64_t ld_logits,
                              void* stream) {
   PLIP_REQUIRE(img_dev && txt_dev && logits_dev, "plip_similarity: null argument");
+  PLIP_REQUIRE(n >= 0, "plip_similarity: negative row count n=%lld", (long long)n);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int64_t chunk = 65535LL * 64;  // grid.y limit
   for (int64_t i = 0; i < n; i += chunk) {

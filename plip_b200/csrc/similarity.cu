@@ -586,10 +586,11 @@ int launch_similarity(const float* a, int64_t n, const float* b, int64_t m, floa
   PLIP_REQUIRE((reinterpret_cast<uintptr_t>(a) & 15) == 0 && (reinterpret_cast<uintptr_t>(b) & 15) == 0 &&
                (reinterpret_cast<uintptr_t>(out) & 15) == 0, "similarity: operands must be 16-byte aligned");
   // Tensor-core path for wide score matrices (>= 256 columns) whenever the output rows can take the 128-column
-  // padding of the GEMM tile (plip_b200's own callers allocate ld_logits that way).
+  // padding of the GEMM tile (plip_b200's own callers allocate ld_logits that way) and the GEMM's row stride
+  // (a multiple of 8 floats).
   const int64_t m_pad = (m + 127) / 128 * 128;
   // (the choice depends on m only, so a row-sharded call computes bit-identical rows to the unsharded one)
-  if (m >= 256 && ldo >= m_pad && ldo % 4 == 0 && ldo < 0x7fffffff)
+  if (m >= 256 && ldo >= m_pad && ldo % 8 == 0 && ldo < 0x7fffffff)
     return launch_similarity_tc(a, n, b, m, scale, norm_a, norm_b, out, ldo, st);
   const int64_t gy = (n + TM - 1) / TM, gx = (m + TN - 1) / TN;
   PLIP_REQUIRE(gy <= 65535, "similarity: n=%lld too large for one launch (chunk rows)", (long long)n);

@@ -35,6 +35,15 @@ def shard_range(n: int, rank: int, world_size: int) -> Tuple[int, int]:
     return lo, lo + counts[rank]
 
 
+def merge_topk_candidates(cand_i: torch.Tensor, cand_v: torch.Tensor, k: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Merge per-shard top-k lists: ``cand_i`` int64 / ``cand_v`` ``[n_queries, shards * k]`` in shard-major order
+    (global indices, -1 for an exhausted list) -> the best ``k`` by score, equal scores by lower global index."""
+    cand_v = torch.where(cand_i < 0, torch.full_like(cand_v, float("-inf")), cand_v)
+    # shard-major candidate order = ascending global index among equal scores; a stable sort keeps it
+    order = torch.sort(cand_v, dim=1, descending=True, stable=True).indices[:, :k]
+    return torch.gather(cand_i, 1, order), torch.gather(cand_v, 1, order)
+
+
 def all_gather_rows(local: torch.Tensor, counts: Optional[Sequence[int]] = None, group=None) -> torch.Tensor:
     """Concatenate per-rank row blocks ``[n_r, d]`` in rank order -> ``[sum n_r, d]`` on every rank.
 
@@ -170,7 +179,10 @@ class ShardedCLIP:
         ``argsort()[-k:][::-1]`` over all images): every rank takes the fused top-k of all queries over its own
         gallery rows (never materialising ``[n_queries, n_gallery]``), the ``[n_queries, k]`` candidates (score +
         global image index) are all-gathered (8 x 10k x 50 x 8 B = 32 MB at cfg5) and merged.  Ties resolve to the
-        lower global index, as on one GPU.  Returns ``(idx int64 [n_queries,k], val [n_queries,k])`` on every rank."""
+        lower global index.  The result equals the one-GPU result bit for bit when every shard takes the path the
+        whole gallery takes (``plip_similarity_topk``: the tensor-core chunks for >= 256 queries and >= 8192 rows);
+        a shard below that runs the fp32 kernels, whose scores differ in the last bits, so near-ties may then
+        resolve differently than on one GPU (every score stays within its kernel's bound).  Returns ``(idx int64 [n_queries,k], val [n_queries,k])`` on every rank."""
         if self.topk is None:
             raise RuntimeError("ShardedCLIP was built without a top-k kernel")
         idx, val = self.topk(q_all, gal_local, k)                    # local candidates, descending
@@ -182,7 +194,4 @@ class ShardedCLIP:
         nq = q_all.shape[0]
         cand_v = all_gather_rows(val.contiguous()).view(self.world_size, nq, k).permute(1, 0, 2).reshape(nq, -1)
         cand_i = all_gather_rows(gidx.contiguous()).view(self.world_size, nq, k).permute(1, 0, 2).reshape(nq, -1)
-        cand_v = torch.where(cand_i < 0, torch.full_like(cand_v, float("-inf")), cand_v)
-        # rank-major candidate order = ascending global index among equal scores; a stable sort keeps it
-        order = torch.sort(cand_v, dim=1, descending=True, stable=True).indices[:, :k]
-        return torch.gather(cand_i, 1, order), torch.gather(cand_v, 1, order)
+        return merge_topk_candidates(cand_i, cand_v, k)
