@@ -32,7 +32,7 @@ extern "C" {
 
 #define PLIP_API __attribute__((visibility("default")))
 
-#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts, plip_window_mask_counts, plip_resize_region_*, plip_resize_filter_bounds, plip_sgd_*, plip_linear_decision, plip_densenet_*, plip_resize_crop_bilinear_u8, plip_warp_tiles_u8, plip_resize_crop_fill_u8, plip_mask_value_sets_u8, plip_encode_pair, plip_sgd_fit_f64, plip_linear_decision_f64 (new symbols only) */
+#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts, plip_window_mask_counts, plip_resize_region_*, plip_resize_filter_bounds, plip_sgd_*, plip_linear_decision, plip_densenet_*, plip_resize_crop_bilinear_u8, plip_warp_tiles_u8, plip_resize_crop_fill_u8, plip_mask_value_sets_u8, plip_encode_pair, plip_sgd_fit_f64, plip_linear_decision_f64, plip_dbg_layernorm_ex, plip_dbg_im2col_hw, plip_dbg_text_embed, plip_dbg_mask_to_i32, plip_dbg_cls_rows, plip_dbg_gather_rows (new symbols only) */
 
 /* Model constants (TF:configuration_clip.py:47-64,97-109,160-161). */
 #define PLIP_IMAGE_SIZE 224
@@ -488,6 +488,12 @@ PLIP_API int plip_dbg_rowstats_cast(const float* x, int64_t rows, int dim, void*
 PLIP_API int plip_dbg_layernorm(const float* x, int64_t rows, int dim, int64_t in_row_stride,
                                 const float* gamma, const float* beta, float* out_f32, void* out_bf16,
                                 void* stream);
+/* The whole LayerNorm launcher: row r of the output is LayerNorm(x + row_index[r] * in_row_stride) (row_index NULL:
+ * r * in_row_stride); out_f32 [rows, dim] and / or out16 [rows, dim] (either may be NULL; x == out_f32 is allowed).
+ * x, gamma, beta, out_f32 16-byte aligned, out16 8-byte aligned; dim 768 or 512. */
+PLIP_API int plip_dbg_layernorm_ex(const float* x, const int32_t* row_index, int64_t in_row_stride, int64_t rows,
+                                   int dim, const float* gamma, const float* beta, float* out_f32, void* out16,
+                                   void* stream);
 /* seq_len <= 128: any causal / key_mask; 128 < seq_len <= 1025 (long-sequence kernel): causal = 0, key_mask = NULL. */
 PLIP_API int plip_dbg_attention(const void* qkv_bf16, int64_t n_seq, int seq_len, int heads, int causal,
                                 const int32_t* key_mask, void* out_bf16, void* stream);
@@ -506,6 +512,24 @@ PLIP_API int plip_dbg_densenet_op(int op, const void* in_dev, int lda, int64_t n
                                   const float* a_scale, const float* a_shift, const float* e_scale,
                                   const float* e_shift, void* out_dev, int ldo, void* stream);
 PLIP_API int plip_dbg_im2col(const void* pixels, int pixel_format, int64_t n, void* out_bf16, void* stream);
+/* plip_dbg_im2col at any image size plip_encode_images_hw accepts: out16 [n * (height/32) * (width/32), 3072]. */
+PLIP_API int plip_dbg_im2col_hw(const void* pixels, int pixel_format, int64_t n, int height, int width, void* out16,
+                                void* stream);
+/* Text embeddings of n captions (the first seq_len of ids_stride ids per row) with caller tables tok float32
+ * [49408, 512] and pos float32 [>= seq_len, 512]: x_out [n * seq_len, 512] and the pooled row b * seq_len + t of each
+ * caption in eos_rows_out int32 [n] (t = first eos 49407, else 0, or with no_eos_argmax the first largest id). */
+PLIP_API int plip_dbg_text_embed(const void* ids, int ids_dtype, int64_t n, int seq_len, int ids_stride,
+                                 const float* tok, const float* pos, float* x_out, int32_t* eos_rows_out,
+                                 int no_eos_argmax, void* stream);
+/* out[i] = mask[(i / seq_len) * stride + i % seq_len] != 0 for i < count (mask_dtype PLIP_IDS_I32 / I64). */
+PLIP_API int plip_dbg_mask_to_i32(const void* mask, int mask_dtype, int64_t count, int seq_len, int stride,
+                                  int32_t* out, void* stream);
+/* x[b * seq * 768 + c] = cls[c] + pos[c] for b < n: the class rows of n sequences of seq rows. */
+PLIP_API int plip_dbg_cls_rows(const float* cls, const float* pos, int64_t n, int seq, float* x, void* stream);
+/* Rows idx(i) = row_index[i] (or i * row_stride when row_index is NULL) of a16 [*, dim] (16-bit) and x32 [*, dim]
+ * (float32) copied to rows i of a16_out and x32_out, i < n; every pointer 16-byte aligned, dim % 8 == 0. */
+PLIP_API int plip_dbg_gather_rows(const void* a16, const float* x32, const int32_t* row_index, int64_t row_stride,
+                                  int64_t n, int dim, void* a16_out, float* x32_out, void* stream);
 /* The vision position table pos_dev (float32 [50,768]) resized to a grid_h x grid_w patch grid as
  * plip_encode_images_hw does it: out_dev float32 [1 + grid_h * grid_w, 768]; 1 <= grid_h, grid_w <= 32. */
 PLIP_API int plip_dbg_pos_interp(const float* pos_dev, int grid_h, int grid_w, float* out_dev, void* stream);

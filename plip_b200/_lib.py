@@ -148,6 +148,12 @@ SIGNATURES = {
     "plip_dbg_hidden_states": (_i, [_vp, _i, _vp, _i, _vp, _i64, _i, _fp, _vp]),
     "plip_dbg_pos_interp": (_i, [_fp, _i, _i, _fp, _vp]),
     "plip_dbg_hidden_states_hw": (_i, [_vp, _vp, _i, _i64, _i, _i, _i, _fp, _vp]),
+    "plip_dbg_layernorm_ex": (_i, [_fp, _vp, _i64, _i64, _i, _fp, _fp, _fp, _vp, _vp]),
+    "plip_dbg_im2col_hw": (_i, [_vp, _i, _i64, _i, _i, _vp, _vp]),
+    "plip_dbg_text_embed": (_i, [_vp, _i, _i64, _i, _i, _fp, _fp, _fp, _vp, _i, _vp]),
+    "plip_dbg_mask_to_i32": (_i, [_vp, _i, _i64, _i, _i, _vp, _vp]),
+    "plip_dbg_cls_rows": (_i, [_fp, _fp, _i64, _i, _fp, _vp]),
+    "plip_dbg_gather_rows": (_i, [_vp, _fp, _vp, _i64, _i64, _i, _vp, _fp, _vp]),
 }
 
 _LIB = None

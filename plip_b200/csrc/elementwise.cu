@@ -516,6 +516,9 @@ __global__ void __launch_bounds__(kEwThreads) l2_normalize_kernel(float* __restr
   }
 }
 
+// p is a multiple of `bytes` (a power of two); null passes (optional outputs are checked where they are required).
+inline bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
 inline int grid_for(int64_t work_items, int per_block) {
   int64_t blocks = (work_items + per_block - 1) / per_block;
   const int64_t cap = 16LL * sm_count();
@@ -533,7 +536,11 @@ int launch_im2col(const void* pixels, int fmt, int64_t n, int height, int width,
                "im2col: image size %dx%d out of range", height, width);
   const bool fixed = height == kImage && width == kImage;
   const uintptr_t addr = reinterpret_cast<uintptr_t>(pixels);
+  PLIP_REQUIRE(pixels && out, "im2col: null argument");
   PLIP_REQUIRE(!fixed || (addr & 15) == 0, "im2col: pixels must be 16-byte aligned");
+  PLIP_REQUIRE(aligned(pixels, fmt == PLIP_PIX_F32_NCHW ? 4 : fmt == PLIP_PIX_BF16_NCHW ? 2 : 1),
+               "im2col: pixels not aligned to their element size");
+  PLIP_REQUIRE(aligned(out, 16), "im2col: out must be 16-byte aligned");
   // vector loads need every row start aligned: f32 16 B (W % 4 == 0), bf16 16 B (W % 8), u8 8 B (3 W % 8)
   const bool aligned = (addr & (fmt == PLIP_PIX_U8_NHWC ? 7 : 15)) == 0;
   const int vec = aligned && width % (fmt == PLIP_PIX_F32_NCHW ? 4 : 8) == 0 ? 1 : 0;
@@ -596,6 +603,10 @@ int launch_layernorm(const float* x, const int32_t* row_index, int64_t in_row_st
                      cudaStream_t st) {
   PLIP_REQUIRE(rows > 0, "layernorm: rows must be positive");
   PLIP_REQUIRE(in_row_stride % 4 == 0, "layernorm: row stride must be a multiple of 4 floats");
+  PLIP_REQUIRE(x && gamma && beta, "layernorm: null argument");
+  // float4 loads of x, gamma, beta and stores of out_f32; 8-byte stores of the 16-bit output
+  PLIP_REQUIRE(aligned(x, 16) && aligned(gamma, 16) && aligned(beta, 16) && aligned(out_f32, 16) && aligned(out_bf16, 8),
+               "layernorm: x, gamma, beta and out_f32 must be 16-byte aligned, the 16-bit output 8-byte aligned");
   const int grid = grid_for(rows, kEwThreads / 32);
   if (dim == kVisDim)
     PLIP_CUDA_CHECK(launch_kernel(layernorm_kernel<kVisDim>, dim3(grid), dim3(kEwThreads), 0, st, 1, x, row_index, in_row_stride, rows, gamma, beta, out_f32, out_bf16, f16));
@@ -611,6 +622,9 @@ int launch_layernorm(const float* x, const int32_t* row_index, int64_t in_row_st
 
 int launch_rowstats_cast(const float* x, int64_t rows, int dim, __nv_bfloat16* xb, float2* stats, int f16, cudaStream_t st) {
   PLIP_REQUIRE(rows > 0, "rowstats_cast: rows must be positive");
+  PLIP_REQUIRE(x && xb && stats, "rowstats_cast: null argument");
+  PLIP_REQUIRE(aligned(x, 16) && aligned(xb, 8) && aligned(stats, 8),
+               "rowstats_cast: x must be 16-byte aligned, xb and stats 8-byte aligned");
   const int grid = grid_for(rows, kEwThreads / 32);
   if (dim == kVisDim)
     PLIP_CUDA_CHECK(launch_kernel(rowstats_cast_kernel<kVisDim>, dim3(grid), dim3(kEwThreads), 0, st, 1, x, rows, xb, stats, f16));
@@ -620,6 +634,7 @@ int launch_rowstats_cast(const float* x, int64_t rows, int dim, __nv_bfloat16* x
     set_last_error("rowstats_cast: unsupported dim %d", dim);
     return -2;
   }
+  PLIP_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 
@@ -628,6 +643,10 @@ int launch_text_embed(const void* ids, int ids_dtype, int64_t n, int seq_len, in
   PLIP_REQUIRE(ids_stride >= seq_len, "text_embed: ids row stride %d < seq_len %d", ids_stride, seq_len);
   PLIP_REQUIRE(n > 0 && seq_len > 0 && seq_len <= kTxtSeq, "text_embed: bad shape n=%lld seq_len=%d",
                (long long)n, seq_len);
+  PLIP_REQUIRE(ids && tok && pos && x && eos_rows, "text_embed: null argument");
+  PLIP_REQUIRE(aligned(ids, ids_dtype == PLIP_IDS_I64 ? 8 : 4) && aligned(tok, 16) && aligned(pos, 16) && aligned(x, 16) &&
+                   aligned(eos_rows, 4),
+               "text_embed: tok, pos and x must be 16-byte aligned, ids and eos_rows to their element size");
   const int grid = grid_for(n * seq_len, kEwThreads / 32);
   const int grid2 = grid_for(n, kEwThreads / 32);
   if (ids_dtype == PLIP_IDS_I64) {
@@ -646,6 +665,12 @@ int launch_text_embed(const void* ids, int ids_dtype, int64_t n, int seq_len, in
 
 int launch_mask_to_i32(const void* mask, int dtype, int64_t count, int seq_len, int stride, int32_t* out,
                        cudaStream_t st) {
+  PLIP_REQUIRE(mask && out, "mask_to_i32: null argument");
+  PLIP_REQUIRE(dtype == PLIP_IDS_I32 || dtype == PLIP_IDS_I64, "mask_to_i32: unknown mask dtype %d", dtype);
+  PLIP_REQUIRE(count > 0 && seq_len > 0 && stride >= seq_len && count % seq_len == 0,
+               "mask_to_i32: bad shape count=%lld seq_len=%d stride=%d", (long long)count, seq_len, stride);
+  PLIP_REQUIRE(aligned(mask, dtype == PLIP_IDS_I64 ? 8 : 4) && aligned(out, 4),
+               "mask_to_i32: mask and out must be aligned to their element size");
   const int grid = grid_for(count, kEwThreads);
   if (dtype == PLIP_IDS_I64)
     PLIP_CUDA_CHECK(launch_kernel(mask_to_i32_kernel<long long>, dim3(grid), dim3(kEwThreads), 0, st, 1, static_cast<const long long*>(mask), count, seq_len, stride, out));
@@ -656,6 +681,9 @@ int launch_mask_to_i32(const void* mask, int dtype, int64_t count, int seq_len, 
 }
 
 int launch_cls_rows(const float* cls, const float* pos, int64_t n, int seq, float* x, cudaStream_t st) {
+  PLIP_REQUIRE(cls && pos && x, "cls_rows: null argument");
+  PLIP_REQUIRE(n > 0 && seq > 0, "cls_rows: bad shape n=%lld seq=%d", (long long)n, seq);
+  PLIP_REQUIRE(aligned(cls, 16) && aligned(pos, 16) && aligned(x, 16), "cls_rows: cls, pos and x must be 16-byte aligned");
   PLIP_CUDA_CHECK(launch_kernel(cls_rows_kernel, dim3(grid_for(n * (kVisDim / 4), kEwThreads)), dim3(kEwThreads), 0, st, 1, cls, pos, n, seq, x));
   PLIP_CUDA_CHECK(cudaGetLastError());
   return 0;
@@ -664,6 +692,10 @@ int launch_cls_rows(const float* cls, const float* pos, int64_t n, int seq, floa
 int launch_gather_rows(const __nv_bfloat16* a16, const float* x32, const int32_t* row_index, int64_t row_stride,
                        int64_t n, int dim, __nv_bfloat16* a16_out, float* x32_out, cudaStream_t st) {
   PLIP_REQUIRE(n > 0 && dim > 0 && dim % 8 == 0, "gather_rows: bad shape");
+  PLIP_REQUIRE(a16 && x32 && a16_out && x32_out, "gather_rows: null argument");
+  PLIP_REQUIRE(row_index || row_stride >= 0, "gather_rows: negative row stride");
+  PLIP_REQUIRE(aligned(a16, 16) && aligned(x32, 16) && aligned(a16_out, 16) && aligned(x32_out, 16) && aligned(row_index, 4),
+               "gather_rows: a16, x32 and both outputs must be 16-byte aligned");
   const int64_t items = n * (dim / 8 + dim / 4);
   PLIP_CUDA_CHECK(launch_kernel(gather_rows_kernel, dim3(grid_for(items, kEwThreads)), dim3(kEwThreads), 0, st, 1,
                                 reinterpret_cast<const uint4*>(a16), reinterpret_cast<const uint4*>(x32), row_index,

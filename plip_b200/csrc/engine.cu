@@ -1617,6 +1617,13 @@ PLIP_API int plip_dbg_layernorm(const float* x, int64_t rows, int dim, int64_t i
                           static_cast<__nv_bfloat16*>(out_bf16), g_dbg_f16, static_cast<cudaStream_t>(stream));
 }
 
+PLIP_API int plip_dbg_layernorm_ex(const float* x, const int32_t* row_index, int64_t in_row_stride, int64_t rows,
+                                   int dim, const float* gamma, const float* beta, float* out_f32, void* out16,
+                                   void* stream) {
+  return launch_layernorm(x, row_index, in_row_stride, rows, dim, gamma, beta, out_f32,
+                          static_cast<__nv_bfloat16*>(out16), g_dbg_f16, static_cast<cudaStream_t>(stream));
+}
+
 PLIP_API int plip_dbg_attention(const void* qkv_bf16, int64_t n_seq, int seq_len, int heads, int causal,
                                 const int32_t* key_mask, void* out_bf16, void* stream) {
   return launch_attention(static_cast<const __nv_bfloat16*>(qkv_bf16), n_seq, seq_len, heads, causal != 0, key_mask,
@@ -1632,6 +1639,34 @@ PLIP_API int plip_dbg_attention_probs(const void* qkv_bf16, int64_t n_seq, int s
 PLIP_API int plip_dbg_im2col(const void* pixels, int pixel_format, int64_t n, void* out_bf16, void* stream) {
   return launch_im2col(pixels, pixel_format, n, kImage, kImage, static_cast<__nv_bfloat16*>(out_bf16), g_dbg_f16,
                        static_cast<cudaStream_t>(stream));
+}
+
+PLIP_API int plip_dbg_im2col_hw(const void* pixels, int pixel_format, int64_t n, int height, int width, void* out16,
+                                void* stream) {
+  return launch_im2col(pixels, pixel_format, n, height, width, static_cast<__nv_bfloat16*>(out16), g_dbg_f16,
+                       static_cast<cudaStream_t>(stream));
+}
+
+PLIP_API int plip_dbg_text_embed(const void* ids, int ids_dtype, int64_t n, int seq_len, int ids_stride,
+                                 const float* tok, const float* pos, float* x_out, int32_t* eos_rows_out,
+                                 int no_eos_argmax, void* stream) {
+  return launch_text_embed(ids, ids_dtype, n, seq_len, ids_stride, tok, pos, x_out, eos_rows_out, kEosId,
+                           no_eos_argmax, static_cast<cudaStream_t>(stream));
+}
+
+PLIP_API int plip_dbg_mask_to_i32(const void* mask, int mask_dtype, int64_t count, int seq_len, int stride,
+                                  int32_t* out, void* stream) {
+  return launch_mask_to_i32(mask, mask_dtype, count, seq_len, stride, out, static_cast<cudaStream_t>(stream));
+}
+
+PLIP_API int plip_dbg_cls_rows(const float* cls, const float* pos, int64_t n, int seq, float* x, void* stream) {
+  return launch_cls_rows(cls, pos, n, seq, x, static_cast<cudaStream_t>(stream));
+}
+
+PLIP_API int plip_dbg_gather_rows(const void* a16, const float* x32, const int32_t* row_index, int64_t row_stride,
+                                  int64_t n, int dim, void* a16_out, float* x32_out, void* stream) {
+  return launch_gather_rows(static_cast<const __nv_bfloat16*>(a16), x32, row_index, row_stride, n, dim,
+                            static_cast<__nv_bfloat16*>(a16_out), x32_out, static_cast<cudaStream_t>(stream));
 }
 
 PLIP_API int plip_dbg_pos_interp(const float* pos_dev, int grid_h, int grid_w, float* out_dev, void* stream) {

@@ -55,6 +55,9 @@ def test_pos_interp_matches_torch_bicubic(state_dict, gh, gw):
     if (gh, gw) == (7, 7):
         assert torch.equal(got, pos)
     assert (got - ref).abs().max().item() <= 1e-6 * pos.abs().max().item()
+    from helper_oracle import pos_interp_ref
+    cref, slack = pos_interp_ref(pos, gh, gw)               # the kernel's fp32 weights, gamma(8) sum |w||p| per element
+    assert ((got.double() - cref).abs() <= slack).all()
 
 
 # ---- 2. vision hidden states -------------------------------------------------------------------------------------
