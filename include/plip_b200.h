@@ -32,7 +32,7 @@ extern "C" {
 
 #define PLIP_API __attribute__((visibility("default")))
 
-#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts, plip_window_mask_counts, plip_resize_region_*, plip_resize_filter_bounds, plip_sgd_*, plip_linear_decision, plip_densenet_*, plip_resize_crop_bilinear_u8, plip_warp_tiles_u8, plip_resize_crop_fill_u8, plip_mask_value_sets_u8, plip_encode_pair, plip_sgd_fit_f64, plip_linear_decision_f64, plip_dbg_layernorm_ex, plip_dbg_im2col_hw, plip_dbg_text_embed, plip_dbg_mask_to_i32, plip_dbg_cls_rows, plip_dbg_gather_rows (new symbols only) */
+#define PLIP_B200_ABI_VERSION 5  /* 3: + plip_resize_crop_u8; 4: + plip_profile_*, plip_create_ex (operand format); 5: + plip_set_last_layer_pruning, later plip_*_hw, plip_*_outputs, plip_encode_windows, plip_window_background_counts, plip_window_mask_counts, plip_resize_region_*, plip_resize_filter_bounds, plip_sgd_*, plip_linear_decision, plip_densenet_*, plip_resize_crop_bilinear_u8, plip_warp_tiles_u8, plip_resize_crop_fill_u8, plip_mask_value_sets_u8, plip_encode_pair, plip_sgd_fit_f64, plip_linear_decision_f64, plip_dbg_layernorm_ex, plip_dbg_im2col_hw, plip_dbg_text_embed, plip_dbg_mask_to_i32, plip_dbg_cls_rows, plip_dbg_gather_rows, plip_weights_*_patch, plip_create_patch, plip_vision_patch, plip_dbg_im2col_patch, plip_dbg_window_im2col_patch, plip_dbg_pos_interp_patch (new symbols only) */
 
 /* Model constants (TF:configuration_clip.py:47-64,97-109,160-161). */
 #define PLIP_IMAGE_SIZE 224
@@ -89,6 +89,12 @@ typedef struct plip_tensor_info {
 PLIP_API int plip_weights_num_tensors(void);
 PLIP_API int plip_weights_tensor_info(int index, plip_tensor_info_t* info);
 PLIP_API uint64_t plip_weights_blob_bytes(void);
+/* The layout above is CLIP ViT-B/32's (PLIP).  The same for a vision patch size: 32 (the functions above) or 16
+ * (CLIP ViT-B/16: the same tensors in the same order; only patch_embedding.weight [768, 768] and
+ * position_embedding.weight [197, 768] differ, so every offset after the first differs too).
+ * plip_weights_num_tensors() holds for both.  blob_bytes_patch returns 0 for another patch size. */
+PLIP_API int plip_weights_tensor_info_patch(int patch, int index, plip_tensor_info_t* info);
+PLIP_API uint64_t plip_weights_blob_bytes_patch(int patch);
 
 /* ---- engine lifetime ----------------------------------------------------------------------- */
 /* host_blob: packed weights (layout above), plus exp(logit_scale) passed separately.
@@ -101,11 +107,20 @@ PLIP_API int plip_create(const void* host_blob, uint64_t blob_bytes, float logit
 /* Same with an explicit operand format: the 16-bit entries of host_blob must have been packed in that format. */
 PLIP_API int plip_create_ex(const void* host_blob, uint64_t blob_bytes, float logit_scale_exp, int device,
                             int max_micro_batch, int operand_format, plip_engine_t** out);
+/* Same for the vision patch size of the weights: 32 (ViT-B/32, = plip_create_ex) or 16 (ViT-B/16, blob in the
+ * plip_weights_tensor_info_patch(16, ...) layout).  Every vision call of the engine uses that patch size: images of
+ * H x W pixels have (H / P) * (W / P) patches (196 at 224 x 224 for P = 16, 197 tokens), at most 32 per side, and a
+ * micro-batch holds floor(50 * max_micro_batch / S) images of S tokens (259 of 197 tokens at 1024), so a ViT-B/16
+ * engine needs max_micro_batch >= 4. */
+PLIP_API int plip_create_patch(const void* host_blob, uint64_t blob_bytes, float logit_scale_exp, int device,
+                               int max_micro_batch, int operand_format, int vision_patch, plip_engine_t** out);
 PLIP_API int plip_destroy(plip_engine_t* e);
 PLIP_API uint64_t plip_workspace_bytes(int max_micro_batch);
 PLIP_API float plip_logit_scale_exp(const plip_engine_t* e);
 PLIP_API int plip_max_micro_batch(const plip_engine_t* e);
 PLIP_API int plip_operand_format(const plip_engine_t* e);
+/* The engine's vision patch size (32 or 16; 0 for a NULL handle). */
+PLIP_API int plip_vision_patch(const plip_engine_t* e);
 /* Pooled position of a caption WITHOUT an eos token (49407).  0 (default): position 0, as transformers does for
  * configs with eos_token_id == 49407 (TF:571-584: argmax of an all-zero match vector).  1: first position of the
  * largest id, as legacy configs (eos_token_id == 2 — what openai/clip-vit-base-patch32 ships) and OpenAI clip's
@@ -515,6 +530,15 @@ PLIP_API int plip_dbg_im2col(const void* pixels, int pixel_format, int64_t n, vo
 /* plip_dbg_im2col at any image size plip_encode_images_hw accepts: out16 [n * (height/32) * (width/32), 3072]. */
 PLIP_API int plip_dbg_im2col_hw(const void* pixels, int pixel_format, int64_t n, int height, int width, void* out16,
                                 void* stream);
+/* plip_dbg_im2col_hw for a patch size of 32 or 16: out16 [n * (height/patch) * (width/patch), 3 * patch^2], row
+ * b * gh * gw + py * gw + px, column c * patch^2 + ky * patch + kx. */
+PLIP_API int plip_dbg_im2col_patch(const void* pixels, int pixel_format, int64_t n, int height, int width, int patch,
+                                   void* out16, void* stream);
+/* The patch matrix plip_encode_windows builds: n 224 x 224 windows of a uint8 RGB region (rows row_pitch_bytes apart)
+ * at device int32 (row, col) origins_dev [n, 2] (8-byte aligned, each window inside the region; not checked here),
+ * in the layout of plip_dbg_im2col_patch. */
+PLIP_API int plip_dbg_window_im2col_patch(const void* region_dev, int64_t row_pitch_bytes, const int32_t* origins_dev,
+                                          int64_t n, int patch, void* out16, void* stream);
 /* Text embeddings of n captions (the first seq_len of ids_stride ids per row) with caller tables tok float32
  * [49408, 512] and pos float32 [>= seq_len, 512]: x_out [n * seq_len, 512] and the pooled row b * seq_len + t of each
  * caption in eos_rows_out int32 [n] (t = first eos 49407, else 0, or with no_eos_argmax the first largest id). */
@@ -533,6 +557,9 @@ PLIP_API int plip_dbg_gather_rows(const void* a16, const float* x32, const int32
 /* The vision position table pos_dev (float32 [50,768]) resized to a grid_h x grid_w patch grid as
  * plip_encode_images_hw does it: out_dev float32 [1 + grid_h * grid_w, 768]; 1 <= grid_h, grid_w <= 32. */
 PLIP_API int plip_dbg_pos_interp(const float* pos_dev, int grid_h, int grid_w, float* out_dev, void* stream);
+/* The same for the stored table of a patch size: 32 (pos_dev [50, 768], a 7 x 7 grid) or 16 ([197, 768], 14 x 14). */
+PLIP_API int plip_dbg_pos_interp_patch(const float* pos_dev, int patch, int grid_h, int grid_w, float* out_dev,
+                                       void* stream);
 /* Vision tower at any image size (plip_encode_images_hw geometry): the fp32 residual stream [n*S, 768] after
  * `num_layers` layers; n must fit one pass. */
 PLIP_API int plip_dbg_hidden_states_hw(plip_engine_t* e, const void* pixels_dev, int pixel_format, int64_t n,

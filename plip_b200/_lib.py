@@ -83,9 +83,13 @@ SIGNATURES = {
     "plip_weights_num_tensors": (_i, []),
     "plip_weights_tensor_info": (_i, [_i, C.POINTER(TensorInfo)]),
     "plip_weights_blob_bytes": (_u64, []),
+    "plip_weights_tensor_info_patch": (_i, [_i, _i, C.POINTER(TensorInfo)]),
+    "plip_weights_blob_bytes_patch": (_u64, [_i]),
     "plip_create": (_i, [_vp, _u64, _f, _i, _i, C.POINTER(_vp)]),
     "plip_create_ex": (_i, [_vp, _u64, _f, _i, _i, _i, C.POINTER(_vp)]),
+    "plip_create_patch": (_i, [_vp, _u64, _f, _i, _i, _i, _i, C.POINTER(_vp)]),
     "plip_operand_format": (_i, [_vp]),
+    "plip_vision_patch": (_i, [_vp]),
     "plip_set_text_pooling": (_i, [_vp, _i]),
     "plip_set_last_layer_pruning": (_i, [_vp, _i]),
     "plip_last_layer_pruning": (_i, [_vp]),
@@ -150,6 +154,9 @@ SIGNATURES = {
     "plip_dbg_hidden_states_hw": (_i, [_vp, _vp, _i, _i64, _i, _i, _i, _fp, _vp]),
     "plip_dbg_layernorm_ex": (_i, [_fp, _vp, _i64, _i64, _i, _fp, _fp, _fp, _vp, _vp]),
     "plip_dbg_im2col_hw": (_i, [_vp, _i, _i64, _i, _i, _vp, _vp]),
+    "plip_dbg_im2col_patch": (_i, [_vp, _i, _i64, _i, _i, _i, _vp, _vp]),
+    "plip_dbg_window_im2col_patch": (_i, [_vp, _i64, _vp, _i64, _i, _vp, _vp]),
+    "plip_dbg_pos_interp_patch": (_i, [_fp, _i, _i, _i, _fp, _vp]),
     "plip_dbg_text_embed": (_i, [_vp, _i, _i64, _i, _i, _fp, _fp, _fp, _vp, _i, _vp]),
     "plip_dbg_mask_to_i32": (_i, [_vp, _i, _i64, _i, _i, _vp, _vp]),
     "plip_dbg_cls_rows": (_i, [_fp, _fp, _i64, _i, _fp, _vp]),

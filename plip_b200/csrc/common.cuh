@@ -30,6 +30,12 @@ constexpr int kVisDim = 768;
 constexpr int kVisHeads = 12;
 constexpr int kVisFF = 3072;
 constexpr int kPatchK = 3072;      // 3 * 32 * 32
+// CLIP ViT-B/16: the same towers behind a 16-pixel patch.  An engine's patch size (32 or 16) comes from its weights;
+// the k* constants above are the ViT-B/32 geometry, these give any accepted patch size's.
+constexpr int kPatch16 = 16;
+constexpr int vis_grid(int patch) { return kImage / patch; }                      // 7 or 14 patches per side at 224
+constexpr int vis_seq(int patch) { return vis_grid(patch) * vis_grid(patch) + 1; }  // 50 or 197 tokens at 224
+constexpr int patch_k(int patch) { return 3 * patch * patch; }                    // 3072 or 768
 constexpr int kTxtSeq = 77;
 constexpr int kTxtDim = 512;
 constexpr int kTxtHeads = 8;

@@ -22,12 +22,13 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8], int f16) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// im2col of non-overlapping 32x32 patches: pixels -> A0[b*49 + py*7 + px][c*1024 + ky*32 + kx] (bf16).
-// Restates nn.Conv2d(3,768,32,32,bias=False) input gathering (TF:modeling_clip.py:148-154,209-210);
+// im2col of non-overlapping P x P patches (P = 32: ViT-B/32, 16: ViT-B/16):
+// pixels -> A0[b*patches + py*gw + px][c*P*P + ky*P + kx] (bf16), i.e. [b*49 + py*7 + px][c*1024 + ky*32 + kx] at 32.
+// Restates nn.Conv2d(3,768,P,P,bias=False) input gathering (TF:modeling_clip.py:148-154,209-210);
 // the uint8 path fuses CLIPImageProcessor's rescale + normalise (TF:image_processing_clip.py:50-62).
-// One thread moves 8 consecutive x of one image row.
-// Any image size (interpolated position table): the image is H x W, the patch grid gh x gw (the H % 32 bottom rows
-// and W % 32 right columns are never read, as with the stride-32 conv).  FIXED = the 224 x 224 geometry as
+// One thread moves 8 consecutive x of one image row (a patch row is 4 or 2 such groups).
+// Any image size (interpolated position table): the image is H x W, the patch grid gh x gw (the H % P bottom rows
+// and W % P right columns are never read, as with the stride-P conv).  FIXED = the 224 x 224 geometry as
 // compile-time constants.  vec = 0 (rows whose start is not aligned for the vector loads, e.g. W = 250): the same
 // pixels read one value at a time.
 // ------------------------------------------------------------------------------------------------
@@ -35,8 +36,17 @@ struct ImGeom {
   int H, W, gh, gw;
 };
 
+template <int P>
+struct PatchShift;  // log2 of the patch size: patch coordinates by shifts and masks
+template <>
+struct PatchShift<32> { static constexpr int value = 5; };
+template <>
+struct PatchShift<16> { static constexpr int value = 4; };
+
 // 8 consecutive RGB pixels of one image row (24 bytes, interleaved) -> the three channel rows of one patch-matrix row
-// at dst (channel c at dst + c * 1024).  Shared by the tile and the window im2col, so both produce the same bits.
+// at dst (channel c at dst + c * CS, CS = P * P).  Shared by the tile and the window im2col, so both produce the same
+// bits.
+template <int CS>
 __device__ __forceinline__ void store_u8_patch_row(const uint8_t (&bytes)[24], __nv_bfloat16* dst, int f16) {
   const float mean[3] = {0.48145466f, 0.4578275f, 0.40821073f};
   const float istd[3] = {1.0f / 0.26862954f, 1.0f / 0.26130258f, 1.0f / 0.27577711f};
@@ -45,18 +55,19 @@ __device__ __forceinline__ void store_u8_patch_row(const uint8_t (&bytes)[24], _
     float f[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) f[j] = (bytes[j * 3 + c] * (1.0f / 255.0f) - mean[c]) * istd[c];
-    *reinterpret_cast<uint4*>(dst + c * 1024) = pack8(f, f16);
+    *reinterpret_cast<uint4*>(dst + c * CS) = pack8(f, f16);
   }
 }
 
-template <int FMT, bool FIXED>
+template <int FMT, bool FIXED, int P>
 __global__ void __launch_bounds__(kEwThreads) im2col_kernel(const void* __restrict__ pixels,
                                                             __nv_bfloat16* __restrict__ out, int64_t n, int f16,
                                                             ImGeom geo, int vec) {
+  constexpr int SH = PatchShift<P>::value, CS = P * P, K = 3 * CS;
   const int H = FIXED ? kImage : geo.H, W = FIXED ? kImage : geo.W;
-  const int gw = FIXED ? kGrid : geo.gw, patches = FIXED ? kPatches : geo.gh * geo.gw;
-  const int rows = FIXED ? kImage : geo.gh * 32;  // image rows that reach a patch
-  const int kX8 = FIXED ? kImage / 8 : geo.gw * 4;  // groups of 8 pixels per image row (28 at 224)
+  const int gw = FIXED ? vis_grid(P) : geo.gw, patches = FIXED ? vis_grid(P) * vis_grid(P) : geo.gh * geo.gw;
+  const int rows = FIXED ? kImage : geo.gh * P;  // image rows that reach a patch
+  const int kX8 = FIXED ? kImage / 8 : geo.gw * (P / 8);  // groups of 8 pixels per image row (28 at 224)
   const bool vload = FIXED || vec != 0;
   const int64_t total = (FMT == PLIP_PIX_U8_NHWC) ? n * rows * kX8 : n * 3 * rows * kX8;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
@@ -66,7 +77,7 @@ __global__ void __launch_bounds__(kEwThreads) im2col_kernel(const void* __restri
     const int y = (int)(r % rows);
     r /= rows;
     const int x = x8 * 8;
-    const int py = y >> 5, ky = y & 31, px = x >> 5, kx = x & 31;
+    const int py = y >> SH, ky = y & (P - 1), px = x >> SH, kx = x & (P - 1);
     if constexpr (FMT == PLIP_PIX_U8_NHWC) {
       const int64_t b = r;
       const uint8_t* src = static_cast<const uint8_t*>(pixels) + ((b * H + y) * W + x) * 3;
@@ -81,13 +92,13 @@ __global__ void __launch_bounds__(kEwThreads) im2col_kernel(const void* __restri
 #pragma unroll
         for (int j = 0; j < 24; ++j) bytes[j] = __ldg(src + j);
       }
-      store_u8_patch_row(bytes, out + (b * patches + py * gw + px) * (int64_t)kPatchK + ky * 32 + kx, f16);
+      store_u8_patch_row<CS>(bytes, out + (b * patches + py * gw + px) * (int64_t)K + ky * P + kx, f16);
     } else {
       const int c = (int)(r % 3);
       const int64_t b = r / 3;
       const int64_t src_off = ((b * 3 + c) * H + y) * W + x;
       __nv_bfloat16* dst =
-          out + (b * patches + py * gw + px) * (int64_t)kPatchK + c * 1024 + ky * 32 + kx;
+          out + (b * patches + py * gw + px) * (int64_t)K + c * CS + ky * P + kx;
       if constexpr (FMT == PLIP_PIX_F32_NCHW) {
         const float* s = static_cast<const float*>(pixels) + src_off;
         float f[8];
@@ -155,11 +166,13 @@ __device__ __forceinline__ void load24(const uint8_t* src, uint8_t (&bytes)[24])
   for (int k = 0; k < 6; ++k) out[k] = __byte_perm(v[k], v[k + 1], sel);
 }
 
-// Window im2col: the matrix im2col_kernel<PLIP_PIX_U8_NHWC, true> builds from the same windows cut out as [n,224,224,3]
-// tiles, bit for bit (same store_u8_patch_row).  origins: device int32 (row, col) pairs, one per window.
+// Window im2col: the matrix im2col_kernel<PLIP_PIX_U8_NHWC, true, P> builds from the same windows cut out as
+// [n,224,224,3] tiles, bit for bit (same store_u8_patch_row).  origins: device int32 (row, col) pairs, one per window.
+template <int P>
 __global__ void __launch_bounds__(kEwThreads) window_im2col_kernel(const uint8_t* __restrict__ region, int64_t pitch,
                                                                    const int2* __restrict__ origins, int64_t n,
                                                                    __nv_bfloat16* __restrict__ out, int f16) {
+  constexpr int SH = PatchShift<P>::value, CS = P * P, K = 3 * CS, G = vis_grid(P);
   constexpr int kX8 = kImage / 8;
   const int64_t total = n * kImage * kX8;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
@@ -172,8 +185,8 @@ __global__ void __launch_bounds__(kEwThreads) window_im2col_kernel(const uint8_t
     const int2 o = __ldg(origins + b);
     alignas(16) uint8_t bytes[24];
     load24(region + (int64_t)(o.x + y) * pitch + (int64_t)(o.y + x) * 3, bytes);
-    const int py = y >> 5, ky = y & 31, px = x >> 5, kx = x & 31;
-    store_u8_patch_row(bytes, out + (b * kPatches + py * kGrid + px) * (int64_t)kPatchK + ky * 32 + kx, f16);
+    const int py = y >> SH, ky = y & (P - 1), px = x >> SH, kx = x & (P - 1);
+    store_u8_patch_row<CS>(bytes, out + (b * (G * G) + py * G + px) * (int64_t)K + ky * P + kx, f16);
   }
 }
 
@@ -439,12 +452,14 @@ __global__ void __launch_bounds__(kEwThreads) cls_rows_kernel(const float* __res
 }
 
 // Position table of a gh x gw patch grid (TF:modeling_clip.py:161-200, interpolate_pos_encoding): row 0 (class) is
-// copied; rows 1..49 of the stored table, viewed as [768, 7, 7], are resized to [768, gh, gw] the way
-// F.interpolate(mode="bicubic", align_corners=False) does it: cubic convolution with A = -0.75, source coordinate
-// (i + 0.5) * 7 / g - 0.5, taps clamped to [0, 6], no antialias; out row 1 + y * gw + x.  One thread per output value.
+// copied; rows 1..SRC^2 of the stored table (SRC = 7 for ViT-B/32, 14 for ViT-B/16), viewed as [768, SRC, SRC], are
+// resized to [768, gh, gw] the way F.interpolate(mode="bicubic", align_corners=False) does it: cubic convolution with
+// A = -0.75, source coordinate (i + 0.5) * SRC / g - 0.5, taps clamped to [0, SRC - 1], no antialias; out row
+// 1 + y * gw + x.  One thread per output value.
+template <int SRC>
 __device__ __forceinline__ void cubic_taps(int g, int i, int (&idx)[4], float (&w)[4]) {
   constexpr float A = -0.75f;
-  const float scale = (float)kGrid / (float)g;
+  const float scale = (float)SRC / (float)g;
   const float real = scale * ((float)i + 0.5f) - 0.5f;
   const float fl = floorf(real);
   const float t = real - fl;
@@ -454,9 +469,10 @@ __device__ __forceinline__ void cubic_taps(int g, int i, int (&idx)[4], float (&
   w[2] = ((A + 2.f) * t2 - (A + 3.f)) * t2 * t2 + 1.f;
   w[3] = ((A * t3 - 5.f * A) * t3 + 8.f * A) * t3 - 4.f * A;
 #pragma unroll
-  for (int k = 0; k < 4; ++k) idx[k] = min(max((int)fl - 1 + k, 0), kGrid - 1);
+  for (int k = 0; k < 4; ++k) idx[k] = min(max((int)fl - 1 + k, 0), SRC - 1);
 }
 
+template <int SRC>
 __global__ void __launch_bounds__(kEwThreads) pos_interp_kernel(const float* __restrict__ pos, int gh, int gw,
                                                                 float* __restrict__ out) {
   const int total = (1 + gh * gw) * kVisDim;
@@ -469,14 +485,14 @@ __global__ void __launch_bounds__(kEwThreads) pos_interp_kernel(const float* __r
     const int y = (row - 1) / gw, x = (row - 1) - y * gw;
     int iy[4], ix[4];
     float wy[4], wx[4];
-    cubic_taps(gh, y, iy, wy);
-    cubic_taps(gw, x, ix, wx);
+    cubic_taps<SRC>(gh, y, iy, wy);
+    cubic_taps<SRC>(gw, x, ix, wx);
     float acc = 0.f;
 #pragma unroll
     for (int a = 0; a < 4; ++a) {
       float t = 0.f;
 #pragma unroll
-      for (int b = 0; b < 4; ++b) t += __ldg(pos + (size_t)(1 + iy[a] * kGrid + ix[b]) * kVisDim + c) * wx[b];
+      for (int b = 0; b < 4; ++b) t += __ldg(pos + (size_t)(1 + iy[a] * SRC + ix[b]) * kVisDim + c) * wx[b];
       acc += t * wy[a];
     }
     out[i] = acc;
@@ -530,9 +546,10 @@ inline int grid_for(int64_t work_items, int per_block) {
 }  // namespace
 
 int launch_im2col(const void* pixels, int fmt, int64_t n, int height, int width, __nv_bfloat16* out, int f16,
-                  cudaStream_t st) {
+                  cudaStream_t st, int patch) {
+  PLIP_REQUIRE(patch == kPatch || patch == kPatch16, "im2col: patch size %d (32 or 16)", patch);
   PLIP_REQUIRE(n > 0, "im2col: n must be positive");
-  PLIP_REQUIRE(height >= kPatch && width >= kPatch && height / kPatch <= kMaxGrid && width / kPatch <= kMaxGrid,
+  PLIP_REQUIRE(height >= patch && width >= patch && height / patch <= kMaxGrid && width / patch <= kMaxGrid,
                "im2col: image size %dx%d out of range", height, width);
   const bool fixed = height == kImage && width == kImage;
   const uintptr_t addr = reinterpret_cast<uintptr_t>(pixels);
@@ -544,30 +561,39 @@ int launch_im2col(const void* pixels, int fmt, int64_t n, int height, int width,
   // vector loads need every row start aligned: f32 16 B (W % 4 == 0), bf16 16 B (W % 8), u8 8 B (3 W % 8)
   const bool aligned = (addr & (fmt == PLIP_PIX_U8_NHWC ? 7 : 15)) == 0;
   const int vec = aligned && width % (fmt == PLIP_PIX_F32_NCHW ? 4 : 8) == 0 ? 1 : 0;
-  const ImGeom geo{height, width, height / kPatch, width / kPatch};
-  const int64_t items = (fmt == PLIP_PIX_U8_NHWC ? 1 : 3) * n * (geo.gh * 32) * (geo.gw * 4);
+  const ImGeom geo{height, width, height / patch, width / patch};
+  const int64_t items = (fmt == PLIP_PIX_U8_NHWC ? 1 : 3) * n * (geo.gh * patch) * (geo.gw * (patch / 8));
   const int grid = grid_for(items, kEwThreads);
-#define PLIP_IM2COL(F)                                                                                                 \
-  PLIP_CUDA_CHECK(fixed ? launch_kernel(im2col_kernel<F, true>, dim3(grid), dim3(kEwThreads), 0, st, 1, pixels, out, n, \
-                                        f16, geo, vec)                                                                 \
-                        : launch_kernel(im2col_kernel<F, false>, dim3(grid), dim3(kEwThreads), 0, st, 1, pixels, out,  \
-                                        n, f16, geo, vec))
-  switch (fmt) {
-    case PLIP_PIX_F32_NCHW: PLIP_IM2COL(PLIP_PIX_F32_NCHW); break;
-    case PLIP_PIX_BF16_NCHW: PLIP_IM2COL(PLIP_PIX_BF16_NCHW); break;
-    case PLIP_PIX_U8_NHWC: PLIP_IM2COL(PLIP_PIX_U8_NHWC); break;
-    default: set_last_error("im2col: unknown pixel format %d", fmt); return -2;
+#define PLIP_IM2COL(F, P)                                                                                              \
+  PLIP_CUDA_CHECK(fixed ? launch_kernel(im2col_kernel<F, true, P>, dim3(grid), dim3(kEwThreads), 0, st, 1, pixels, out, \
+                                        n, f16, geo, vec)                                                              \
+                        : launch_kernel(im2col_kernel<F, false, P>, dim3(grid), dim3(kEwThreads), 0, st, 1, pixels,    \
+                                        out, n, f16, geo, vec))
+#define PLIP_IM2COL_FMT(P)                                                                                             \
+  switch (fmt) {                                                                                                       \
+    case PLIP_PIX_F32_NCHW: PLIP_IM2COL(PLIP_PIX_F32_NCHW, P); break;                                                  \
+    case PLIP_PIX_BF16_NCHW: PLIP_IM2COL(PLIP_PIX_BF16_NCHW, P); break;                                                \
+    case PLIP_PIX_U8_NHWC: PLIP_IM2COL(PLIP_PIX_U8_NHWC, P); break;                                                    \
+    default: set_last_error("im2col: unknown pixel format %d", fmt); return -2;                                        \
   }
+  if (patch == kPatch) {
+    PLIP_IM2COL_FMT(kPatch)
+  } else {
+    PLIP_IM2COL_FMT(kPatch16)
+  }
+#undef PLIP_IM2COL_FMT
 #undef PLIP_IM2COL
   PLIP_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 
-int launch_window_im2col(const WindowSrc& win, int64_t n, __nv_bfloat16* out, int f16, cudaStream_t st) {
+int launch_window_im2col(const WindowSrc& win, int64_t n, __nv_bfloat16* out, int f16, cudaStream_t st, int patch) {
   PLIP_REQUIRE(n > 0 && win.region && win.origins && out, "window_im2col: bad argument");
+  PLIP_REQUIRE(patch == kPatch || patch == kPatch16, "window_im2col: patch size %d (32 or 16)", patch);
   PLIP_REQUIRE((reinterpret_cast<uintptr_t>(win.origins) & 7) == 0, "window_im2col: origins must be 8-byte aligned");
   const int grid = grid_for(n * kImage * (kImage / 8), kEwThreads);
-  PLIP_CUDA_CHECK(launch_kernel(window_im2col_kernel, dim3(grid), dim3(kEwThreads), 0, st, 1, win.region, win.pitch,
+  PLIP_CUDA_CHECK(launch_kernel(patch == kPatch ? window_im2col_kernel<kPatch> : window_im2col_kernel<kPatch16>,
+                                dim3(grid), dim3(kEwThreads), 0, st, 1, win.region, win.pitch,
                                 reinterpret_cast<const int2*>(win.origins), n, out, f16));
   PLIP_CUDA_CHECK(cudaGetLastError());
   return 0;
@@ -587,13 +613,16 @@ int launch_window_mask(const uint8_t* mask, int64_t pitch, int channels, const i
                                origins_host, n, threshold, counts, st);
 }
 
-int launch_pos_interp(const float* pos, int gh, int gw, float* out, cudaStream_t st) {
+int launch_pos_interp(const float* pos, int src_grid, int gh, int gw, float* out, cudaStream_t st) {
   PLIP_REQUIRE(pos && out, "pos_interp: null argument");
+  PLIP_REQUIRE(src_grid == vis_grid(kPatch) || src_grid == vis_grid(kPatch16),
+               "pos_interp: stored grid %d (7 or 14)", src_grid);
   PLIP_REQUIRE(gh >= 1 && gw >= 1 && gh <= kMaxGrid && gw <= kMaxGrid, "pos_interp: grid %dx%d out of [1,%d]", gh, gw,
                kMaxGrid);
   const int64_t items = (int64_t)(1 + gh * gw) * kVisDim;
-  PLIP_CUDA_CHECK(launch_kernel(pos_interp_kernel, dim3(grid_for(items, kEwThreads)), dim3(kEwThreads), 0, st, 1, pos,
-                                gh, gw, out));
+  PLIP_CUDA_CHECK(launch_kernel(src_grid == kGrid ? pos_interp_kernel<vis_grid(kPatch)>
+                                                  : pos_interp_kernel<vis_grid(kPatch16)>,
+                                dim3(grid_for(items, kEwThreads)), dim3(kEwThreads), 0, st, 1, pos, gh, gw, out));
   PLIP_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

@@ -62,11 +62,13 @@ void add_tower(std::vector<Spec>& v, const std::string& pfx, int D, int FF) {
   }
 }
 
-std::vector<Spec> build_specs() {
+// The blob layout of a vision patch size: ViT-B/32 (PLIP) and ViT-B/16 differ only in the patch embedding
+// [768, 3 * patch^2] and the stored position table [(224 / patch)^2 + 1, 768].
+std::vector<Spec> build_specs(int patch) {
   std::vector<Spec> v;
-  add(v, "vision_model.embeddings.patch_embedding.weight", 1, kVisDim, kPatchK);
+  add(v, "vision_model.embeddings.patch_embedding.weight", 1, kVisDim, patch_k(patch));
   add(v, "vision_model.embeddings.class_embedding", 0, kVisDim, 1);
-  add(v, "vision_model.embeddings.position_embedding.weight", 0, kVisSeq, kVisDim);
+  add(v, "vision_model.embeddings.position_embedding.weight", 0, vis_seq(patch), kVisDim);
   add(v, "vision_model.pre_layrnorm.weight", 0, kVisDim, 1);
   add(v, "vision_model.pre_layrnorm.bias", 0, kVisDim, 1);
   add_tower(v, "vision_model", kVisDim, kVisFF);
@@ -88,13 +90,17 @@ std::vector<Spec> build_specs() {
   return v;
 }
 
-const std::vector<Spec>& specs() {
-  static const std::vector<Spec> v = build_specs();  // C++11: initialised once, thread-safe
-  return v;
+bool valid_patch(int patch) { return patch == kPatch || patch == kPatch16; }
+
+// patch: 32 or 16 (valid_patch)
+const std::vector<Spec>& specs(int patch = kPatch) {
+  static const std::vector<Spec> v32 = build_specs(kPatch);  // C++11: initialised once, thread-safe
+  static const std::vector<Spec> v16 = build_specs(kPatch16);
+  return patch == kPatch16 ? v16 : v32;
 }
 
-uint64_t blob_bytes() {
-  const auto& v = specs();
+uint64_t blob_bytes(int patch = kPatch) {
+  const auto& v = specs(patch);
   const Spec& s = v.back();
   return (s.offset + s.numel * (s.dtype == 1 ? 2 : 4) + 255) & ~255ull;
 }
@@ -118,16 +124,17 @@ size_t pixel_bytes(int fmt, int height = kImage, int width = kImage) {
   return fmt == PLIP_PIX_F32_NCHW ? px * 4 : (fmt == PLIP_PIX_BF16_NCHW ? px * 2 : px);
 }
 
-// Input geometry of the vision tower: H x W pixels -> gh x gw patches (the H % 32 / W % 32 remainder is ignored, as by
-// the stride-32 conv), S = gh * gw + 1 tokens.  224 x 224 (7 x 7, S = 50) uses the stored position table; any other
-// grid an interpolated one (TF:modeling_clip.py:161-218, interpolate_pos_encoding).
+// Input geometry of the vision tower: H x W pixels -> gh x gw patches of the engine's patch size P (the H % P / W % P
+// remainder is ignored, as by the stride-P conv), S = gh * gw + 1 tokens.  The stored grid (224 / P per side: 7 x 7,
+// S = 50 for ViT-B/32; 14 x 14, S = 197 for ViT-B/16) uses the stored position table; any other grid an interpolated
+// one (TF:modeling_clip.py:161-218, interpolate_pos_encoding).
 struct VisGeom {
-  int H = kImage, W = kImage, gh = kGrid, gw = kGrid, S = kVisSeq;
+  int H, W, gh, gw, S;
 };
 
-VisGeom vis_geom(int height, int width) {
+VisGeom vis_geom(int patch, int height = kImage, int width = kImage) {
   VisGeom g;
-  g.H = height; g.W = width; g.gh = height / kPatch; g.gw = width / kPatch; g.S = g.gh * g.gw + 1;
+  g.H = height; g.W = width; g.gh = height / patch; g.gw = width / patch; g.S = g.gh * g.gw + 1;
   return g;
 }
 
@@ -188,6 +195,7 @@ struct plip_engine {
   int text_pool_argmax = 0;  // rows without an eos token: 0 = position 0 (HF, eos_token_id 49407), 1 = argmax of the ids (legacy / OpenAI)
   int prune_last = 0;  // plip_set_last_layer_pruning: embedding calls run the last layer's out_proj / MLP on the pooled rows only
   int f16 = 0;  // 16-bit operand format of the packed GEMM weights and of every activation operand: 0 bf16, 1 IEEE half
+  int patch = kPatch;  // vision patch size of the weights (plip_create_patch): 32 (ViT-B/32) or 16 (ViT-B/16)
   float logit_scale_exp = 1.f;
   uint8_t* d_blob = nullptr;
   // vision
@@ -266,7 +274,7 @@ const T* wptr(const plip_engine* e, const Spec& s) {
 }
 
 int bind_weights(plip_engine* e) {
-  const auto& v = specs();
+  const auto& v = specs(e->patch);
   size_t i = 0;
   auto nextf = [&]() { return wptr<float>(e, v[i++]); };
   auto nextb = [&]() { return wptr<__nv_bfloat16>(e, v[i++]); };
@@ -534,23 +542,25 @@ int vision_embed(plip_engine* e, const VisInput& in, int64_t mb, const VisGeom& 
   const int patches = geo.gh * geo.gw;
   // Position table of the grid.  An interpolated one goes to the QKV buffer, which nothing reads before the first
   // layer's QKV GEMM: [geo.S, 768] fp32 fits, since S <= kVisSeq * max_mb and QKV holds that many rows of 2 x 2304 B.
+  // The im2col matrix [mb * patches, 3 * P^2] fits H: at P = 16 it has 768 of the 3072 columns of the P = 32 one.
+  const int grid = vis_grid(e->patch), K = patch_k(e->patch);
   const float* pos = e->v_pos;
-  if (geo.gh != kGrid || geo.gw != kGrid) {
+  if (geo.gh != grid || geo.gw != grid) {
     float* table = reinterpret_cast<float*>(w.QKV);
-    ProfScope ps(e, st, PK_MISC, 0, (double)kVisSeq * kVisDim * 4 + (double)geo.S * kVisDim * 4);
-    if (int rc = launch_pos_interp(e->v_pos, geo.gh, geo.gw, table, st)) return rc;
+    ProfScope ps(e, st, PK_MISC, 0, (double)vis_seq(e->patch) * kVisDim * 4 + (double)geo.S * kVisDim * 4);
+    if (int rc = launch_pos_interp(e->v_pos, grid, geo.gh, geo.gw, table, st)) return rc;
     pos = table;
   }
   {
     // windows: fmt is PLIP_PIX_U8_NHWC and geo 224 x 224, so the bytes are those of the same windows as tiles
-    ProfScope ps(e, st, PK_IM2COL, 0, dmb * (double)pixel_bytes(in.fmt, geo.H, geo.W) + dmb * patches * kPatchK * 2);
-    const int rc = in.win.region ? launch_window_im2col(in.win, mb, w.H, e->f16, st)
-                                 : launch_im2col(in.pixels, in.fmt, mb, geo.H, geo.W, w.H, e->f16, st);
+    ProfScope ps(e, st, PK_IM2COL, 0, dmb * (double)pixel_bytes(in.fmt, geo.H, geo.W) + dmb * patches * K * 2);
+    const int rc = in.win.region ? launch_window_im2col(in.win, mb, w.H, e->f16, st, e->patch)
+                                 : launch_im2col(in.pixels, in.fmt, mb, geo.H, geo.W, w.H, e->f16, st, e->patch);
     if (rc) return rc;
   }
   GemmArgs g;
-  g.A = w.H; g.lda = kPatchK; g.W = e->v_patch_w; g.ldw = kPatchK;
-  g.M = (int)(mb * patches); g.N = kVisDim; g.K = kPatchK;
+  g.A = w.H; g.lda = K; g.W = e->v_patch_w; g.ldw = K;
+  g.M = (int)(mb * patches); g.N = kVisDim; g.K = K;
   g.out = w.X; g.ldo = kVisDim; g.pos = pos; g.patches = patches; g.seq = geo.S; g.epi = EPI_PATCH_F32;
   if (int rc = gemm(e, PK_PATCH, g, st)) return rc;
   {
@@ -688,7 +698,8 @@ int pair_pass(plip_engine* e, const void* pixels, int fmt, int64_t mb_img, const
   if (int rc = text_pass(e, e->ws_txt, ids, ids_dtype, mask, mb_txt, seq_len, seq_len, embeds_only(out_txt, normalize),
                          prune, s_txt)) return rc;
   if (s_txt != st) PLIP_CUDA_CHECK(cudaEventRecord(e->ev_join, s_txt));
-  if (int rc = vision_pass(e, tiles(pixels, fmt), mb_img, VisGeom(), embeds_only(out_img, normalize), prune, st))
+  if (int rc = vision_pass(e, tiles(pixels, fmt), mb_img, vis_geom(e->patch), embeds_only(out_img, normalize), prune,
+                          st))
     return rc;
   if (s_txt != st) PLIP_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_join, 0));
   return 0;
@@ -831,19 +842,21 @@ int capture_graph(plip_engine* e, F&& body, Graph* out) {
   return 0;
 }
 
-// Arguments of a call on n images (interpolate_pos_encoding: any size): 32 <= H, W and a patch grid of at most
-// kMaxGrid x kMaxGrid, and one image's tokens must fit the workspace's kVisSeq * max_micro_batch token rows.  Pointers
-// and shapes are checked before the handle, so a bad argument is reported as such whatever else is wrong.
+// Arguments of a call on n images (interpolate_pos_encoding: any size): P <= H, W and a patch grid of at most
+// kMaxGrid x kMaxGrid for the engine's patch size P (32 without an engine), and one image's tokens must fit the
+// workspace's kVisSeq * max_micro_batch token rows.  Pointers and shapes are checked before the handle, so a bad
+// argument is reported as such whatever else is wrong.
 int check_pixels(const char* fn, const plip_engine* e, const void* in, const void* out, int fmt, int64_t n,
                  int height, int width) {
   PLIP_REQUIRE(in && out, "%s: null argument", fn);
   PLIP_REQUIRE(n > 0, "%s: n must be positive (got %lld)", fn, (long long)n);
   PLIP_REQUIRE(fmt >= 0 && fmt <= 2, "%s: unknown pixel format %d", fn, fmt);
-  PLIP_REQUIRE(height >= kPatch && width >= kPatch && height / kPatch <= kMaxGrid && width / kPatch <= kMaxGrid,
-               "%s: image size %dx%d out of range (32 <= height, width and at most %d patches of 32 per side)", fn,
-               height, width, kMaxGrid);
+  const int P = e ? e->patch : kPatch;
+  PLIP_REQUIRE(height >= P && width >= P && height / P <= kMaxGrid && width / P <= kMaxGrid,
+               "%s: image size %dx%d out of range (%d <= height, width and at most %d patches of %d per side)", fn,
+               height, width, P, kMaxGrid, P);
   PLIP_REQUIRE(e != nullptr, "%s: null engine", fn);
-  const int S = (height / kPatch) * (width / kPatch) + 1;
+  const int S = (height / P) * (width / P) + 1;
   PLIP_REQUIRE(S <= (int64_t)kVisSeq * e->max_mb,
                "%s: a %dx%d image has %d tokens, more than the %lld token rows of the workspace "
                "(%d x max_micro_batch %d); create the engine with max_micro_batch >= %d",
@@ -964,7 +977,7 @@ int dbg_hidden_states(const char* fn, plip_engine* e, int tower, const void* in,
   PLIP_REQUIRE(num_layers >= 0 && num_layers <= kLayers, "%s: num_layers %d out of range", fn, num_layers);
   if (int rc = tower == 0 ? check_pixels(fn, e, in, hidden, fmt, n, height, width)
                           : check_ids(fn, e, in, hidden, fmt, n, kTxtSeq, kTxtSeq)) return rc;
-  const VisGeom geo = vis_geom(height, width);
+  const VisGeom geo = vis_geom(e->patch, height, width);
   const int S = tower == 0 ? geo.S : kTxtSeq, D = tower == 0 ? kVisDim : kTxtDim;
   const int64_t per_pass = tower == 0 ? images_per_pass(e->max_mb, S) : e->max_mb;
   PLIP_REQUIRE(n <= per_pass, "%s: n=%lld sequences of %d tokens exceed one pass (%lld)", fn, (long long)n, S,
@@ -991,7 +1004,12 @@ PLIP_API uint64_t plip_launch_count(void) { return plip::g_launch_count.load(std
 PLIP_API int plip_weights_num_tensors(void) { return (int)specs().size(); }
 
 PLIP_API int plip_weights_tensor_info(int index, plip_tensor_info_t* info) {
-  const auto& v = specs();
+  return plip_weights_tensor_info_patch(kPatch, index, info);
+}
+
+PLIP_API int plip_weights_tensor_info_patch(int patch, int index, plip_tensor_info_t* info) {
+  PLIP_REQUIRE(valid_patch(patch), "tensor_info: vision patch size %d (32 or 16)", patch);
+  const auto& v = specs(patch);
   PLIP_REQUIRE(info != nullptr && index >= 0 && index < (int)v.size(), "tensor_info: index %d out of range", index);
   memset(info, 0, sizeof(*info));
   strncpy(info->name, v[index].name.c_str(), sizeof(info->name) - 1);
@@ -1004,7 +1022,8 @@ PLIP_API int plip_weights_tensor_info(int index, plip_tensor_info_t* info) {
   return 0;
 }
 
-PLIP_API uint64_t plip_weights_blob_bytes(void) { return blob_bytes(); }
+PLIP_API uint64_t plip_weights_blob_bytes(void) { return blob_bytes(kPatch); }
+PLIP_API uint64_t plip_weights_blob_bytes_patch(int patch) { return valid_patch(patch) ? blob_bytes(patch) : 0; }
 
 PLIP_API uint64_t plip_workspace_bytes(int max_micro_batch) {
   return max_micro_batch > 0 ? ws_layout(max_micro_batch).total : 0;
@@ -1017,13 +1036,24 @@ PLIP_API int plip_create(const void* host_blob, uint64_t nbytes, float logit_sca
 
 PLIP_API int plip_create_ex(const void* host_blob, uint64_t nbytes, float logit_scale_exp, int device,
                             int max_micro_batch, int operand_format, plip_engine_t** out) {
+  return plip_create_patch(host_blob, nbytes, logit_scale_exp, device, max_micro_batch, operand_format, kPatch, out);
+}
+
+PLIP_API int plip_create_patch(const void* host_blob, uint64_t nbytes, float logit_scale_exp, int device,
+                               int max_micro_batch, int operand_format, int vision_patch, plip_engine_t** out) {
   PLIP_REQUIRE(out != nullptr && host_blob != nullptr, "plip_create: null argument");
   PLIP_REQUIRE(operand_format == PLIP_OPERAND_BF16 || operand_format == PLIP_OPERAND_FP16,
                "plip_create: unknown operand format %d", operand_format);
-  PLIP_REQUIRE(nbytes == blob_bytes(), "plip_create: blob is %llu bytes, expected %llu",
-               (unsigned long long)nbytes, (unsigned long long)blob_bytes());
+  PLIP_REQUIRE(valid_patch(vision_patch), "plip_create: vision patch size %d (32: ViT-B/32, 16: ViT-B/16)",
+               vision_patch);
+  PLIP_REQUIRE(nbytes == blob_bytes(vision_patch), "plip_create: blob is %llu bytes, expected %llu",
+               (unsigned long long)nbytes, (unsigned long long)blob_bytes(vision_patch));
   PLIP_REQUIRE(max_micro_batch >= 1 && max_micro_batch <= 8192, "plip_create: max_micro_batch %d out of [1,8192]",
                max_micro_batch);
+  // the workspace holds kVisSeq * max_micro_batch vision token rows: one 224 x 224 image must fit
+  PLIP_REQUIRE(vis_seq(vision_patch) <= kVisSeq * max_micro_batch,
+               "plip_create: a 224x224 image has %d tokens at patch size %d; max_micro_batch must be >= %d",
+               vis_seq(vision_patch), vision_patch, (vis_seq(vision_patch) + kVisSeq - 1) / kVisSeq);
   int ndev = 0;
   PLIP_CUDA_CHECK(cudaGetDeviceCount(&ndev));
   PLIP_REQUIRE(device >= 0 && device < ndev, "plip_create: device %d not present (%d devices)", device, ndev);
@@ -1036,6 +1066,7 @@ PLIP_API int plip_create_ex(const void* host_blob, uint64_t nbytes, float logit_
   e->device = device;
   e->max_mb = max_micro_batch;
   e->f16 = operand_format == PLIP_OPERAND_FP16 ? 1 : 0;
+  e->patch = vision_patch;
   if (const char* gm = getenv("PLIP_GRAPH_MAX")) e->graph_max_n = atoi(gm) < 0 ? 0 : (atoi(gm) > 1024 ? 1024 : atoi(gm));
   e->logit_scale_exp = logit_scale_exp;
   const WsLayout w = ws_layout(max_micro_batch);
@@ -1139,6 +1170,7 @@ PLIP_API int plip_profile_read(plip_engine_t* e, plip_kernel_time_t* out, int ca
 PLIP_API float plip_logit_scale_exp(const plip_engine_t* e) { return e ? e->logit_scale_exp : 0.f; }
 PLIP_API int plip_max_micro_batch(const plip_engine_t* e) { return e ? e->max_mb : 0; }
 PLIP_API int plip_operand_format(const plip_engine_t* e) { return e ? e->f16 : -1; }
+PLIP_API int plip_vision_patch(const plip_engine_t* e) { return e ? e->patch : 0; }
 PLIP_API int plip_set_text_pooling(plip_engine_t* e, int no_eos_argmax) {
   PLIP_REQUIRE(e != nullptr, "plip_set_text_pooling: null engine");
   e->text_pool_argmax = no_eos_argmax != 0;
@@ -1160,11 +1192,12 @@ PLIP_API int plip_encode_images(plip_engine_t* e, const void* pixels_dev, int pi
 PLIP_API int plip_encode_images_hw(plip_engine_t* e, const void* pixels_dev, int pixel_format, int64_t n, int height,
                                    int width, float* out_dev, int normalize, void* stream) {
   if (int rc = check_pixels("plip_encode_images_hw", e, pixels_dev, out_dev, pixel_format, n, height, width)) return rc;
-  const VisGeom geo = vis_geom(height, width);
+  const VisGeom geo = vis_geom(e->patch, height, width);
   const size_t pb = pixel_bytes(pixel_format, height, width);
   const bool prune = e->prune_last != 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (height == kImage && width == kImage && graph_eligible(e, n)) {
+  // graph replay: ViT-B/32 224 x 224 calls (a ViT-B/16 engine's 197-token passes run eagerly, as other sizes do)
+  if (height == kImage && width == kImage && e->patch == kPatch && graph_eligible(e, n)) {
     const GraphKey key{0, (int)n, pixel_format, normalize ? 1 : 0, 0, 0, 0, 0, e->prune_last};
     return graph_call(e, key, {{{pixels_dev, (size_t)n * pb}, {nullptr, 0}}}, out_dev, st,
                       [&](cudaStream_t s, const void* pixels, const void*, float* out) {
@@ -1193,9 +1226,10 @@ PLIP_API int plip_encode_windows(plip_engine_t* e, const void* region_dev, int h
   const bool prune = e->prune_last != 0;
   const uint8_t* region = static_cast<const uint8_t*>(region_dev);
   // the micro-batches of plip_encode_images on tiles (no graph replay: its staging buffers hold tiles)
-  return micro_batches(e, n, images_per_pass(e->max_mb, kVisSeq), st, [&](int64_t i, int64_t mb) {
+  const VisGeom geo = vis_geom(e->patch);
+  return micro_batches(e, n, images_per_pass(e->max_mb, geo.S), st, [&](int64_t i, int64_t mb) {
     const VisInput in{nullptr, PLIP_PIX_U8_NHWC, WindowSrc{region, row_pitch_bytes, e->d_win + 2 * i}};
-    return vision_pass(e, in, mb, VisGeom(), embeds_only(out_dev + i * kProj, normalize), prune, st);
+    return vision_pass(e, in, mb, geo, embeds_only(out_dev + i * kProj, normalize), prune, st);
   });
 }
 
@@ -1254,8 +1288,10 @@ PLIP_API int plip_encode_pair(plip_engine_t* e, const void* pixels_dev, int pixe
     return rc;
   if (int rc = check_ids("plip_encode_pair", e, ids_dev, txt_out_dev, ids_dtype, n_txt, seq_len, seq_len)) return rc;
   // One micro-batch of each tower, neither of them small enough for the graph-replayed path: the two calls otherwise
-  // (the text tower first, as the sharded forward orders them).
-  if (n_img > e->max_mb || n_txt > e->max_mb || graph_eligible(e, n_img) || graph_eligible(e, n_txt)) {
+  // (the text tower first, as the sharded forward orders them).  A micro-batch of images holds fewer than max_mb
+  // ViT-B/16 images (197 tokens each).
+  if (n_img > images_per_pass(e->max_mb, vis_seq(e->patch)) || n_txt > e->max_mb || graph_eligible(e, n_img) ||
+      graph_eligible(e, n_txt)) {
     if (int rc = plip_encode_text(e, ids_dev, ids_dtype, attention_mask_dev, n_txt, seq_len, txt_out_dev, normalize,
                                   stream)) return rc;
     return plip_encode_images(e, pixels_dev, pixel_format, n_img, img_out_dev, normalize, stream);
@@ -1288,7 +1324,7 @@ PLIP_API int plip_vision_outputs(plip_engine_t* e, const void* pixels_dev, int p
                                  int width, const plip_tower_outputs_t* outputs, void* stream) {
   if (int rc = check_outputs("plip_vision_outputs", outputs)) return rc;
   if (int rc = check_pixels("plip_vision_outputs", e, pixels_dev, outputs, pixel_format, n, height, width)) return rc;
-  const VisGeom geo = vis_geom(height, width);
+  const VisGeom geo = vis_geom(e->patch, height, width);
   const size_t pb = pixel_bytes(pixel_format, height, width);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   return micro_batches(e, n, images_per_pass(e->max_mb, geo.S), st, [&](int64_t i, int64_t mb) {
@@ -1462,7 +1498,8 @@ PLIP_API int plip_encode_images_host(plip_engine_t* e, const void* pixels_host, 
   if (int rc = ensure_host_path(e)) return rc;
   PLIP_CUDA_CHECK(cudaStreamWaitEvent(e->s_compute, e->ev_last, 0));  // earlier device-API work owns the workspace
   const size_t pb = pixel_bytes(pixel_format);
-  const int64_t chunk = e->max_mb;
+  const VisGeom geo = vis_geom(e->patch);
+  const int64_t chunk = images_per_pass(e->max_mb, geo.S);
   const size_t in_bytes = (size_t)(n < chunk ? n : chunk) * pb;
   if (e->d_in_bytes < in_bytes) {
     size_t have0 = e->d_in_bytes, have1 = e->d_in_bytes;
@@ -1494,7 +1531,7 @@ PLIP_API int plip_encode_images_host(plip_engine_t* e, const void* pixels_host, 
     PLIP_CUDA_CHECK(cudaMemcpyAsync(e->d_in[b], src, (size_t)mb * pb, cudaMemcpyHostToDevice, e->s_copy));
     PLIP_CUDA_CHECK(cudaEventRecord(e->ev_copied[b], e->s_copy));
     PLIP_CUDA_CHECK(cudaStreamWaitEvent(e->s_compute, e->ev_copied[b], 0));
-    if (int rc = vision_pass(e, tiles(e->d_in[b], pixel_format), mb, VisGeom(),
+    if (int rc = vision_pass(e, tiles(e->d_in[b], pixel_format), mb, geo,
                              embeds_only(e->d_out + i * kProj, normalize), e->prune_last != 0, e->s_compute)) return rc;
     PLIP_CUDA_CHECK(cudaEventRecord(e->ev_done[b], e->s_compute));
   }
@@ -1638,13 +1675,25 @@ PLIP_API int plip_dbg_attention_probs(const void* qkv_bf16, int64_t n_seq, int s
 
 PLIP_API int plip_dbg_im2col(const void* pixels, int pixel_format, int64_t n, void* out_bf16, void* stream) {
   return launch_im2col(pixels, pixel_format, n, kImage, kImage, static_cast<__nv_bfloat16*>(out_bf16), g_dbg_f16,
-                       static_cast<cudaStream_t>(stream));
+                       static_cast<cudaStream_t>(stream), kPatch);
 }
 
 PLIP_API int plip_dbg_im2col_hw(const void* pixels, int pixel_format, int64_t n, int height, int width, void* out16,
                                 void* stream) {
   return launch_im2col(pixels, pixel_format, n, height, width, static_cast<__nv_bfloat16*>(out16), g_dbg_f16,
-                       static_cast<cudaStream_t>(stream));
+                       static_cast<cudaStream_t>(stream), kPatch);
+}
+
+PLIP_API int plip_dbg_im2col_patch(const void* pixels, int pixel_format, int64_t n, int height, int width, int patch,
+                                   void* out16, void* stream) {
+  return launch_im2col(pixels, pixel_format, n, height, width, static_cast<__nv_bfloat16*>(out16), g_dbg_f16,
+                       static_cast<cudaStream_t>(stream), patch);
+}
+
+PLIP_API int plip_dbg_window_im2col_patch(const void* region_dev, int64_t row_pitch_bytes, const int32_t* origins_dev,
+                                          int64_t n, int patch, void* out16, void* stream) {
+  return launch_window_im2col(WindowSrc{static_cast<const uint8_t*>(region_dev), row_pitch_bytes, origins_dev}, n,
+                              static_cast<__nv_bfloat16*>(out16), g_dbg_f16, static_cast<cudaStream_t>(stream), patch);
 }
 
 PLIP_API int plip_dbg_text_embed(const void* ids, int ids_dtype, int64_t n, int seq_len, int ids_stride,
@@ -1670,7 +1719,13 @@ PLIP_API int plip_dbg_gather_rows(const void* a16, const float* x32, const int32
 }
 
 PLIP_API int plip_dbg_pos_interp(const float* pos_dev, int grid_h, int grid_w, float* out_dev, void* stream) {
-  return launch_pos_interp(pos_dev, grid_h, grid_w, out_dev, static_cast<cudaStream_t>(stream));
+  return launch_pos_interp(pos_dev, kGrid, grid_h, grid_w, out_dev, static_cast<cudaStream_t>(stream));
+}
+
+PLIP_API int plip_dbg_pos_interp_patch(const float* pos_dev, int patch, int grid_h, int grid_w, float* out_dev,
+                                       void* stream) {
+  PLIP_REQUIRE(valid_patch(patch), "pos_interp: vision patch size %d (32 or 16)", patch);
+  return launch_pos_interp(pos_dev, vis_grid(patch), grid_h, grid_w, out_dev, static_cast<cudaStream_t>(stream));
 }
 
 PLIP_API int plip_dbg_hidden_states(plip_engine_t* e, int tower, const void* input_dev, int input_format,

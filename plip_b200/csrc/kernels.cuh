@@ -9,9 +9,9 @@ namespace plip {
 
 // elementwise.cu  (f16 = 1: 16-bit outputs are IEEE half instead of bfloat16; the pointer type stays a 16-bit tag)
 // pixels: n images of height x width (224 x 224 unless the position table is interpolated) -> the patch matrix
-// [n * gh * gw, 3072], gh = height / 32, gw = width / 32.
+// [n * gh * gw, 3 * patch^2], gh = height / patch, gw = width / patch; patch 32 (ViT-B/32) or 16 (ViT-B/16).
 int launch_im2col(const void* pixels, int fmt, int64_t n, int height, int width, __nv_bfloat16* out, int f16,
-                  cudaStream_t st);
+                  cudaStream_t st, int patch);
 // 224 x 224 windows of one uint8 RGB region [H, W, 3] with a row pitch in bytes.  origins: int32 (row, col) pairs, one
 // per window, each window inside the region (the callers check that on the host).
 struct WindowSrc {
@@ -19,8 +19,10 @@ struct WindowSrc {
   int64_t pitch;
   const int32_t* origins;  // device memory, 8-byte aligned
 };
-// n windows -> the patch matrix [n * 49, 3072], bit-identical to launch_im2col of the same windows as u8 tiles.
-int launch_window_im2col(const WindowSrc& win, int64_t n, __nv_bfloat16* out, int f16, cudaStream_t st);
+// n windows -> the patch matrix [n * (224 / patch)^2, 3 * patch^2], bit-identical to launch_im2col of the same windows
+// as u8 tiles.
+int launch_window_im2col(const WindowSrc& win, int64_t n, __nv_bfloat16* out, int f16, cudaStream_t st,
+                         int patch);
 // Per window, the pixels whose three channels are all >= threshold -> counts int32 [n].  origins_host: host memory,
 // consumed before the call returns.
 int launch_window_background(const uint8_t* region, int64_t pitch, const int32_t* origins_host, int64_t n,
@@ -28,8 +30,9 @@ int launch_window_background(const uint8_t* region, int64_t pitch, const int32_t
 // Per window of a uint8 mask [H, W, channels] (channels 1 or 3), the elements > threshold -> counts int32 [n].
 int launch_window_mask(const uint8_t* mask, int64_t pitch, int channels, const int32_t* origins_host, int64_t n,
                        int threshold, int32_t* counts, cudaStream_t st);
-// The vision position table resized to a gh x gw patch grid: fp32 [1 + gh * gw, 768] (bicubic, as HF).
-int launch_pos_interp(const float* pos, int gh, int gw, float* out, cudaStream_t st);
+// The vision position table of a src_grid x src_grid patch grid (7: ViT-B/32, 14: ViT-B/16) resized to a gh x gw
+// one: fp32 [1 + gh * gw, 768] (bicubic, as HF).
+int launch_pos_interp(const float* pos, int src_grid, int gh, int gw, float* out, cudaStream_t st);
 int launch_layernorm(const float* x, const int32_t* row_index, int64_t in_row_stride, int64_t rows, int dim,
                      const float* gamma, const float* beta, float* out_f32, __nv_bfloat16* out_bf16, int f16,
                      cudaStream_t st);

@@ -196,10 +196,27 @@ def mudipath_checkpoint() -> str:
         f"$TORCH_MODEL_ZOO (default $TORCH_HOME/models, ~/.torch/models).  Looked at: {path}")
 
 
+# PC_CLIP_ARCH values the engine runs (clip.load names) -> the file name of clip's download cache.  ViT-L/14 and the
+# ResNet CLIPs have other widths / no transformer image tower and are not implemented.
+CLIP_ARCHS = {"ViT-B/32": "ViT-B-32.pt", "ViT-B/16": "ViT-B-16.pt"}
+
+
+def _check_arch(arch: str, sd, what: str) -> None:
+    """The reference loads the weights into ``clip.load(arch)``'s model, strictly, so weights of another patch size
+    than ``arch``'s fail there: raise ``ValueError`` for them here as well."""
+    from .weights import vision_patch
+    want = int(arch.rsplit("/", 1)[1])
+    got = vision_patch(sd)
+    if got != want:
+        raise ValueError(f"PC_CLIP_ARCH={arch!r} needs {want}-pixel patches; the weights of {what} have {got}-pixel ones")
+
+
 class EmbedderFactory:
     """``reproducibility/embedders/factory.py:15-47``: ``args.model_name`` selects the flavour.  For ``plip`` / ``clip``
     ``args.backbone`` is the path of an OpenAI-clip (or HF) state dict saved with ``torch.save``; for ``mudipath`` it
-    is only a name kept on the embedder, as in the reference, and the weights come from :func:`mudipath_checkpoint`."""
+    is only a name kept on the embedder, as in the reference, and the weights come from :func:`mudipath_checkpoint`.
+    ``$PC_CLIP_ARCH`` (default ``ViT-B/32``) may be ``ViT-B/32`` or ``ViT-B/16``; the engine takes the patch size from
+    the weights it loads."""
 
     def factory(self, args):
         name, path = args.model_name, args.backbone
@@ -211,17 +228,20 @@ class EmbedderFactory:
             sd = torch.load(mudipath_checkpoint(), map_location="cpu", weights_only=True)
             return DenseNetEmbedder(DenseNetEngine(sd), None, name, path)
         arch = os.environ.get("PC_CLIP_ARCH", "ViT-B/32")
-        if arch != "ViT-B/32":
-            raise ValueError(f"plip_b200 implements ViT-B/32 only (PC_CLIP_ARCH={arch!r})")
+        if arch not in CLIP_ARCHS:
+            raise ValueError(f"plip_b200 implements {' and '.join(CLIP_ARCHS)} only (PC_CLIP_ARCH={arch!r})")
         if name == "plip":      # clip.load(arch) + load_state_dict(torch.load(path))     (factory.py:20-27)
             sd = torch.load(path, map_location="cpu")
             if isinstance(sd, dict) and "state_dict" in sd:
                 sd = sd["state_dict"]
+            _check_arch(arch, sd, path)
             model = PlipCLIPModel.from_openai_state_dict(sd) if "visual.conv1.weight" in sd else PlipCLIPModel(sd)
             model.eval()
             return CLIPEmbedder(model, None, name, path)
         if name == "clip":      # the PRETRAINED OpenAI weights; `path` is only a cache key there (factory.py:29-32)
-            model = PlipCLIPModel.from_openai_state_dict(self._openai_pretrained_state_dict(arch))
+            sd = self._openai_pretrained_state_dict(arch)
+            _check_arch(arch, sd, "OpenAI's pretrained checkpoint")
+            model = PlipCLIPModel.from_openai_state_dict(sd)
             model.eval()
             return CLIPEmbedder(model, None, name, path)
         raise ValueError(f"unsupported embedder {name!r} (plip / clip / mudipath)")
@@ -229,15 +249,16 @@ class EmbedderFactory:
     @staticmethod
     def _openai_pretrained_state_dict(arch: str):
         """``clip.load(arch)``'s weights without running its model: through the ``clip`` package when it is
-        installed, else from its download cache (``~/.cache/clip/ViT-B-32.pt``, a TorchScript archive) or
-        ``$PLIP_B200_OPENAI_CLIP``.  Never falls back to ``args.backbone``: that is the PLIP checkpoint."""
+        installed, else from ``$PLIP_B200_OPENAI_CLIP`` or its download cache (``~/.cache/clip/ViT-B-32.pt`` /
+        ``ViT-B-16.pt``, a TorchScript archive).  Never falls back to ``args.backbone``: that is the PLIP checkpoint."""
         try:
             import clip                                   # noqa: PLC0415 - optional, as in the reference
             model, _ = clip.load(arch, device="cpu")
             return model.state_dict()
         except ImportError:
             pass
-        cands = [os.environ.get("PLIP_B200_OPENAI_CLIP"), os.path.expanduser("~/.cache/clip/ViT-B-32.pt")]
+        fname = CLIP_ARCHS[arch]
+        cands = [os.environ.get("PLIP_B200_OPENAI_CLIP"), os.path.expanduser(f"~/.cache/clip/{fname}")]
         for c in cands:
             if c and os.path.isfile(c):
                 try:
@@ -246,6 +267,6 @@ class EmbedderFactory:
                     sd = torch.load(c, map_location="cpu")
                     return sd["state_dict"] if isinstance(sd, dict) and "state_dict" in sd else sd
         raise FileNotFoundError(
-            "embedder 'clip' needs OpenAI's pretrained ViT-B/32 weights: install the `clip` package, or put "
-            "ViT-B-32.pt into ~/.cache/clip/ (or point $PLIP_B200_OPENAI_CLIP at it).  args.backbone is NOT used for "
+            f"embedder 'clip' needs OpenAI's pretrained {arch} weights: install the `clip` package, or put "
+            f"{fname} into ~/.cache/clip/ (or point $PLIP_B200_OPENAI_CLIP at it).  args.backbone is NOT used for "
             "this branch (reproducibility/embedders/factory.py:29-32 never loads it).")

@@ -10,7 +10,7 @@ import torch
 
 from ._lib import SgdProblem as _SgdProblem
 from ._lib import check, lib
-from .weights import operand_format, pack_state_dict
+from .weights import operand_format, pack_state_dict, vision_patch
 
 PIX_F32_NCHW, PIX_BF16_NCHW, PIX_U8_NHWC = 0, 1, 2
 IDS_I32, IDS_I64 = 0, 1
@@ -26,31 +26,34 @@ VISION_DIM, VISION_HEADS = 768, 12
 TEXT_DIM, TEXT_HEADS = 512, 8
 NUM_LAYERS = 12
 
+# Module-level defaults are CLIP ViT-B/32's (PLIP); an Engine on ViT-B/16 weights passes its own patch size (16).
 PATCH = 32
-MAX_GRID = 32  # interpolate_pos_encoding: at most 32 x 32 patches (1024 px per side, 1025 tokens)
+MAX_GRID = 32  # interpolate_pos_encoding: at most 32 x 32 patches (1024 px per side at patch 32, 512 at 16; 1025 tokens)
 
 
-def _check_size(h: int, w: int, interpolate_pos_encoding: bool) -> None:
+def _check_size(h: int, w: int, interpolate_pos_encoding: bool, patch: int = PATCH) -> None:
     if not interpolate_pos_encoding:
         if h != IMAGE_SIZE or w != IMAGE_SIZE:
             raise ValueError(f"Input image size ({h}*{w}) doesn't match model (224*224).")  # TF:204-207
-    elif not (h >= PATCH and w >= PATCH and h // PATCH <= MAX_GRID and w // PATCH <= MAX_GRID):
+    elif not (h >= patch and w >= patch and h // patch <= MAX_GRID and w // patch <= MAX_GRID):
         raise ValueError(f"Input image size ({h}*{w}) out of range for interpolate_pos_encoding: height and width "
-                         f"must be >= {PATCH} with at most {MAX_GRID} patches of {PATCH} per side (<= 1055 px)")
+                         f"must be >= {patch} with at most {MAX_GRID} patches of {patch} per side "
+                         f"(<= {(MAX_GRID + 1) * patch - 1} px)")
 
 
-def _pixel_format(t: Union[torch.Tensor, np.ndarray], interpolate_pos_encoding: bool = False) -> int:
+def _pixel_format(t: Union[torch.Tensor, np.ndarray], interpolate_pos_encoding: bool = False, patch: int = PATCH) -> int:
     """Validate an image batch and return its C-ABI pixel format (error text mirrors TF:204-207).  With
-    ``interpolate_pos_encoding`` any height / width with ``32 <= H, W`` and ``H // 32, W // 32 <= 32`` is accepted."""
+    ``interpolate_pos_encoding`` any height / width with ``P <= H, W`` and ``H // P, W // P <= 32`` is accepted
+    (``P``: the vision patch size, 32 or 16)."""
     shape, dtype = tuple(t.shape), t.dtype
     if dtype in (torch.uint8, np.dtype("uint8")):
         if len(shape) != 4 or shape[3] != 3:
             raise ValueError(f"uint8 images must be [n,224,224,3] (NHWC), got {shape}")
-        _check_size(shape[1], shape[2], interpolate_pos_encoding)
+        _check_size(shape[1], shape[2], interpolate_pos_encoding, patch)
         return PIX_U8_NHWC
     if len(shape) != 4 or shape[1] != 3:
         raise ValueError(f"pixel_values must be [n,3,224,224], got {shape}")
-    _check_size(shape[2], shape[3], interpolate_pos_encoding)
+    _check_size(shape[2], shape[3], interpolate_pos_encoding, patch)
     if dtype in (torch.float32, np.dtype("float32")):
         return PIX_F32_NCHW
     if dtype == torch.bfloat16:
@@ -63,9 +66,10 @@ def _pixel_hw(t: Union[torch.Tensor, np.ndarray], fmt: int) -> Tuple[int, int]:
     return (int(t.shape[1]), int(t.shape[2])) if fmt == PIX_U8_NHWC else (int(t.shape[2]), int(t.shape[3]))
 
 
-def vision_seq_len(height: int, width: int) -> int:
-    """Tokens of one image: ``(H // 32) * (W // 32)`` patches + the class token (50 at 224 x 224)."""
-    return (height // PATCH) * (width // PATCH) + 1
+def vision_seq_len(height: int, width: int, patch: int = PATCH) -> int:
+    """Tokens of one image: ``(H // P) * (W // P)`` patches of ``P`` pixels + the class token (50 at 224 x 224 for
+    ``P = 32``, 197 for ``P = 16``)."""
+    return (height // patch) * (width // patch) + 1
 
 
 def _ids_dtype(dtype) -> int:
@@ -551,15 +555,17 @@ class Engine:
         self.device = torch.device("cuda", dev.index if dev.index is not None else torch.cuda.current_device())
         fmt, _ = operand_format(operand_dtype)
         self.operand_dtype = "fp16" if fmt == 1 else "bf16"
+        patch = vision_patch(state_dict)                   # 32: ViT-B/32 (PLIP), 16: ViT-B/16
         blob, scale = pack_state_dict(state_dict, self.operand_dtype)
         self.logit_scale_exp = float(scale)
         h = C.c_void_p()
         with torch.cuda.device(self.device):
             torch.cuda.init()
-            check(self._L.plip_create_ex(blob.data_ptr(), blob.numel(), C.c_float(scale), self.device.index,
-                                         int(max_micro_batch), fmt, C.byref(h)), "plip_create_ex")
+            check(self._L.plip_create_patch(blob.data_ptr(), blob.numel(), C.c_float(scale), self.device.index,
+                                            int(max_micro_batch), fmt, patch, C.byref(h)), "plip_create_patch")
         self._h = h
         self.max_micro_batch = int(max_micro_batch)
+        self.vision_patch = int(self._L.plip_vision_patch(h))
 
     def set_text_pooling(self, no_eos_argmax: bool) -> None:
         """Captions without an eos token: pool position 0 (HF, ``eos_token_id == 49407``; default) or the first argmax
@@ -570,6 +576,13 @@ class Engine:
         """Embedding calls run the last encoder layer's out_proj / LayerNorm 2 / MLP on the pooled rows only (CLS, first
         eos) — same embeddings, less work; hidden-state requests are never pruned.  See ``plip_set_last_layer_pruning``."""
         check(self._L.plip_set_last_layer_pruning(self._h, int(bool(on))), "plip_set_last_layer_pruning")
+
+    def vision_seq_len(self, height: int = IMAGE_SIZE, width: int = IMAGE_SIZE) -> int:
+        """Tokens of one ``height x width`` image at this engine's patch size (50 or 197 at 224 x 224)."""
+        return vision_seq_len(height, width, self.vision_patch)
+
+    def _pixel_format(self, t, interpolate_pos_encoding: bool = False) -> int:
+        return _pixel_format(t, interpolate_pos_encoding, self.vision_patch)
 
     @property
     def last_layer_pruning(self) -> bool:
@@ -614,11 +627,11 @@ class Engine:
                       interpolate_pos_encoding: bool = False) -> torch.Tensor:
         """``get_image_features``: ``[n,3,224,224]`` f32/bf16 or ``[n,224,224,3]`` u8 -> ``[n,512]`` f32 (device).
 
-        ``interpolate_pos_encoding=True``: any ``[n,3,H,W]`` / ``[n,H,W,3]`` with ``32 <= H, W`` and at most 32 patches
-        of 32 pixels per side; the position table is resized bicubically to the patch grid, as HF does
-        (``plip_encode_images_hw``).  An image's ``(H // 32) * (W // 32) + 1`` tokens must fit the workspace's
+        ``interpolate_pos_encoding=True``: any ``[n,3,H,W]`` / ``[n,H,W,3]`` with ``P <= H, W`` and at most 32 patches
+        of ``P = vision_patch`` pixels per side; the position table is resized bicubically to the patch grid, as HF
+        does (``plip_encode_images_hw``).  An image's ``(H // P) * (W // P) + 1`` tokens must fit the workspace's
         ``50 * max_micro_batch`` token rows."""
-        fmt = _pixel_format(pixels, interpolate_pos_encoding)
+        fmt = self._pixel_format(pixels, interpolate_pos_encoding)
         n = int(pixels.shape[0])
         if n == 0:
             return torch.empty(0, EMBED_DIM, device=self.device)
@@ -685,7 +698,7 @@ class Engine:
         (``plip_encode_pair``): when each side fits one micro-batch, the text tower runs on the engine's own stream at
         the same time as the vision tower, each filling the SMs the other leaves idle.  Needs a second, text-only
         workspace (about 0.9 GB at ``max_micro_batch`` 1024), allocated on the first such call."""
-        fmt = _pixel_format(pixels)
+        fmt = self._pixel_format(pixels)
         n_img = int(pixels.shape[0])
         n_txt, s = _check_ids(input_ids, attention_mask)
         if n_img == 0 or n_txt == 0:
@@ -781,11 +794,11 @@ class Engine:
           ``[0]`` after ``pre_layrnorm``, ``[l]`` after layer ``l``; ``last_hidden_state`` is then ``hidden_states[12]``;
         - ``attentions``: 12 views ``[n,12,S,S]`` of one ``[12,n,12,S,S]`` tensor (``output_attentions``).
 
-        ``S = vision_seq_len(H, W)`` (50 at 224 x 224).  The attentions take ``12 * 12 * S^2 * 4`` bytes per image
-        (1.4 MB at 224 x 224, 605 MB at 1024 x 1024)."""
-        fmt = _pixel_format(pixels, interpolate_pos_encoding)
+        ``S = self.vision_seq_len(H, W)`` (50 at 224 x 224, 197 on ViT-B/16).  The attentions take
+        ``12 * 12 * S^2 * 4`` bytes per image (1.4 MB at 224 x 224, 605 MB at 1025 tokens)."""
+        fmt = self._pixel_format(pixels, interpolate_pos_encoding)
         h, w = _pixel_hw(pixels, fmt)
-        n, S = int(pixels.shape[0]), vision_seq_len(h, w)
+        n, S = int(pixels.shape[0]), self.vision_seq_len(h, w)
         st, out = self._outputs(n, S, VISION_DIM, VISION_HEADS, output_hidden_states, output_attentions, True)
         st.normalize = int(bool(normalize))
         if n:
@@ -821,7 +834,7 @@ class Engine:
     def encode_images_host(self, pixels: Union[np.ndarray, torch.Tensor], normalize: bool = False,
                            out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Host array in, host ``[n,512]`` f32 tensor out; H2D/D2H pipelined inside the C call."""
-        fmt = _pixel_format(pixels)
+        fmt = self._pixel_format(pixels)
         t = torch.from_numpy(np.ascontiguousarray(pixels)) if isinstance(pixels, np.ndarray) else pixels.contiguous()
         assert not t.is_cuda, "encode_images_host takes host memory; use encode_images for device tensors"
         n = int(t.shape[0])
@@ -868,13 +881,13 @@ class Engine:
                       attention_mask: Optional[torch.Tensor] = None,
                       interpolate_pos_encoding: bool = False) -> torch.Tensor:
         """Residual stream after ``num_layers`` encoder layers (fp32), for layer-wise parity tests.  Vision with
-        ``interpolate_pos_encoding``: any accepted image size, ``[n, S, 768]`` with ``S = vision_seq_len(H, W)``."""
+        ``interpolate_pos_encoding``: any accepted image size, ``[n, S, 768]`` with ``S = self.vision_seq_len(H, W)``."""
         x = self._dev(inputs)
         n = int(x.shape[0])
         if tower == "vision":
-            fmt = _pixel_format(x, interpolate_pos_encoding)
+            fmt = self._pixel_format(x, interpolate_pos_encoding)
             h, w = _pixel_hw(x, fmt)
-            out = torch.empty((n, vision_seq_len(h, w), 768), device=self.device, dtype=torch.float32)
+            out = torch.empty((n, self.vision_seq_len(h, w), 768), device=self.device, dtype=torch.float32)
             with torch.cuda.device(self.device):
                 check(self._L.plip_dbg_hidden_states_hw(self._h, x.data_ptr(), fmt, n, h, w, int(num_layers),
                                                         out.data_ptr(), self._stream()), "plip_dbg_hidden_states_hw")

@@ -17,6 +17,7 @@ from typing import Mapping, Optional, Tuple, Union
 import torch
 
 from .engine import Engine
+from .weights import PATCH_SIZES
 
 
 @dataclass
@@ -64,8 +65,30 @@ def _model_output(o) -> BaseModelOutputWithPooling:
                                       hidden_states=o["hidden_states"], attentions=o["attentions"])
 
 
+def check_config(cfg) -> None:
+    """``ValueError`` unless a ``CLIPConfig`` has a geometry the kernels run: every field they hard-code (common.cuh
+    model constants; TF:configuration_clip.py:47-64,97-109), the vision patch size 32 (ViT-B/32, PLIP's architecture)
+    or 16 (ViT-B/16)."""
+    v, t = cfg.vision_config, cfg.text_config
+    want = {"vision hidden_size": (v.hidden_size, 768),
+            "vision patch_size": (v.patch_size, v.patch_size if v.patch_size in PATCH_SIZES else PATCH_SIZES),
+            "vision image_size": (v.image_size, 224), "vision num_hidden_layers": (v.num_hidden_layers, 12),
+            "vision num_attention_heads": (v.num_attention_heads, 12), "vision intermediate_size": (v.intermediate_size, 3072),
+            "vision hidden_act": (v.hidden_act, "quick_gelu"), "vision layer_norm_eps": (float(v.layer_norm_eps), 1e-5),
+            "text hidden_size": (t.hidden_size, 512), "text num_hidden_layers": (t.num_hidden_layers, 12),
+            "text num_attention_heads": (t.num_attention_heads, 8), "text intermediate_size": (t.intermediate_size, 2048),
+            "text hidden_act": (t.hidden_act, "quick_gelu"), "text layer_norm_eps": (float(t.layer_norm_eps), 1e-5),
+            "text max_position_embeddings": (t.max_position_embeddings, 77), "text vocab_size": (t.vocab_size, 49408),
+            "projection_dim": (cfg.projection_dim, 512)}
+    bad = {k: got for k, (got, exp) in want.items() if got != exp}
+    if bad:
+        raise ValueError("plip_b200 implements the CLIP ViT-B/32 and ViT-B/16 geometries only (PLIP's architecture, "
+                         f"and the same towers behind a 16-pixel patch); this checkpoint differs in {bad}")
+
+
 class PlipCLIPModel:
-    """CUDA-engine-backed stand-in for ``CLIPModel`` (ViT-B/32 geometry only, as PLIP ships)."""
+    """CUDA-engine-backed stand-in for ``CLIPModel``: the CLIP ViT-B/32 geometry PLIP ships, or ViT-B/16 (the same
+    towers behind a 16-pixel patch), as the weights say."""
 
     def __init__(self, state_dict: Mapping[str, torch.Tensor], device: Union[int, str, torch.device, None] = None,
                  max_micro_batch: int = 1024, operand_dtype="bf16"):
@@ -86,30 +109,16 @@ class PlipCLIPModel:
         if tok is not None:
             hf_kwargs.setdefault("token", tok)
         hf = CLIPModel.from_pretrained(name_or_path, **hf_kwargs)
-        cfg = hf.config
-        v, t = cfg.vision_config, cfg.text_config
-        # every field the kernels hard-code (common.cuh model constants; TF:configuration_clip.py:47-64,97-109)
-        want = {"vision hidden_size": (v.hidden_size, 768), "vision patch_size": (v.patch_size, 32),
-                "vision image_size": (v.image_size, 224), "vision num_hidden_layers": (v.num_hidden_layers, 12),
-                "vision num_attention_heads": (v.num_attention_heads, 12), "vision intermediate_size": (v.intermediate_size, 3072),
-                "vision hidden_act": (v.hidden_act, "quick_gelu"), "vision layer_norm_eps": (float(v.layer_norm_eps), 1e-5),
-                "text hidden_size": (t.hidden_size, 512), "text num_hidden_layers": (t.num_hidden_layers, 12),
-                "text num_attention_heads": (t.num_attention_heads, 8), "text intermediate_size": (t.intermediate_size, 2048),
-                "text hidden_act": (t.hidden_act, "quick_gelu"), "text layer_norm_eps": (float(t.layer_norm_eps), 1e-5),
-                "text max_position_embeddings": (t.max_position_embeddings, 77), "text vocab_size": (t.vocab_size, 49408),
-                "projection_dim": (cfg.projection_dim, 512)}
-        bad = {k: got for k, (got, exp) in want.items() if got != exp}
-        if bad:
-            raise ValueError("plip_b200 implements the CLIP ViT-B/32 geometry only (PLIP's architecture); this "
-                             f"checkpoint differs in {bad}")
+        check_config(hf.config)
         m = cls(hf.state_dict(), device=device, max_micro_batch=max_micro_batch, operand_dtype=operand_dtype)
         # legacy configs (eos_token_id == 2) pool at argmax(input_ids) (TF:564-570); same row whenever an eos exists
-        m.engine.set_text_pooling(getattr(t, "eos_token_id", 49407) == 2)
+        m.engine.set_text_pooling(getattr(hf.config.text_config, "eos_token_id", 49407) == 2)
         return m
 
     @classmethod
     def from_openai_state_dict(cls, state_dict, device=None, max_micro_batch: int = 1024, operand_dtype="bf16"):
-        """``clip.load(arch)`` + ``load_state_dict(torch.load(path))`` (``embedders/factory.py:20-27``)."""
+        """``clip.load(arch)`` + ``load_state_dict(torch.load(path))`` (``embedders/factory.py:20-27``).  The patch size
+        (ViT-B/32 or ViT-B/16) is read from ``visual.conv1.weight``, as ``clip.model.build_model`` does."""
         m = cls(state_dict, device=device, max_micro_batch=max_micro_batch, operand_dtype=operand_dtype)
         m.engine.set_text_pooling(True)          # OpenAI clip: x[arange, text.argmax(-1)] (eot has the largest id)
         return m

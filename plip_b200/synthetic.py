@@ -1,4 +1,4 @@
-"""Seeded synthetic CLIP ViT-B/32 weights and inputs (the BASELINE.json configs' data).
+"""Seeded synthetic CLIP ViT-B/32 (and ViT-B/16) weights and inputs (the BASELINE.json configs' data).
 
 No pretrained PLIP checkpoint is reachable offline (``vinid/plip`` needs the network; SURVEY.md §8c), so the
 benchmark, the smoke test and the parity tests all run on seeded random weights with the exact state-dict names /
@@ -82,9 +82,13 @@ def _add_outliers(sd, g, prefix: str, dim: int, layers: int) -> None:
             b[sh] = torch.tensor([2.0, -2.0, 1.0, -1.0])
 
 
-def make_state_dict(seed: int = 0, mode: str = "rich") -> "OrderedDict[str, torch.Tensor]":
-    """fp32 state dict with the HF ``CLIPModel`` key set (``load_state_dict(strict=True)``-able)."""
+def make_state_dict(seed: int = 0, mode: str = "rich", patch: int = 32) -> "OrderedDict[str, torch.Tensor]":
+    """fp32 state dict with the HF ``CLIPModel`` key set (``load_state_dict(strict=True)``-able).  ``patch``: the
+    vision patch size, 32 (ViT-B/32; ``CLIPConfig()``) or 16 (ViT-B/16: ``patch_embedding.weight`` ``[768,3,16,16]``,
+    a ``[197,768]`` position table).  The ViT-B/32 draws are those of the generator before the argument existed."""
     assert mode in ("rich", "hf_init", "outlier")
+    assert patch in (32, 16)
+    vseq = (VISION["image"] // patch) ** 2 + 1
     rich = mode != "hf_init"
     g = torch.Generator(device="cpu").manual_seed(seed)
 
@@ -103,8 +107,8 @@ def make_state_dict(seed: int = 0, mode: str = "rich") -> "OrderedDict[str, torc
     # ---- vision tower (TF:modeling_clip.py:138-218, 647-691)
     vd = VISION["dim"]
     sd["vision_model.embeddings.class_embedding"] = randn(vd, std=vd ** -0.5)
-    sd["vision_model.embeddings.patch_embedding.weight"] = randn(vd, 3, 32, 32, std=0.02)
-    sd["vision_model.embeddings.position_embedding.weight"] = randn(VISION["seq"], vd, std=0.02)
+    sd["vision_model.embeddings.patch_embedding.weight"] = randn(vd, 3, patch, patch, std=0.02)
+    sd["vision_model.embeddings.position_embedding.weight"] = randn(vseq, vd, std=0.02)
     sd["vision_model.pre_layrnorm.weight"] = 1.0 + randn(vd, std=0.1 if rich else 0.0)
     sd["vision_model.pre_layrnorm.bias"] = randn(vd, std=0.05 if rich else 0.0)
     _tower(sd, g, "vision_model", vd, VISION["ff"], VISION["layers"], rich)

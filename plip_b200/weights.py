@@ -13,7 +13,11 @@ as the way weights reach the device.  The blob layout is owned by the CUDA libra
   ``LN(x) W^T + b = rstd (x (gamma o W)^T - mean colsum) + (b + W beta)`` with
   ``colsum[n] = sum_k bf16(gamma o W)[n,k]``; the device keeps ``bf16(gamma o W)``, ``colsum`` and the
   adjusted bias, never the LayerNorm parameters themselves;
-* the conv patch embedding ``[768,3,32,32]`` is viewed as ``[768, 3072]`` (c, ky, kx order).
+* the conv patch embedding ``[768,3,P,P]`` is viewed as ``[768, 3 P^2]`` (c, ky, kx order).
+
+The vision patch size ``P`` is read from the weights, as OpenAI's ``build_model`` reads it from
+``visual.conv1.weight.shape[-1]``: 32 (ViT-B/32, PLIP) or 16 (ViT-B/16).  The two blob layouts differ only in the
+patch embedding and the stored position table (``plip_weights_tensor_info_patch``).
 """
 from __future__ import annotations
 
@@ -80,13 +84,27 @@ def normalize_state_dict(sd: Mapping[str, torch.Tensor]) -> Dict[str, torch.Tens
     raise KeyError("state dict is neither a HuggingFace CLIPModel nor an OpenAI-clip CLIP state dict")
 
 
-def tensor_table():
-    """The library's blob layout as a list of :class:`TensorInfo`."""
+PATCH_SIZES = (32, 16)  # vision patch sizes the engine runs: CLIP ViT-B/32 (PLIP) and ViT-B/16
+
+
+def vision_patch(sd: Mapping[str, torch.Tensor]) -> int:
+    """The vision patch size of a state dict (HF, prefixed HF or OpenAI-clip names): the last dimension of the conv
+    patch embedding.  ``ValueError`` for a size the engine does not run."""
+    w = normalize_state_dict(sd)["vision_model.embeddings.patch_embedding.weight"]
+    patch = int(w.shape[-1])
+    if patch not in PATCH_SIZES:
+        raise ValueError("plip_b200 implements the CLIP ViT-B/32 and ViT-B/16 geometries only; this checkpoint "
+                         f"differs in {{'vision patch_size': {patch}}}")
+    return patch
+
+
+def tensor_table(patch: int = 32):
+    """The library's blob layout for a vision patch size (32 or 16) as a list of :class:`TensorInfo`."""
     L = lib()
     infos = []
     for i in range(L.plip_weights_num_tensors()):
         ti = TensorInfo()
-        check(L.plip_weights_tensor_info(i, C.byref(ti)), "plip_weights_tensor_info")
+        check(L.plip_weights_tensor_info_patch(int(patch), i, C.byref(ti)), "plip_weights_tensor_info_patch")
         infos.append(ti)
     return infos
 
@@ -104,12 +122,14 @@ def operand_format(operand_dtype) -> Tuple[int, torch.dtype]:
 
 
 def pack_state_dict(state_dict: Mapping[str, torch.Tensor], operand_dtype="bf16") -> Tuple[torch.Tensor, float]:
-    """Return ``(blob, exp(logit_scale))``; ``blob`` is a contiguous CPU uint8 tensor.  GEMM weights are rounded
-    once to ``operand_dtype`` (the format the engine is created with: ``plip_create_ex``)."""
+    """Return ``(blob, exp(logit_scale))``; ``blob`` is a contiguous CPU uint8 tensor in the layout of the weights'
+    vision patch size (:func:`vision_patch`).  GEMM weights are rounded once to ``operand_dtype`` (the format the
+    engine is created with: ``plip_create_patch``)."""
     _, odt = operand_format(operand_dtype)
     sd = normalize_state_dict(state_dict)
+    patch = vision_patch(sd)
     L = lib()
-    blob = torch.zeros(int(L.plip_weights_blob_bytes()), dtype=torch.uint8)
+    blob = torch.zeros(int(L.plip_weights_blob_bytes_patch(patch)), dtype=torch.uint8)
     folded = {}  # (base name, "weight"/"bias"/"colsum") -> fp32 tensor, computed once per projection
 
     def fold(base: str, flags: int):
@@ -138,7 +158,7 @@ def pack_state_dict(state_dict: Mapping[str, torch.Tensor], operand_dtype="bf16"
         folded[(base, "bias")] = b
         folded[(base, "colsum")] = w.to(odt).to(torch.float32).sum(dim=1)
 
-    for ti in tensor_table():
+    for ti in tensor_table(patch):
         name = ti.name.decode()
         if ti.fused:
             base, kind = name.rsplit(".", 1)
